@@ -2,24 +2,31 @@
 """bench.py -- continuation steps/sec on 2-D Swift-Hohenberg (SH2d-fronts 1024^2, fp64) + achieved HBM GB/s of the
 fused JVP+Arnoldi kernel, per BASELINE.json.
 
-Workload (BASELINE.json configs[2]: "SH2d-fronts 1024^2, PALC branch of 200 steps sharded 8xB200"): the localized-front branch
+Workload (BASELINE.json configs[2]: "SH2d-fronts 1024^2, PALC branch of 200 steps sharded 8xH100"): the localized-front branch
 of examples/SH2d-fronts.jl from its start point over a fixed WINDOW of PALC arclength S = K * B * dsmax -- the same window for
 every number of GPUs (strong scaling).  A bench "step" = one BATCH of B = 10 continuation steps at dsmax (the unit after
-which the (lambda, ||u||) rows are exchanged, north_star); `value` = K * B / t in continuation steps per second, where a
+which the (lambda, ||u||) rows are exchanged, north_star); `value` = S_taken / t in continuation steps per second, where a
 continuation step = secant predictor + Newton-Krylov corrector (per Newton iteration 2 residuals and one MatrixFreeBLS solve =
 one GMRES(100) with the DCT preconditioner on the right, fused JVP+Arnoldi kernels).  K = 20, B = 10 -> the 200-step branch.
+S_taken = the continuation steps the timed window actually took: K * B, or fewer when the branch ends first (the step size falls
+below dsmin); `details.window_complete` says which, and every rate of the line (`value`, `ms_per_step`, `e2e`, `e2e_native`) is
+computed from the steps actually taken.
 
-N = 1: plain continuation over the window (exactly K * B steps).  N > 1 ("replicas only", SURVEY.md 8(e) / tier rule 5): PALC is a
+N = 1: plain continuation over the window (at most K * B steps).  N > 1 ("replicas only", SURVEY.md 8(e) / tier rule 5): PALC is a
 sequential recurrence, so one branch does not shard; every rank runs an independent replica of the same job (replicated state,
 nothing crosses NVLink), the rows (lambda, ||u||, itnewton, itlinear) are all_gathered per job -- and must agree bit for bit
-across the GPUs, which the JSON reports -- `value` = N * K * B / max-over-ranks time, "scaling": "weak".  (A family of branches
+across the GPUs, which the JSON reports -- `value` = (steps taken over all ranks) / max-over-ranks time, "scaling": "weak".  (A family of branches
 nu_r = nu (1 + 0.002 r) was tried first: at nu_1 the same start-up already lands on a different, 30x cheaper branch, so the
 ranks would not do comparable work.)
 The alternative `--partition scout` cuts ONE branch window into chunks seeded by a cheap scout inside the timed region
-(segments.py); measured on this branch it does not work -- a scout loose enough to be cheap leaves the snaking branch
-(profiles/r02_scout_probe.txt, DESIGN.md section 6) -- so it is kept as an option, not the default.
+(segments.py); on this branch it does not work -- a scout loose enough to be cheap leaves the snaking branch
+(tools/scout_probe.py, DESIGN.md section 6) -- so it is kept as an option, not the default.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--grid 1024] [--batch 10] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--grid 1024] [--batch 10] [--impl reference] [--dump-outputs DIR]
+
+--dump-outputs DIR : after the timed window, writes what it computed as float64 .npy files (rank 0 only): branch.npy (one row
+per continuation step: lambda, ||u||, itnewton, itlinear, ds, step), u_final.npy (the state at the window's last step, 8 MB at
+1024^2; above 7 Mi values a fixed sample of it, the sorted indices drawn by np.random.default_rng(0)) and p_final.npy.  The inputs depend only on the arguments, so two builds can be compared output for output.
 
 Besides `e2e` (the plugin surfaces with host vectors) the line carries `e2e_native`: the same window through ONE C-ABI call from and
 to host buffers (bk_palc_run, the PALC loop as host C++ inside the library), with a check that its rows equal the device-resident
@@ -113,27 +120,6 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of k2_fused<8,1> from the committed `ncu --set full` capture of
-    the shipped kernel (profiles/r02_ncu_k2_fused.csv, falling back to the round-1 capture of k2_fused<7,1>)."""
-    p = os.path.join(ROOT, "profiles", "r02_ncu_k2_fused.csv")
-    if not os.path.exists(p):
-        p = os.path.join(ROOT, "profiles", "r01c_ncu_k2_fused.csv")
-    try:
-        import csv
-        rows = list(csv.reader(open(p)))
-        h = rows[0]
-        vals = [float(r[h.index("dram__bytes_read.sum")]) + float(r[h.index("dram__bytes_write.sum")]) for r in rows[2:]]
-        out = {"bytes_per_launch": 1e6 * sum(vals) / len(vals), "source": os.path.relpath(p, ROOT) + " (k2_fused, one ncu --set full capture)"}
-        if p.endswith("r02_ncu_k2_fused.csv"):
-            # the capture sits at Krylov index j = 14 of a 1024^2 solve: algorithmic 8N(j+2) + 16N = 151 MB; moved in addition: the
-            # right-preconditioned input z (its own vector, +8N) and the stencil halo rows ((E+4)/E on z)
-            out.update(j_at_capture=14, algorithmic_bytes_at_capture=8 * 1024 * 1024 * (14 + 2) + 16 * 1024 * 1024)
-        return out
-    except Exception:
-        return None
-
-
 def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -141,7 +127,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 # ----------------------------------------------------------------------------------------------- GPU arm
@@ -301,7 +287,8 @@ class StepTimer:
         def f(st):
             self.stop()
             keep = cb(st) if cb is not None else True
-            self.start()
+            if keep is not False:  # a stopping callback ends the timed window: no pair is opened for a step that is not taken
+                self.start()
             return keep
         return f
 
@@ -354,13 +341,16 @@ def window_job(bk, ctx, ls, n, u_start, s_total, rank, world, torch, flush, timi
         # point per step, both inside the timed region.
         cp1 = cpf()
         cp1.max_steps = nsteps
-        rows, st, sinfo = S.continuation_speculative(P, mkprob(u_start, PAR[0]), alg, cp1, P.norminf, spec[0], torch, spec[1], callback=tm.wrap(None))
+        rows, st, sinfo = S.continuation_speculative(P, mkprob(u_start, PAR[0]), alg, cp1, P.norminf, spec[0], torch, spec[1],
+                                                   callback=tm.wrap(lambda s: s.step < nsteps))  # stop at step nsteps, as below
         rows = rows[: nsteps + 1]
         info["speculative"] = sinfo
     elif world == 1:
         cp1 = cpf()
         cp1.max_steps = nsteps
-        rows, st = P.continuation(mkprob(u_start, PAR[0]), alg, cp1, normC=P.norminf, callback=tm.wrap(None))
+        # stop at step nsteps: without the callback's stop the loop would correct one more step (st.step <= max_steps) and
+        # time it, although its row is dropped
+        rows, st = P.continuation(mkprob(u_start, PAR[0]), alg, cp1, normC=P.norminf, callback=tm.wrap(lambda s: s.step < nsteps))
         rows = rows[: nsteps + 1]
     else:
         tm.start()  # the scout's two start-up Newton solves are part of the job
@@ -386,16 +376,39 @@ def window_job(bk, ctx, ls, n, u_start, s_total, rank, world, torch, flush, timi
     ctx.set_timing(False)
     s1 = ctx.stats()
     if st is not None:
-        info.update(rejected=int(st.nfail), work_newton=int(st.work_newton), work_linear=int(st.work_linear))
+        info.update(rejected=int(st.nfail), work_newton=int(st.work_newton), work_linear=int(st.work_linear), state=st)
     return rows, ms, {k: s1[k] - s0[k] for k in s1}, info
 
 
 def config_dict(n, workload, K, B):
     """Identical in both arms (driver: same_config); everything run-specific goes under "details"."""
     return {"workload": workload, "grid": [n, n],
-            "window": f"localized-front branch of examples/SH2d-fronts.jl from lambda = -0.1: {K} batches x {B} continuation steps",
+            "window": f"localized-front branch of examples/SH2d-fronts.jl from lambda = -0.1: up to {K} batches x {B} continuation steps "
+                      "(fewer if the branch ends first: details.continuation_steps_taken)",
             "batch": B, "newton_tol": 1e-9, "gmres": GMRES, "bls": BLS["kind"], "continuation": CONT,
             "l2": "GPU arm: 256 MiB L2 flush between continuation steps (outside the event pairs); the Krylov basis of a solve exceeds L2"}
+
+
+DUMP_MAX_VALUES = 7 * 1024 * 1024  # 56 MB of float64: with the rows and p_final the dump stays under 64 MB
+
+
+def dump_outputs(d, rows, st):
+    """The timed window's results as a caller of the continuation receives them: the branch rows and the last step's state."""
+    os.makedirs(d, exist_ok=True)
+    keys = ("param", "x", "itnewton", "itlinear", "ds", "step")
+    np.save(os.path.join(d, "branch.npy"), np.array([[float(r[k]) for k in keys] for r in rows], dtype=np.float64))
+    if st is not None:
+        u = np.ascontiguousarray(st.z_u.numpy() if hasattr(st.z_u, "numpy") else np.asarray(st.z_u), dtype=np.float64)
+        if u.size > DUMP_MAX_VALUES:  # a fixed, seeded sample of the state (reproducible from the seed, so no index file)
+            u = u[np.sort(np.random.default_rng(0).choice(u.size, DUMP_MAX_VALUES, replace=False))]
+        np.save(os.path.join(d, "u_final.npy"), u)
+        np.save(os.path.join(d, "p_final.npy"), np.array([st.z_p], dtype=np.float64))
+
+
+def steps_taken(rows, nsteps, world):
+    """Continuation steps one rank's window took: nsteps, or fewer when its branch ended first.  The scout partition (world > 1)
+    covers an arclength window in chunks, so its count is the window's nsteps."""
+    return min(nsteps, len(rows) - 1) if world == 1 else nsteps
 
 
 def cpp_opts(cb, max_steps, workers):
@@ -421,7 +434,11 @@ def main():
     ap.add_argument("--branch", default="front", choices=["front", "hexagons"])
     ap.add_argument("--partition", default="replicas", choices=["replicas", "scout", "speculative"],
                     help="N > 1: independent replicas (default), one window cut by a scout, or one branch with speculative step sizes (not measured on GPUs yet)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the timed window's branch rows and final state as float64 .npy files into DIR (rank 0)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes what the GPU arm computed; the reference arm has no such outputs")
     n, K, B = args.grid, args.steps, args.batch
     BLS["kind"] = args.bls
     BRANCH["kind"] = args.branch
@@ -490,7 +507,7 @@ def main():
     replicas = world > 1 and args.partition == "replicas"
     ctx, ls, u_front = gpu_setup(bk, n, dev)
     jw = 1 if (replicas or world == 1) else world  # "world" seen by window_job
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=f"cuda:{dev}")  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=f"cuda:{dev}")  # > the 50 MB L2 of an H100
 
     # ---- warm-up: W untimed continuation steps from the start point (kernels, caches, allocator pools)
     if args.warmup > 0:
@@ -507,6 +524,11 @@ def main():
     if dist:
         dist.barrier()
     clocks = sampler.stop()
+    if len(rows) - 1 < K * B and (world == 1 or spec):
+        print(f"bench.py: the branch ended after {len(rows) - 1} of the window's {K * B} continuation steps (step size below dsmin); "
+              f"the rates count the steps taken", file=sys.stderr)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, rows, info.get("state"))
     tt = torch.tensor([my_ms, float(len(rows)), info["scout_ms"], float(info["rejected"]), float(info["work_newton"]), float(info["work_linear"])],
                       dtype=torch.float64, device=f"cuda:{dev}")
     replica_dev = None
@@ -542,17 +564,19 @@ def main():
         ctx.pin_host = False
         bk.palc.V.host_alloc = None
         th = torch.tensor([ms_h, float(d_h["h2d_bytes"]), float(d_h["d2h_bytes"]), float(info_h["work_newton"]), float(info_h["work_linear"]),
-                           float(info_h["rejected"])], dtype=torch.float64, device=f"cuda:{dev}")
+                           float(info_h["rejected"]), float(steps_taken(rows_h, K * B, jw))], dtype=torch.float64, device=f"cuda:{dev}")
         if dist:
             allh = [torch.zeros_like(th) for _ in range(world)]
             dist.all_gather(allh, th)
             tmax_h = max(float(t[0]) for t in allh)
             h2d, d2h = sum(float(t[1]) for t in allh), sum(float(t[2]) for t in allh)
             wh = [int(sum(float(t[k]) for t in allh)) for k in (3, 4, 5)]
+            steps_h = int(sum(float(t[6]) for t in allh)) if replicas else int(float(allh[0][6]))
         else:
             tmax_h, h2d, d2h = ms_h, float(d_h["h2d_bytes"]), float(d_h["d2h_bytes"])
             wh = [info_h["work_newton"], info_h["work_linear"], info_h["rejected"]]
-        e2e = {"value": (world if replicas else 1) * K * B / (tmax_h * 1e-3), "unit": "steps/s", "h2d_bytes_per_step": int(h2d / K), "d2h_bytes_per_step": int(d2h / K),
+            steps_h = steps_taken(rows_h, K * B, jw)
+        e2e = {"value": steps_h / (tmax_h * 1e-3), "unit": "steps/s", "continuation_steps_taken": steps_h, "h2d_bytes_per_step": int(h2d / K), "d2h_bytes_per_step": int(d2h / K),
                "corrector_work": {"newton_its": int(wh[0]), "linear_its": int(wh[1]), "rejected_steps": int(wh[2])},
                "note": "step acceptance in the snaking region is sensitive to rounding: the host-vector path (BLAS reductions) rejects a different set of steps than the device path, so its corrector work -- and its steps/s -- differ from run to run by up to 1.5x; the same window with pinned host NumPy state vectors: every residual / Jacobian / bordered solve crosses the C ABI with host pointers (H2D + D2H inside the timed region); bytes are per bench step (batch), all ranks"}
     if rank != 0:
@@ -577,7 +601,8 @@ def main():
             st_n = torch.cuda.ExternalStream(ctx.lib.bk_stream(ctx.handle))
             ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             ev0.record(st_n)
-            rows_n, info_n = Pn.continuation_native(prob_n, alg_n, cpn, normC=Pn.norminf)
+            # stop at step K * B, as the timed window does (bk_palc_run corrects while step <= max_steps)
+            rows_n, info_n = Pn.continuation_native(prob_n, alg_n, cpn, normC=Pn.norminf, callback=lambda step, row, z_u, z_p: step < K * B)
             info_n["u"].numpy()  # the final state back on the host, inside the timed region
             ev1.record(st_n)
             ctx.sync()
@@ -586,7 +611,7 @@ def main():
             rows_n = rows_n[: K * B + 1]
             same = len(rows_n) == len(rows) and all(a["param"] == b["param"] and a["x"] == b["x"] and a["itlinear"] == b["itlinear"]
                                                     for a, b in zip(rows_n, rows))
-            e2e_native = {"value": (world if replicas else 1) * K * B / (ms_n * 1e-3), "unit": "steps/s",
+            e2e_native = {"value": (len(rows_n) - 1) / (ms_n * 1e-3), "unit": "steps/s", "continuation_steps_taken": len(rows_n) - 1,
                           "h2d_bytes_per_step": int((sn1["h2d_bytes"] - sn0["h2d_bytes"]) / K), "d2h_bytes_per_step": int((sn1["d2h_bytes"] - sn0["d2h_bytes"] + 8 * 6 * len(rows_n)) / K),  # final state (counted by the library) + the rows
                           "abi_calls": 1, "rows_identical_to_the_device_resident_run": bool(same),
                           "corrector_work": {"newton_its": int(info_n["work_newton"]), "linear_its": int(info_n["work_linear"]), "rejected_steps": int(info_n["nfail"])},
@@ -597,7 +622,11 @@ def main():
         except Exception as exc:  # an extra measurement: it must never cost the line
             e2e_native = {"error": repr(exc)}
 
-    value = (world if replicas else 1) * K * B / (tmax * 1e-3)
+    if replicas:
+        taken = sum(p["steps"] - 1 for p in per_rank)  # per_rank steps = rows per rank, start point included
+    else:
+        taken = steps_taken(rows, K * B, 1 if spec else jw)
+    value = taken / (tmax * 1e-3)
     nst = len(branch)
     peak, peak_src = measured_peak()
     fused_ms, fused_b, fused_l = delta.get("total_fused_ms", 0.0), delta.get("total_fused_bytes", 0), delta.get("total_fused_launches", 0)
@@ -605,7 +634,7 @@ def main():
     pc_ms, pc_n = delta.get("total_precond_ms", 0.0), delta.get("total_precond_applies", 0)
     roofline = {"bound": "hbm", "kernel": "k2_fused<E,bordered> + k2_update<E> (fused JVP+Arnoldi step = 2 launches per Krylov iteration; TMA ring)",
                 "achieved": ach, "peak": peak, "unit": "GB/s", "frac": (ach / peak) if ach else None, "peak_source": peak_src,
-                "traffic": ncu_traffic(), "launches": int(fused_l), "avg_launch_us": (fused_ms * 1e3 / fused_l) if fused_l else None,
+                "launches": int(fused_l), "avg_launch_us": (fused_ms * 1e3 / fused_l) if fused_l else None,
                 "algorithmic_bytes_per_launch": (fused_b / fused_l) if fused_l else None,
                 "share_of_step": (TIMING_EVERY * fused_ms / my_ms) if my_ms else None,
                 "sampling": f"CUDA-event pairs around both kernels of every {TIMING_EVERY}th GMRES solve of the timed region",
@@ -613,11 +642,11 @@ def main():
                                    "algorithmic_bytes_per_apply": 3 * 16 * n * n}}
 
     out = {"metric": metric, "value": value, "unit": "steps/s", "n_gpus": world, "steps": K, "warmup": args.warmup,
-           "ms_per_step": tmax / max(1, K), "higher_is_better": True, "scaling": "weak" if (replicas or world == 1) else "strong", "vs_baseline": None,
+           "ms_per_step": tmax * B * (world if replicas else 1) / max(1, taken), "higher_is_better": True, "scaling": "weak" if (replicas or world == 1) else "strong", "vs_baseline": None,
            "dtype": "f64", "data": "synthetic",
            "config": config_dict(n, workload, K, B),
            "details": dict({
-               "continuation_steps_taken": int(nst - (world if replicas else (1 if world == 1 else 0))), "mean_itnewton": float(np.mean(branch[1:, 2])) if nst > 1 else 0.0,
+               "continuation_steps_taken": int(taken), "window_complete": bool(taken >= (world if replicas else 1) * K * B), "mean_itnewton": float(np.mean(branch[1:, 2])) if nst > 1 else 0.0,
                "mean_itlinear_per_step": float(np.mean(branch[1:, 3])) if nst > 1 else 0.0,
                "corrector_work": {"newton_its": int(wn), "linear_its": int(wl)}, "rejected_steps": int(sum(p["rejected"] for p in per_rank)) if per_rank else int(info["rejected"]),
                "parallelism": ("1 GPU" if world == 1 else
@@ -636,8 +665,10 @@ def main():
     try:
         sm = info.get("step_ms")
         nref = max(1, min(K, args.ref_batches)) * B
-        if sm and len(sm) >= nref:
-            out["details"]["per_batch_ms"] = [round(float(sum(sm[i * B:(i + 1) * B])), 1) for i in range(K)]
+        done = min(len(sm), len(rows) - 1) if sm else 0  # pairs of steps taken; a trailing pair holds only the attempts that failed
+        if sm:
+            out["details"]["per_batch_ms"] = [round(float(sum(sm[i * B:(i + 1) * B])), 1) for i in range(done // B)]  # batches that ran
+        if sm and done >= nref:
             out["details"]["on_reference_sample"] = {
                 "steps": nref, "steps_per_s": (world if replicas else 1) * nref / (sum(sm[:nref]) * 1e-3),
                 "note": f"this rank's device time over the first {nref} continuation steps of the window = the sample bench.py --impl reference times"}

@@ -1,4 +1,4 @@
-"""bk200: B200-native Newton-Krylov corrector for BifurcationKit-style pseudo-arclength
+"""bk200: H100-native Newton-Krylov corrector for BifurcationKit-style pseudo-arclength
 continuation.  The directory name carries a dot (bifurcationkit.jl_b200), so import it through
 ``__graft_entry__.load_package()`` (registers it as the module ``bk200``).
 

@@ -1,5 +1,5 @@
 // bk_async.cuh -- PTX wrappers for the asynchronous copy engine (TMA bulk copies, SASS UBLKCP) and mbarriers, shared by the
-// Krylov kernels (bk_krylov_tma.cuh) and the transform kernels (bk_fft_fast.cuh).  sm_100a.
+// Krylov kernels (bk_krylov_tma.cuh) and the transform kernels (bk_fft_fast.cuh).  sm_90a.
 #pragma once
 #include "bk_common.cuh"
 

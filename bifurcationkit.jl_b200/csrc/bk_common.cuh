@@ -1,5 +1,5 @@
 // bk_common.cuh -- context, operator descriptor and small device helpers shared by the
-// libbk200 translation units.  sm_100a only.
+// libbk200 translation units.  sm_90a only.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -16,7 +16,7 @@ struct BkRange {  // RAII range
 };
 
 #define BK_MAX_PAR 8
-#define BK_NSM_FALLBACK 148
+#define BK_NSM_FALLBACK 132
 
 // Operator descriptor, passed BY VALUE to kernels.  Describes  out = a0*in + a1*J(u)*in  for the
 // named PDE stencils, optionally bordered (MatrixFreeBLSmap, src/LinearBorderSolver.jl:299-335).

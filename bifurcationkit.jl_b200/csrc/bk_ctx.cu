@@ -108,6 +108,10 @@ extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dim
   cudaDeviceProp prop;
   BK_CUDA(c, cudaGetDeviceProperties(&prop, device));
   c->nsm = prop.multiProcessorCount;
+  if (const char* e = getenv("BK_NSM")) {  // diagnostics: size grids and reductions as for a device with BK_NSM SMs
+    const int v = atoi(e);
+    if (v >= 1 && v <= 1024) c->nsm = v;
+  }
   BK_CUDA(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   size_t ld = (size_t)c->ld, m = (size_t)c->m;
   BK_CUDA(c, cudaMalloc(&c->u_state, 8 * ld));

@@ -2,8 +2,7 @@
 //
 // The preconditioner of the Swift-Hohenberg examples, (L1 + shift I)^-1 with L1 = (I + Lap_Neumann)^2
 // (examples/SH2d-fronts.jl:120-122, examples/SH3d.jl:88), is diagonal in the DCT-II basis (bk_precond.cu).  The second
-// generation (round 1: radix-4 passes IN shared memory) was instruction-bound: 6-12 M warp instructions per 2^20 points
-// and kernel, 0.10-0.17 of the HBM bound (profiles/r01c_ncu_k_dct2.csv).  This version keeps the data in registers:
+// generation (radix-4 passes IN shared memory) was instruction-bound.  This version keeps the data in registers:
 //
 //  * TWO real lines form ONE complex line z = v1 + i v2 after Makhoul's reordering (v[m] = x[2m], v[n-1-m] = x[2m+1]).  In
 //    the strided directions the two lines are neighbouring columns, so z is simply a 16-byte load.  One length-n complex FFT
@@ -184,7 +183,7 @@ struct Tables {  // global memory (built on the host by build_tables)
   const double2* lam2;  // lam2[reg * T + tau] = (lambda[k], lambda[(n-k) % n])
 };
 // Every table entry is read exactly once per line pair, by one thread: straight from global memory each read is an exposed L2
-// round trip (ncu, first version: long-scoreboard stalls 4.4 per issue at 3.5 warps per SM, 37 us for the fused kernel).  The
+// round trip, and with few warps per SM nothing hides it.  The
 // CTA therefore pulls its tables into shared memory with three bulk copies issued BEFORE griddepcontrol.wait -- the tables are
 // constants, so the copies overlap the tail of the previous kernel -- and waits on the mbarrier just before the first use.
 template <class C, bool FUSED>
@@ -470,8 +469,8 @@ static __global__ void BKF_BOUNDS(C) k_strided(const double* __restrict__ in, do
 // written straight from / to global memory (8-byte accesses at a 16-byte stride: the other half of every sector belongs to the
 // mirror register of another thread of the same CTA, L1 / L2 merge them); the frequency side goes through a NATURAL-order
 // shared-memory array with its own conflict-free padding, so that global accesses in k are fully coalesced.  (The first
-// version staged whole rows in natural order and scattered into them by digit-reversed k: 54-71 % of its shared-memory
-// wavefronts were bank conflicts, profiles/r02_ncu_fft.csv.)
+// version staged whole rows in natural order and scattered into them by digit-reversed k: most of its shared-memory
+// wavefronts were bank conflicts.)
 template <class C>
 __device__ __forceinline__ int nslot(int k, int pr) { return C::padn(k) * C::PP + pr; }
 

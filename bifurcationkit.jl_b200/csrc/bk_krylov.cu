@@ -239,9 +239,8 @@ static inline size_t bk2_budget() { return (size_t)(233472 / BK2_BLOCKS_PER_SM) 
 static Plan2 plan2(bk_ctx* c, long long units_of_256, size_t scratch_bytes_per_E(int), int force_E = 0) {
   Plan2 p;
   const long long slots = (long long)c->nsm * BK2_BLOCKS_PER_SM;
-  // Tile height: a taller tile amortises the per-vector cost of a CTA (barrier wait + warp reduction), measured
-  // +8% at 512^2 (E 2 -> 4) and +2% at 1024^2 (E 7 -> 8).  Single wave: the tallest tile that still gives every SM
-  // about two CTAs.  Several waves: the height in 5..8 that fills the waves most evenly.
+  // Tile height: a taller tile amortises the per-vector cost of a CTA (barrier wait + warp reduction).  Single wave: the
+  // tallest tile that still gives every SM about two CTAs.  Several waves: the height in 5..8 that fills the waves most evenly.
   long long E = BK2_EMAX;
   while (E > 1 && (units_of_256 + E - 1) / E < (17 * (long long)c->nsm) / 10) --E;
   if ((units_of_256 + E - 1) / E > slots) {
@@ -324,8 +323,8 @@ static int launch_fused2(bk_ctx* c, const OpDesc& op, const double* in, const do
 static inline int chunk_grid(long long n) { return (int)((n + BK_TILE - 1) / BK_TILE); }
 
 // fused_mode: bk_gmres_opts.fused -- 0 never, 1 automatic (the measured-fastest arrangement), 2 wherever a fused kernel exists.
-// 3-D: the fused kernel is still the first-generation one (64 KB tiles, 2.3 waves at 128^3) and measured 17% slower per
-// iteration than stand-alone JVP + TMA-ring dots, so "automatic" keeps it off until a TMA-ring 3-D kernel exists.
+// 3-D: the fused kernel is still the first-generation one (64 KB tiles, more than two waves at 128^3), slower per iteration
+// than stand-alone JVP + TMA-ring dots, so "automatic" keeps it off until a TMA-ring 3-D kernel exists.
 static bool fused_available(const OpDesc& op, int fused_mode = 2) {
   if (op.cplx) return false;  // the fused kernels tile one real grid; a split complex vector takes the two-launch path
   if (op.bordered > 1) return false;  // block borders: stencil + k_tail2

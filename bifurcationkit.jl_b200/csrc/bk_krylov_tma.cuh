@@ -2,8 +2,8 @@
 // shared-memory ring by the TMA engine (cp.async.bulk + mbarrier), issued by a dedicated producer
 // warp, while 8 consumer warps do the fp64 FMAs.  One CTA owns a tile of up to 8 rows x 256 columns
 // (fused 2-D stencil) or a contiguous segment of up to 8 x 256 values (generic vectors); the tile
-// height E is chosen on the host so that the grid fills every SM of the B200 in whole, balanced waves
-// (the first version ran 512 CTAs on 444 resident slots: 1.15 waves, 24% of DRAM peak in ncu).
+// height E is chosen on the host so that the grid fills every SM of the device in whole, balanced waves
+// (a grid of 1.15 waves leaves most SMs idle during its last wave).
 //
 //   pass 1  k2_fused<E>  : w = a0 v + a1 J(u) v on a 256 x E tile (stencil from shared memory, halo 2),
 //                          then h_i = <v_i, w>, i < j, with V_i tiles arriving through the ring.
@@ -46,8 +46,8 @@ __device__ __forceinline__ void ring_init(Ring* rg, int NS) {
 // Streams V_0..V_{j-1} restricted to the tile through the ring.  MODE 0: sred[i*8 + warp] = warp partial of
 // <V_i, val>; MODE 1: val -= g_i V_i.  Called by all BK2_THREADS threads after a __syncthreads().
 // REV: the basis is traversed from V_{j-1} down to V_0.  Pass 1 (dots) runs forward and pass 2 (update) backward, so each
-// pass starts with the vectors the previous pass touched last, which are still in the 126 MB L2 (with both passes forward
-// the LRU order evicts exactly what is needed next: 11 % hit rate in profiles/r01c_ncu_k2_fused.csv).
+// pass starts with the vectors the previous pass touched last, which may still be in the L2 (50 MB on an H100: the last few
+// 8 MB basis vectors at 1024^2); with both passes forward the LRU order evicts exactly what is needed next.
 template <int E, int MODE, bool REV = false>
 __device__ __forceinline__ void stream_basis(const Tile2& tl, const double* __restrict__ V, long long ld, int j, double* ring,
                                              int NS, Ring* rg, double (&val)[E], double* sred,
@@ -253,7 +253,7 @@ __device__ __forceinline__ void sh2_tile_eval(const OpDesc& op, const double* __
   const bool colok = t < BK2_ROW && gx < nx;
   const int rows = min(E, ny - y0);
   // Epilogue in sub-passes so that each issues E independent global loads before the first use (the first version mixed the
-  // loads of u, a, b with the arithmetic row by row: long-scoreboard stalls 11.7 per issue at 54 registers, ncu round 2).
+  // loads of u, a, b with the arithmetic row by row and stalled on each of them).
   double g[E];
   if (!RESID) {
 #pragma unroll

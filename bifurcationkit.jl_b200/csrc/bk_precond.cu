@@ -142,11 +142,9 @@ static int upload(bk_ctx* c, void** dst, const void* src, size_t bytes) {
 }
 
 // ---- fast path: one instantiation per (values per thread, line length) -----------------------------------------------------
-// Values per thread E = 2^loge of the fast kernels for a line of length n.  Measured on B200: warm, isolated per-kernel times
-// (profiles/r02_fft_warm_times.txt) favour E = 32 at n = 1024 (38.9 us per application against 44-48 us for E = 4 / 8 / 16), but
-// inside the GMRES loop E = 8 wins (46.6 us per application against 52.7 us for E = 32, bench.py `roofline.preconditioner`):
-// more warps per SM hide the latencies that the neighbouring kernels' PDL overlap does not.  n <= 512: E = 4 (18.9 us against
-// 32 us for E = 32, too few warps per SM).  BK_FFT_LOGE overrides (2..5).
+// Values per thread E = 2^loge of the fast kernels for a line of length n: E = 8 for n >= 1024, E = 4 below, chosen for the
+// GMRES loop, where more warps per SM hide the latencies that the neighbouring kernels' PDL overlap does not (an isolated
+// kernel can favour a larger E).  BK_FFT_LOGE overrides (2..5).
 static int fast_loge(long long n) {
   static int e = -1;
   if (e < 0) {

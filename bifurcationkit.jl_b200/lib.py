@@ -64,7 +64,7 @@ class BK200Error(RuntimeError):
 
 
 def build(verbose=False):
-    """Compile libbk200.so for sm_100a with nvcc (works without a GPU)."""
+    """Compile libbk200.so for sm_90a with nvcc (works without a GPU)."""
     r = subprocess.run(["make", "-C", CSRC, "-j8"], capture_output=True, text=True)
     if r.returncode != 0:
         raise BK200Error("nvcc build of libbk200.so failed:\n" + r.stdout[-4000:] + r.stderr[-4000:])

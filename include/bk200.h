@@ -1,4 +1,4 @@
-/* bk200.h -- C ABI of libbk200.so: the B200-native Newton-Krylov corrector hot path of
+/* bk200.h -- C ABI of libbk200.so: the H100-native Newton-Krylov corrector hot path of
  * BifurcationKit.jl's pseudo-arclength continuation (PALC).
  *
  * Every entry point replaces the arithmetic behind one reference plugin surface; the citation
@@ -231,7 +231,9 @@ int32_t bk_palc_run(bk_ctx* ctx, const bk_palc_opts* opts, const bk_gmres_opts* 
  *   BK_NO_PDL=1         launch without programmatic dependent launch (plain stream order)
  *   BK_FFT_LOGE=2..5    complex values per thread (2^e) of the power-of-two transform kernels instead of the per-size default
  *   BK_FFT_NO_FAST=1    every transform through the general mixed-radix kernel (bk_fft_gen.cuh)
- *   BK_SH2D_NO_TMA=1    stand-alone SH2d residual / JVP on the first-generation 64 x 32 tile kernel instead of the TMA-staged tile */
+ *   BK_SH2D_NO_TMA=1    stand-alone SH2d residual / JVP on the first-generation 64 x 32 tile kernel instead of the TMA-staged tile
+ *   BK_NSM=1..1024      size grids and reductions (read at bk_ctx_create) as for a device with that many SMs: changes the summation
+ *                       order of every reduction, so it shows how a result depends on it */
 
 #ifdef __cplusplus
 }

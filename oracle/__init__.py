@@ -16,5 +16,5 @@ test/newton/test_newton.jl, test/periodic_orbits_function_fd/test_potrap.jl);
 GMRES *iterates* and iteration counts are "parity unpinned" (the reference's
 own tests only pin solutions against dense solves).
 
-All citations ``file:line`` are relative to /root/reference.
+All citations ``file:line`` are relative to the root of the BifurcationKit.jl source tree.
 """

@@ -1,5 +1,5 @@
 """bench.py's reference arm runs on the host cores alone (oracle/c, C++/OpenMP): its JSON line is checked here against the
-driver's contract on a small grid (the GPU arm prints the same keys; it needs a B200)."""
+driver's contract on a small grid (the GPU arm prints the same keys; it needs an H100)."""
 import json
 import os
 import subprocess
@@ -34,3 +34,31 @@ def test_reference_arm_other_ranks_exit_without_work():
     r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--gpus", "2", "--grid", "256"],
                        capture_output=True, text=True, timeout=120, cwd=ROOT, env=env)
     assert r.returncode == 0 and r.stdout.strip() == ""
+
+
+def test_dump_outputs_layout_and_size_cap(tmp_path, monkeypatch):
+    """--dump-outputs: one float64 row per continuation step (param, x, itnewton, itlinear, ds, step), the final state -- a
+    seeded sample of it above DUMP_MAX_VALUES -- and the final parameter; the whole dump stays under 64 MB."""
+    import types
+    import numpy as np
+    import bench
+    assert bench.DUMP_MAX_VALUES * 8 + 1024 * 1024 <= 64 * 1024 * 1024
+    rows = [dict(param=-0.1 - 1e-3 * k, x=2.0 + k, itnewton=k % 3, itlinear=10 * k, ds=-1e-3, step=k, n_unstable=-1) for k in range(5)]
+    st = types.SimpleNamespace(z_u=np.linspace(0.0, 1.0, 1000), z_p=-0.104)
+    bench.dump_outputs(str(tmp_path / "full"), rows, st)
+    br = np.load(tmp_path / "full" / "branch.npy")
+    assert br.dtype == np.float64 and br.shape == (5, 6) and br[3].tolist() == [rows[3][k] for k in ("param", "x", "itnewton", "itlinear", "ds", "step")]
+    assert np.array_equal(np.load(tmp_path / "full" / "u_final.npy"), st.z_u)
+    assert np.load(tmp_path / "full" / "p_final.npy").tolist() == [-0.104]
+    monkeypatch.setattr(bench, "DUMP_MAX_VALUES", 100)
+    for d in ("s1", "s2"):
+        bench.dump_outputs(str(tmp_path / d), rows, st)
+    u1, u2 = np.load(tmp_path / "s1" / "u_final.npy"), np.load(tmp_path / "s2" / "u_final.npy")
+    assert u1.dtype == np.float64 and u1.shape == (100,) and np.array_equal(u1, u2) and np.all(np.diff(u1) > 0)
+    assert sorted(os.listdir(tmp_path / "s1")) == ["branch.npy", "p_final.npy", "u_final.npy"]
+
+
+def test_reference_arm_refuses_dump_outputs(tmp_path):
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--dump-outputs", str(tmp_path)],
+                       capture_output=True, text=True, timeout=60, cwd=ROOT)
+    assert r.returncode == 2 and "--dump-outputs" in r.stderr and os.listdir(tmp_path) == []

@@ -1,4 +1,4 @@
-"""To run on a B200 next round, then promote to a GPU test: deflation.py with device vectors.  Same case as
+"""GPU check, a candidate for a GPU test: deflation.py with device vectors.  Same case as
 tests/test_host_logic_cpu.py::test_deflated_newton_finds_the_three_chan_solutions (Chan problem, alpha = 3.3, three solutions
 with max u = 0.77197, 5.97988, 12.85103), linear solves = GMRESB200 with Pl = lu(P) (examples/chan.jl:108-111), two-rhs call."""
 import os, sys

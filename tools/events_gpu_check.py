@@ -1,4 +1,4 @@
-"""To run on a B200 next round, then promote to tests/test_gpu_palc.py: events.py (detect_bifurcation = 3) with device vectors.
+"""GPU check, a candidate for tests/test_gpu_palc.py: events.py (detect_bifurcation = 3) with device vectors.
 cGL2d trivial branch u = 0 continued in r: eigenvalues r + lambda_k(Lap) +- i nu, so the first Hopf point is analytic,
 r_hopf = -lambda_1 (examples/cGL2d.jl:120-135 finds it at r ~ 1.14 on 41 x 21).  Expected: one special point of type hopf,
 delta = (2, 2), |param - r_hopf| below the bisection interval."""

@@ -1,5 +1,5 @@
 // Stand-alone check of k2_dots<E> / k2_update<E> against naive kernels: which tiles / elements differ?
-// build: nvcc -O3 -std=c++17 -lineinfo -gencode arch=compute_100a,code=sm_100a -I../../bifurcationkit.jl_b200/csrc k2_check.cu -o k2_check
+// build: nvcc -O3 -std=c++17 -lineinfo -gencode arch=compute_90a,code=sm_90a -I../../bifurcationkit.jl_b200/csrc k2_check.cu -o k2_check
 #include <cstdio>
 #include <cstdlib>
 #include <cmath>

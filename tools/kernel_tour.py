@@ -1,5 +1,5 @@
-"""Launches every stand-alone kernel of the path once or twice at BASELINE.json's config sizes, for one `ncu --set full` row per kernel
-(profiles/r02_ncu_kernels_tour.csv): K1/K2 stencils of the four problems, BLAS-1 / reductions, the general transform kernel."""
+"""Launches every stand-alone kernel of the path once or twice at BASELINE.json's config sizes, for one `ncu --set full` row per kernel:
+K1/K2 stencils of the four problems, BLAS-1 / reductions, the general transform kernel."""
 import os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

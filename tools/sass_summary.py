@@ -1,6 +1,6 @@
-"""SASS evidence per kernel of libbk200.so (cuobjdump -sass): instruction count and the mnemonics that prove the Blackwell-native
+"""SASS evidence per kernel of libbk200.so (cuobjdump -sass): instruction count and the mnemonics that prove the Hopper-native
 paths (UBLKCP = cp.async.bulk / TMA bulk copy, SYNCS = mbarrier, FENCE.VIEW.ASYNC = fence.proxy.async, DFMA/DADD/DMUL = fp64 pipe,
-LDS/STS = shared memory, LDG/STG = global, ACQBULK / griddepcontrol = PDL).   python tools/sass_summary.py > profiles/sass_r02.txt"""
+LDS/STS = shared memory, LDG/STG = global, ACQBULK / griddepcontrol = PDL).   python tools/sass_summary.py   (prints the table)"""
 import collections, os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 so = os.path.join(ROOT, "bifurcationkit.jl_b200", "libbk200.so")
@@ -22,7 +22,7 @@ for l in out.splitlines():
         if "ACQBULK" in op or "PREEXIT" in op or op.startswith("ACQ"):
             cnt[cur]["PDL"] += 1
 KEYS = ["UBLKCP", "UBLKPF", "SYNCS", "FENCE.VIEW.ASYNC", "DFMA", "DADD", "DMUL", "MUFU", "LDS", "STS", "LDG", "STG", "BAR", "LDL", "STL"]
-print(f"# {os.path.relpath(so, ROOT)}: SASS mnemonic counts per kernel (sm_100a), from `cuobjdump -sass`")
+print(f"# {os.path.relpath(so, ROOT)}: SASS mnemonic counts per kernel (sm_90a), from `cuobjdump -sass`")
 print(f"{'instr':>7} " + " ".join(f"{k[:9]:>9}" for k in KEYS) + "  kernel")
 tot = collections.Counter()
 for k, c in sorted(cnt.items(), key=lambda kv: -sum(kv[1].values())):
