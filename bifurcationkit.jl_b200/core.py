@@ -267,7 +267,7 @@ class ComplexJacobian:
 
 
 def make_opts(reltol=1e-8, abstol=0.0, restart=200, maxiter=100, pc_side=_l.BK_SIDE_NONE, orth=_l.BK_ORTH_CGS, fused=True):
-    return _l.GmresOpts(reltol, abstol, restart, maxiter, pc_side, orth, int(fused), 0)  # fused: 0 off, 1 auto, 2 force
+    return _l.GmresOpts(reltol, abstol, restart, maxiter, pc_side, orth, int(fused), 0)  # fused: 0 off, nonzero where a fused kernel exists
 
 
 class GMRESB200:

@@ -7,7 +7,6 @@
 #include <mutex>
 #include <new>
 #include "bk_common.cuh"
-#include "bk_stencil.cuh"
 
 int bk_fail(bk_ctx* c, int code, const char* what, const char* file, int line) {
   if (c) {
@@ -137,11 +136,6 @@ extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dim
     // the fused 2-D kernel tiles rows, not the flat vector: a narrow grid (nx << 256) has up to ceil(nx/256) * ny CTAs
     long long gf = ((c->dims[0] + 255) / 256) * c->dims[1] + 8;
     if (gf > g) g = gf;
-  }
-  if (kind == BK_SH2D || kind == BK_SH3D) {  // first-generation tile kernels (64x32 / 32x8x8 tiles, ragged grids)
-    long long gt = kind == BK_SH2D ? sh_num_tiles<2>((int)c->dims[0], (int)c->dims[1], 1)
-                                   : sh_num_tiles<3>((int)c->dims[0], (int)c->dims[1], (int)c->dims[2]);
-    if (gt + 8 > g) g = gt + 8;
   }
   if (g < 4 * c->nsm) g = 4 * c->nsm;
   c->gmax = (int)g;

@@ -8,7 +8,7 @@
 //   eigenvalues theta of (J - sigma)^-1 of largest magnitude, lambda = sigma + 1/theta, sorted by
 //   decreasing real part (src/EigSolver.jl:16-19).
 // Outer iteration: explicitly restarted Arnoldi with two classical Gram-Schmidt passes (CGS2) on the
-// device (same k_dots / k_update_norm kernels as GMRES); the small Hessenberg eigenproblem is solved
+// device (same k2_dots / k2_update kernels as GMRES); the small Hessenberg eigenproblem is solved
 // on the host (complex shifted QR + inverse iteration), like the Givens rotations of GMRES.
 #include <algorithm>
 #include <cmath>

@@ -4,14 +4,19 @@
 // (src/LinearSolver.jl:186-206): left/right preconditioning, tolerance max(reltol*||Pl\r0||, abstol)
 // on the preconditioned residual, `iters` = total inner iterations capped by maxiter, x updated at
 // restart and at the end.  Orthogonalisation is single-pass classical Gram-Schmidt in two sweeps
-// over the basis (the reference's backend uses modified GS => tolerance parity, not bit parity):
+// over the basis (the reference's backend uses modified GS => tolerance parity, not bit parity).
+// The basis streams through a TMA ring in every sweep (bk_krylov_tma.cuh):
 //
-//   pass 1  k_fused_jvp_dots : w = a0 v_j + a1 J(u) v_j evaluated as the PDE stencil from a shared-memory
-//                              tile (bk_stencil.cuh) and, in the same kernel, h_i = <v_i, w> for i <= j
-//                              (warp-shuffle reduction -> per-CTA partials -> deterministic last-block sum).
-//                              Algorithmic traffic 8N(j+2) bytes: read u, V_1..V_j, write w.
-//   pass 2  k_update_norm    : v'_{j+1} = w - sum_i h_i v_i, ||v'_{j+1}||^2 reduced the same way.
-//                              Algorithmic traffic 8N(j+2): read w, V_1..V_j, write v'_{j+1}.
+//   pass 1  k2_fused<E,B>     : w = a0 v_j + a1 J(u) v_j evaluated as the SH2d stencil from a TMA-staged tile
+//                               and, in the same kernel, h_i = <v_i, w> for i <= j (per-CTA partials ->
+//                               deterministic last-block sum).  Algorithmic traffic 8N(j+2) bytes: read u,
+//                               V_1..V_j, write w.  Only real SH2d with an even nx, at most one border and no
+//                               left preconditioner (fuses_jvp); every other operator runs its stand-alone
+//                               apply and then
+//           k2_dots<E>        : h_i = <v_i, w> over w already in memory, 8N(j+1).
+//   pass 2  k2_update<E>      : v'_{j+1} = w - sum_i h_i v_i, ||v'_{j+1}||^2 reduced the same way.
+//                               Algorithmic traffic 8N(j+2): read w, V_1..V_j, write v'_{j+1}.
+//   k_lincomb                 : x = beta x + sum_i y_i s_i v'_i at restart and at the end.
 //
 // The basis is stored UN-normalised (v'_i) with the scalars s_i = 1/||v'_i|| kept on device, so
 // normalisation costs no memory pass ("deferred as a scalar") and the host never has to be in the
@@ -23,181 +28,6 @@
 #include "bk_common.cuh"
 #include "bk_stencil.cuh"
 #include "bk_krylov_tma.cuh"
-
-#define BK_DOT_UNROLL 4
-
-// ---- shared device code: dots of the thread-owned points against V_0..V_{j-1} + grid reduction ------
-// val/off: the EPT points this thread owns (off < 0 never occurs here: callers pass clamped offsets and
-// val = 0 for padding).  sred: shared scratch of >= 8*j doubles.
-__device__ __forceinline__ void bk_dots_reduce(const double (&val)[BK_EPT], const int (&off)[BK_EPT],
-                                               const double* __restrict__ V, long long ld, int j,
-                                               const double* __restrict__ scales, double* sred,
-                                               double* __restrict__ partials, unsigned int* counter,
-                                               double* __restrict__ hcol, double* __restrict__ gcoef, int* s_flag) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  for (int i0 = 0; i0 < j; i0 += BK_DOT_UNROLL) {
-    double acc[BK_DOT_UNROLL];
-    double ld_v[BK_DOT_UNROLL][BK_EPT];
-    const int nv = (j - i0) < BK_DOT_UNROLL ? (j - i0) : BK_DOT_UNROLL;
-#pragma unroll
-    for (int u = 0; u < BK_DOT_UNROLL; ++u) {
-      const double* Vi = V + (long long)(i0 + (u < nv ? u : 0)) * ld;
-#pragma unroll
-      for (int e = 0; e < BK_EPT; ++e) ld_v[u][e] = __ldg(Vi + off[e]);
-    }
-#pragma unroll
-    for (int u = 0; u < BK_DOT_UNROLL; ++u) {
-      double a = 0.0;
-#pragma unroll
-      for (int e = 0; e < BK_EPT; ++e) a = fma(ld_v[u][e], val[e], a);
-      acc[u] = bk_warp_sum(a);
-    }
-    if (lane == 0) {
-#pragma unroll
-      for (int u = 0; u < BK_DOT_UNROLL; ++u)
-        if (u < nv) sred[(i0 + u) * 8 + wid] = acc[u];
-    }
-  }
-  __syncthreads();
-  const int G = gridDim.x;
-  for (int i = threadIdx.x; i < j; i += blockDim.x) {
-    double t = 0.0;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) t += sred[i * 8 + k];
-    partials[(long long)i * G + blockIdx.x] = t;
-  }
-  if (bk_last_block(counter, s_flag)) {
-    for (int i = wid; i < j; i += 8) {
-      double t = 0.0;
-      for (int k = lane; k < G; k += 32) t += __ldcg(partials + (long long)i * G + k);
-      t = bk_warp_sum(t);
-      if (lane == 0) {
-        double s = scales[i];
-        double h = s * t;
-        hcol[i] = h;
-        gcoef[i] = h * s;
-      }
-    }
-  }
-}
-
-// ---- pass 1, fused with the SH stencil ---------------------------------------------------------------
-template <int DIM>
-static __global__ void __launch_bounds__(BK_THREADS) k_fused_jvp_dots(OpDesc op, const double* __restrict__ in,
-                                                                      const double* __restrict__ in_scale_ptr,
-                                                                      double* __restrict__ w,
-                                                                      const double* __restrict__ V, long long ld, int j,
-                                                                      const double* __restrict__ scales,
-                                                                      double* __restrict__ partials,
-                                                                      unsigned int* counter, double* __restrict__ hcol,
-                                                                      double* __restrict__ gcoef) {
-  extern __shared__ double smem[];
-  __shared__ int s_flag;
-  double val[BK_EPT];
-  long long off64[BK_EPT];
-  int off[BK_EPT];
-  const double s = in_scale_ptr ? __ldg(in_scale_ptr) : 1.0;
-  sh_tile_eval<DIM, 0>(op, in, s, smem, val, off64);
-#pragma unroll
-  for (int e = 0; e < BK_EPT; ++e) {
-    if (off64[e] >= 0) w[off64[e]] = val[e];
-    off[e] = off64[e] >= 0 ? (int)off64[e] : 0;
-  }
-  __syncthreads();  // stencil tiles are dead: the same shared memory becomes the reduction scratch
-  bk_dots_reduce(val, off, V, ld, j, scales, smem, partials, counter, hcol, gcoef, &s_flag);
-}
-
-// ---- pass 1 without the stencil: w already in memory (left-preconditioned / non-fused operators) ---------
-static __global__ void __launch_bounds__(BK_THREADS) k_dots(const double* __restrict__ w, long long n,
-                                                            const double* __restrict__ V, long long ld, int j,
-                                                            const double* __restrict__ scales,
-                                                            double* __restrict__ partials, unsigned int* counter,
-                                                            double* __restrict__ hcol, double* __restrict__ gcoef) {
-  extern __shared__ double smem[];
-  __shared__ int s_flag;
-  double val[BK_EPT];
-  int off[BK_EPT];
-  const long long base = (long long)blockIdx.x * BK_TILE;
-#pragma unroll
-  for (int e = 0; e < BK_EPT; ++e) {
-    long long g = base + threadIdx.x + e * BK_THREADS;
-    bool ok = g < n;
-    off[e] = ok ? (int)g : 0;
-    val[e] = ok ? w[g] : 0.0;
-  }
-  bk_dots_reduce(val, off, V, ld, j, scales, smem, partials, counter, hcol, gcoef, &s_flag);
-}
-
-// ---- pass 2: v' = w - sum_i g_i V_i ; ||v'||^2 ---------------------------------------------------------
-static __global__ void __launch_bounds__(BK_THREADS) k_update_norm(const double* w, long long n,  // w may alias vout
-                                                                   const double* __restrict__ V, long long ld, int j,
-                                                                   const double* __restrict__ gcoef,
-                                                                   double* vout,
-                                                                   double* __restrict__ partials, unsigned int* counter,
-                                                                   double* __restrict__ h_out,
-                                                                   double* __restrict__ scale_out) {
-  __shared__ double s_w[8];
-  __shared__ int s_flag;
-  double val[BK_EPT];
-  int off[BK_EPT];
-  bool ok[BK_EPT];
-  const long long base = (long long)blockIdx.x * BK_TILE;
-#pragma unroll
-  for (int e = 0; e < BK_EPT; ++e) {
-    long long g = base + threadIdx.x + e * BK_THREADS;
-    ok[e] = g < n;
-    off[e] = ok[e] ? (int)g : 0;
-    val[e] = ok[e] ? w[g] : 0.0;
-  }
-  for (int i0 = 0; i0 < j; i0 += BK_DOT_UNROLL) {
-    double ld_v[BK_DOT_UNROLL][BK_EPT];
-    double gc[BK_DOT_UNROLL];
-    const int nv = (j - i0) < BK_DOT_UNROLL ? (j - i0) : BK_DOT_UNROLL;
-#pragma unroll
-    for (int u = 0; u < BK_DOT_UNROLL; ++u) {
-      const int i = i0 + (u < nv ? u : 0);
-      const double* Vi = V + (long long)i * ld;
-      gc[u] = (u < nv) ? gcoef[i] : 0.0;
-#pragma unroll
-      for (int e = 0; e < BK_EPT; ++e) ld_v[u][e] = __ldg(Vi + off[e]);
-    }
-#pragma unroll
-    for (int u = 0; u < BK_DOT_UNROLL; ++u)
-#pragma unroll
-      for (int e = 0; e < BK_EPT; ++e) val[e] = fma(-gc[u], ld_v[u][e], val[e]);
-  }
-  double acc = 0.0;
-#pragma unroll
-  for (int e = 0; e < BK_EPT; ++e) {
-    if (ok[e]) {
-      vout[off[e]] = val[e];
-      acc = fma(val[e], val[e], acc);
-    }
-  }
-  acc = bk_warp_sum(acc);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) s_w[wid] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0;
-    for (int k = 0; k < 8; ++k) t += s_w[k];
-    partials[blockIdx.x] = t;
-  }
-  if (bk_last_block(counter, &s_flag)) {
-    double t = 0.0;
-    for (int k = threadIdx.x; k < (int)gridDim.x; k += blockDim.x) t += __ldcg(partials + k);
-    t = bk_warp_sum(t);
-    if (lane == 0) s_w[wid] = t;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double r = 0;
-      for (int k = 0; k < 8; ++k) r += s_w[k];
-      double h = sqrt(r);
-      *h_out = h;
-      *scale_out = 1.0 / h;
-    }
-  }
-}
 
 // ---- x = beta x + sum_i coef_i * scales_i * V'_i -----------------------------------------------------------
 static __global__ void __launch_bounds__(BK_THREADS) k_lincomb(double* __restrict__ x, double beta, long long n,
@@ -294,9 +124,15 @@ static size_t sh2_scratch_bytes(int E) { return sizeof(double) * (size_t)((BK2_R
     default: { constexpr int EE = 8; __VA_ARGS__; } break; \
   }
 
-static bool fused2_available(const OpDesc& op) { return op.kind == BK_SH2D && (op.nx % 2 == 0); }
+// Whether the Arnoldi steps of a solve run k2_fused (JVP + dots in one kernel) or the stand-alone apply + k2_dots.  k2_fused
+// tiles one real SH2d grid in TMA rows of an even length and carries at most one border; the operator output must feed the
+// dots directly, so no left preconditioner.  3-D always runs unfused: a ring kernel would gain < 5 % (DESIGN.md §4.4).
+static bool fuses_jvp(const bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o) {
+  const bool left = o->pc_side == BK_SIDE_LEFT && c->pc.kind != BK_PC_NONE;
+  return o->fused && op.kind == BK_SH2D && op.nx % 2 == 0 && !op.cplx && op.bordered <= 1 && !left;
+}
 
-static int launch_fused2(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* w, int j, double* hcol) {
+static int launch_fused(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* w, int j, double* hcol) {
   const int tiles_x = (op.nx + BK2_ROW - 1) / BK2_ROW;
   Plan2 p = plan2(c, (long long)tiles_x * op.ny, sh2_scratch_bytes);
   p.grid = tiles_x * ((op.ny + p.E - 1) / p.E);
@@ -321,41 +157,6 @@ static int launch_fused2(bk_ctx* c, const OpDesc& op, const double* in, const do
 
 // ------------------------------------------------------------------------------------------------ host
 static inline int chunk_grid(long long n) { return (int)((n + BK_TILE - 1) / BK_TILE); }
-
-// fused_mode: bk_gmres_opts.fused -- 0 never, 1 automatic (the measured-fastest arrangement), 2 wherever a fused kernel exists.
-// 3-D: the fused kernel is still the first-generation one (64 KB tiles, more than two waves at 128^3), slower per iteration
-// than stand-alone JVP + TMA-ring dots, so "automatic" keeps it off until a TMA-ring 3-D kernel exists.
-static bool fused_available(const OpDesc& op, int fused_mode = 2) {
-  if (op.cplx) return false;  // the fused kernels tile one real grid; a split complex vector takes the two-launch path
-  if (op.bordered > 1) return false;  // block borders: stencil + k_tail2
-  if (op.kind == BK_SH2D) return !op.bordered || (op.nx % 2 == 0);
-  if (op.kind == BK_SH3D) return !op.bordered && fused_mode >= 2;
-  return false;
-}
-
-static size_t dots_smem(int j) { return sizeof(double) * 8 * (size_t)(j > 0 ? j : 1); }
-
-static int launch_fused(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* w, int j, double* hcol) {
-  size_t red = dots_smem(j);
-  if (op.kind == BK_SH2D) {
-    size_t sm = ShSmem<2>::BYTES > red ? ShSmem<2>::BYTES : red;
-    bk_ensure_smem(c, k_fused_jvp_dots<2>, sm);
-    int g = sh_num_tiles<2>(op.nx, op.ny, 1);
-    BK_CHECK(c, g <= c->gmax, "partial-sum workspace too small for the fused grid");
-    k_fused_jvp_dots<2><<<g, BK_THREADS, sm, c->stream>>>(op, in, sp, w, c->V, c->ld, j, c->scales, c->partials,
-                                                          c->counters + 0, hcol, c->gcoef);
-  } else {
-    size_t sm = ShSmem<3>::BYTES > red ? ShSmem<3>::BYTES : red;
-    bk_ensure_smem(c, k_fused_jvp_dots<3>, sm);
-    int g = sh_num_tiles<3>(op.nx, op.ny, op.nz);
-    BK_CHECK(c, g <= c->gmax, "partial-sum workspace too small for the fused grid");
-    k_fused_jvp_dots<3><<<g, BK_THREADS, sm, c->stream>>>(op, in, sp, w, c->V, c->ld, j, c->scales, c->partials,
-                                                          c->counters + 0, hcol, c->gcoef);
-  }
-  c->stats.kernel_launches++;
-  BK_CUDA(c, cudaGetLastError());
-  return BK_OK;
-}
 
 int bk_launch_dots(bk_ctx* c, const double* basis, const double* scales, const double* w, long long n, int j, double* hcol,
                    double* gcoef) {
@@ -424,7 +225,8 @@ struct TimerScope {
 };
 
 // One Arnoldi step k (0-based): basis v'_0..v'_k -> v'_{k+1}, H column k on device (+ async copy to pinned host).
-static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, long long n, int k, size_t* timer_slot) {
+// fuse: fuses_jvp() of the solve.
+static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, long long n, int k, bool fuse, size_t* timer_slot) {
   const int j = k + 1;
   const int mh = c->m + 4;
   // The H column is written by the kernels' last CTA straight into pinned, device-mapped host memory (UVA): no
@@ -439,15 +241,11 @@ static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, lon
     BK_TRY(bk_precond_apply_dev(c, in, c->z, n));
     in = c->z;
   }
-  const bool fuse = o->fused && fused_available(op, o->fused) && !left;
   TimerScope ts(c);
   const double* wfin = c->w;
   if (fuse) {
     ts.begin((*timer_slot)++);
-    if (fused2_available(op))
-      BK_TRY(launch_fused2(c, op, in, sp, c->w, j, hcol));
-    else
-      BK_TRY(launch_fused(c, op, in, sp, c->w, j, hcol));
+    BK_TRY(launch_fused(c, op, in, sp, c->w, j, hcol));
     ts.end();
   } else {
     BK_TRY(bk_launch_apply(c, op, in, sp, c->w));
@@ -514,6 +312,7 @@ int bk_gmres_dev(bk_ctx* c, const OpDesc& op, const double* rhs, double* x, cons
   const int mh = c->m + 4;
   const bool right = o->pc_side == BK_SIDE_RIGHT && c->pc.kind != BK_PC_NONE;
   BK_CHECK(c, o->pc_side == BK_SIDE_NONE || c->pc.kind != BK_PC_NONE, "pc_side set but no preconditioner was set up");
+  const bool fuse = fuses_jvp(c, op, o);
   c->stats.last_fused_bytes = 0;
   c->stats.last_fused_launches = 0;
   c->stats.last_fused_ms = 0.0;
@@ -564,7 +363,7 @@ int bk_gmres_dev(bk_ctx* c, const OpDesc& op, const double* rhs, double* x, cons
     while (true) {
       bool can_launch = kl < restart && (total + (kl - kd)) < maxiter && !stop;
       if (can_launch && (kl - kd) < 2) {
-        BK_TRY(arnoldi_step(c, op, o, n, kl, &timer_slot));
+        BK_TRY(arnoldi_step(c, op, o, n, kl, fuse, &timer_slot));
         ++kl;
         continue;
       }
@@ -639,7 +438,7 @@ int bk_gmres_dev(bk_ctx* c, const OpDesc& op, const double* rhs, double* x, cons
       if (cudaEventElapsedTime(&t, c->tpairs[i].first, c->tpairs[i].second) == cudaSuccess) ms += t;
     }
     c->stats.last_fused_ms = ms;
-    if (o->fused && fused_available(op, o->fused) && !(o->pc_side == BK_SIDE_LEFT && c->pc.kind != BK_PC_NONE)) c->stats.total_fused_ms += ms;
+    if (fuse) c->stats.total_fused_ms += ms;
   }
   if (converged) *converged = conv ? 1 : 0;
   if (iters) *iters = total;

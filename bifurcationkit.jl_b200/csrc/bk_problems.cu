@@ -361,9 +361,7 @@ static int launch_kind(bk_ctx* c, const OpDesc& op, const double* in, const doub
   switch (op.kind) {
     case BK_SH2D: {
       const bool aligned = (op.nx % 2 == 0) && ((((uintptr_t)in) & 15) == 0);
-      static int no_tma = -1;
-      if (no_tma < 0) no_tma = getenv("BK_SH2D_NO_TMA") ? 1 : 0;  // diagnostics: the first-generation 64 x 32 tile kernel
-      if (aligned && !no_tma) {
+      if (aligned) {
         // TMA-staged tile (bk_krylov_tma.cuh): tallest tile that still gives every SM about two CTAs
         const int tiles_x = (op.nx + BK2_ROW - 1) / BK2_ROW;
         int E = BK2_EMAX;

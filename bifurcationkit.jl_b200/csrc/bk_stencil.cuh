@@ -1,5 +1,6 @@
-// bk_stencil.cuh -- device-side tile evaluators of the named PDE stencils (K1/K2), shared by the
-// stand-alone apply kernels (bk_problems.cu) and the fused JVP+Arnoldi kernel (bk_krylov.cu).
+// bk_stencil.cuh -- device-side tile evaluators of the Swift-Hohenberg stencils (K1/K2) for the
+// stand-alone apply kernel k_sh_apply (bk_problems.cu): every SH3d residual / JVP, and SH2d where the
+// TMA-staged tile of bk_krylov_tma.cuh does not apply (odd nx or an input not 16-byte aligned).
 //
 // Swift-Hohenberg (examples/SH2d-fronts.jl:13-34,124-127; examples/SH3d.jl:16-53):
 //   L1 = (I + Lap)^2 with the Neumann-closure Laplacian (corner diagonal -1/h^2) == two passes of

@@ -71,8 +71,8 @@ typedef struct bk_gmres_opts {
   int32_t maxiter; /* 100  */
   int32_t pc_side; /* BK_SIDE_*: which of Pl / Pr holds the context's preconditioner */
   int32_t orth;    /* BK_ORTH_CGS (single classical Gram-Schmidt pass) or BK_ORTH_CGS2 */
-  int32_t fused;   /* 0: separate kernels; 1: automatic (JVP fused into the Arnoldi dot kernel where that is the fastest
-                      arrangement: 2-D SH incl. the bordered map); 2: fused wherever a fused kernel exists (also 3-D SH) */
+  int32_t fused;   /* 0: separate kernels; nonzero: JVP fused into the Arnoldi dot kernel where a fused kernel exists, i.e. real
+                      SH2d with an even nx, at most one border (the bordered map), preconditioner not on the left */
   int32_t reserved;
 } bk_gmres_opts;
 
@@ -231,7 +231,6 @@ int32_t bk_palc_run(bk_ctx* ctx, const bk_palc_opts* opts, const bk_gmres_opts* 
  *   BK_NO_PDL=1         launch without programmatic dependent launch (plain stream order)
  *   BK_FFT_LOGE=2..5    complex values per thread (2^e) of the power-of-two transform kernels instead of the per-size default
  *   BK_FFT_NO_FAST=1    every transform through the general mixed-radix kernel (bk_fft_gen.cuh)
- *   BK_SH2D_NO_TMA=1    stand-alone SH2d residual / JVP on the first-generation 64 x 32 tile kernel instead of the TMA-staged tile
  *   BK_NSM=1..1024      size grids and reductions (read at bk_ctx_create) as for a device with that many SMs: changes the summation
  *                       order of every reduction, so it shows how a result depends on it */
 

@@ -49,6 +49,9 @@ def test_ring_kernels_use_tma_bulk_copies_and_mbarriers(sass):
         assert c["DFMA"] >= 1 and c["LDL"] == 0 and c["STL"] == 0, (k, dict(c))  # fp64 pipe, nothing spilled to local memory
     fused = [c for k, c in ring.items() if "k2_fused" in k]
     assert all(c["UBLKPF"] >= 1 for c in fused)                        # L2 prefetch of the u / a / b rows (cp.async.bulk.prefetch)
+    # the ring kernels are the only Arnoldi kernels: no non-ring JVP+dots, dots or update kernel is built
+    old = [k for k in cnt if re.search(r"(?<!\d)(16k_fused_jvp_dots|6k_dots|13k_update_norm)", k)]
+    assert not old, old
 
 
 def test_transform_kernels_stage_their_tables_by_bulk_copy(sass):

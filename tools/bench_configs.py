@@ -122,9 +122,8 @@ if "5" in which:
     s0 = (np.cos(X)[None, None, :] * np.cos(X)[None, :, None] * np.ones(n3)[:, None, None])
     s0 = s0 - s0.min(); s0 = s0 / s0.max() * 1.2
     ctx.precond_setup(bk.BK_PC_SH_DCT, 1.0)
-    FUSED = os.environ.get("BK_FUSED3D", "1") == "1"
-    ls = bk.GMRESB200(reltol=1e-9, restart=150, maxiter=150, Pr=True, orth="cgs2", fused=FUSED)  # rtol of examples/SH3d.jl:93
-    ls_newton = bk.GMRESB200(reltol=1e-6, restart=150, maxiter=150, Pr=True, fused=FUSED)
+    ls = bk.GMRESB200(reltol=1e-9, restart=150, maxiter=150, Pr=True, orth="cgs2")  # rtol of examples/SH3d.jl:93
+    ls_newton = bk.GMRESB200(reltol=1e-6, restart=150, maxiter=150, Pr=True)
     # Newton from the raw guess wanders at this domain size (many unstable directions); relax it first with the
     # semi-implicit gradient flow u <- u + (L1 + 1/dt + sigma)^-1 F(u) (same DCT solver, shift 4), then polish with Newton
     u_dev = ctx.to_device(s0.reshape(-1)); fbuf = ctx.zeros(); pbuf = ctx.zeros()
