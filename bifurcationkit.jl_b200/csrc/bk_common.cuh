@@ -61,6 +61,26 @@ struct Plan {
 };
 }  // namespace bkg
 
+// Pointwise prologue / epilogue of the periodic spectral pipeline (BK_SH2D_PERIODIC, bk_fft_fast.cuh k_contig MODE 2 / 3).
+// The x r2c pass reads s v (pro = PW_D: s v d(u)); the x c2r pass turns the spectral result y into the output:
+//   PW_NONE  y                       (preconditioner)
+//   PW_RESID y + l v + nu v^2 - v^3  (residual, v = u)
+//   PW_JVP   y + (a0 + a1 c(u)) s v  (the symbol carries -a1 L1)
+//   PW_FLEFT y - a1 s v              (P (a0 I + a1 J) v = P (d v) - a1 v)
+//   PW_FRIGHT d(u) y - a1 s v        ((a0 I + a1 J) P v = d (P v) - a1 v)
+// with c(u) = l + 2 nu u - 3 u^2,  d(u) = a0 + a1 (spc + c(u)),  s = *sp (1 when sp is NULL).
+enum { PW_NONE = 0, PW_RESID = 1, PW_JVP = 2, PW_FLEFT = 3, PW_FRIGHT = 4 };
+struct PerPw {
+  int pro;               // 0: s v, 1 (PW_D): s v d(u)
+  int epi;               // PW_*
+  const double* v;       // operator input (the epilogue reads it again)
+  const double* u;       // linearisation state
+  const double* sp;      // device scalar s, may be NULL
+  double a0, a1, l, nu;
+  double spc;            // shift of the preconditioner (L1 + spc I)^-1
+};
+#define PW_D 1
+
 struct Precond {
   int kind = BK_PC_NONE;
   double a0 = 0, a1 = 0;
@@ -196,6 +216,14 @@ int bk_potrap_refresh_cache(bk_ctx* c);
 
 int bk_precond_apply_dev(bk_ctx* c, const double* in_dev, double* out_dev, long long n);
 void bk_harvest_pc_timing(bk_ctx* c);
+
+// BK_SH2D_PERIODIC (bk_precond.cu): transform tables and work buffers at bk_ctx_create, then the three-kernel spectral pipeline
+// x r2c -> y (forward, symbol, inverse) -> x c2r for the residual, the JVP and the one-transform preconditioned operator
+int bk_periodic_setup(bk_ctx* c);
+int bk_periodic_residual(bk_ctx* c, const OpDesc& op, const double* u, double* out);
+int bk_periodic_jvp(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* out);
+// left: P (a0 I + a1 J) v, right: (a0 I + a1 J) P v, P = (L1 + pc.a0 I)^-1 (BK_PC_SH_FFT); op unbordered and real
+int bk_periodic_fused(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* out, bool left);
 
 // vector kernels (device pointers)
 int bk_dev_axpby(bk_ctx* c, double* y, double a, const double* x, double b, long long n);

@@ -90,6 +90,14 @@ extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dim
   switch (kind) {
     case BK_CHAN: n = c->dims[0]; break;
     case BK_SH2D: n = c->dims[0] * c->dims[1]; break;
+    case BK_SH2D_PERIODIC:
+      for (int d = 0; d < 2; ++d) {
+        const long long v = c->dims[d];
+        BK_CHECK(c, v >= 64 && v <= 2048 && (v & (v - 1)) == 0,
+                 "BK_SH2D_PERIODIC: Nx and Ny must be powers of two from 64 to 2048");
+      }
+      n = c->dims[0] * c->dims[1];
+      break;
     case BK_SH3D: n = c->dims[0] * c->dims[1] * c->dims[2]; break;
     case BK_CGL2D: n = 2 * c->dims[0] * c->dims[1]; break;
     case BK_POTRAP_CGL2D: n = 2 * c->dims[0] * c->dims[1] * c->dims[2] + 1; break;
@@ -156,6 +164,7 @@ extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dim
     BK_CUDA(c, cudaMemset(c->phi, 0, 8 * ld));
     BK_CUDA(c, cudaMemset(c->xpi, 0, 8 * ld));
   }
+  if (kind == BK_SH2D_PERIODIC) BK_TRY(bk_periodic_setup(c));
   BK_CUDA(c, cudaStreamSynchronize(c->stream));
   return BK_OK;
 }

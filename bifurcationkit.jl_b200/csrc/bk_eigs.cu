@@ -283,7 +283,7 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
   bool converged = false;
   int keff = m;
   // ---------------- symmetric operators (Swift-Hohenberg): thick-restart (Krylov-Schur with Ritz vectors) ----------------
-  const bool sym = (c->kind == BK_SH2D || c->kind == BK_SH3D);
+  const bool sym = (c->kind == BK_SH2D || c->kind == BK_SH3D || c->kind == BK_SH2D_PERIODIC);
   std::vector<double> Ssym, wsym;
   std::vector<int> order;
   if (sym) {

@@ -19,6 +19,9 @@
 //    the lanes of different line pairs);
 //  * shared-memory slot of position i of pair pr:  (i + (i >> 2) + (i >> PB)) * PP + pr  (conflict-free for every pass in the
 //    bank model tools/fftcheck/model.py + tools/fftcheck/padsearch.py).
+//  * the periodic kind (BK_SH2D_PERIODIC) reuses the same FFT as a real 2-D transform: k_contig MODE 2 / 3 (x r2c / c2r, two
+//    rows per complex line, packed half-spectrum, pointwise prologue / epilogue) and k_strided MODE 3 (y forward, periodic
+//    symbol, inverse).
 // Executable specification, thread by thread: tools/fftcheck/model.py (checked against scipy.fft).
 // Device check + timing: tools/fftcheck/fft_check.cu.
 #pragma once
@@ -42,6 +45,11 @@ struct Cfg {
   // resident threads per SM the register budget is sized for (launch bounds): few fat threads (E = 32: 255 registers) ... many thin ones
   static constexpr int TPSM = LOGE == 5 ? 256 : LOGE == 4 ? 512 : LOGE == 3 ? 768 : 1024;
   static constexpr int MINB = TPSM / THREADS > 0 ? TPSM / THREADS : 1;
+  // the periodic r2c split and the periodic y pass hold twice the values across a barrier: one CTA per SM fewer, so the
+  // instantiations the library launches (E = 4 below n = 1024, E = 8 from 1024 on; bk_precond.cu::fast_loge) do not spill
+  // (tests/test_sass_periodic_cpu.py).  Other E, reachable only through BK_FFT_LOGE, still spill in some periodic modes
+  // (e.g. k_strided MODE 3 at n = 512, E = 16; n = 2048, E = 4): correct, but not tuned.
+  static constexpr int MINB_P = MINB > 1 ? MINB - 1 : 1;
   // padding of the NATURAL-order staging array of the contiguous kernels (scatter by register = digit-reversed k, then read
   // k = tau + T i): conflict-free choices from the same bank model (tools/fftcheck/padsearch.py)
   static constexpr int NB = LOGE == 2 ? (LOGN <= 6 ? 0 : LOGN <= 8 ? 4 : LOGN <= 10 ? 6 : 8)
@@ -222,6 +230,7 @@ struct Symbol {
   const double* tail_src;  // optional pass-through of trailing (border) entries
   double* tail_dst;
   int tail_n;
+  int neg;              // periodic kernel (MODE 3): 1 -> symbol -scale L1, 0 -> scale / (L1 + shift)
 };
 
 template <class C>
@@ -372,23 +381,86 @@ __device__ __forceinline__ void strided_store(const double2 (&a)[C::E], double* 
   }
 }
 
-#define BKF_BOUNDS(C) __launch_bounds__(C::THREADS, C::MINB)
+#define BKF_BOUNDS(C, PERIODIC) __launch_bounds__(C::THREADS, (PERIODIC) ? C::MINB_P : C::MINB)
+
+// 1 / x for 0 < x < 2^1000: hardware estimate + two Newton steps (no division slow path: its call frame spills)
+__device__ __forceinline__ double rcp_nr(double x) {
+  double r;
+  asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(x));
+  double e = fma(-x, r, 1.0);
+  r = fma(r, e, r);
+  e = fma(-x, r, 1.0);
+  return fma(r, e, r);
+}
+// periodic symbol of one element, lam = lambda_x + lambda_y (eigenvalues of the periodic Laplacian, -k^2)
+__device__ __forceinline__ double per_symbol(const Symbol& sy, double lam) {
+  const double t = 1.0 + lam, l1 = t * t;
+  return sy.neg ? -sy.scale * l1 : sy.scale * rcp_nr(l1 + sy.shift);
+}
 
 // MODE 0: forward (out = 2 C, natural k along the line), 1: inverse (out = n x from C), 2: forward, divide by the symbol, inverse
+// MODE 3: periodic y pass of BK_SH2D_PERIODIC: forward FFT, multiply by the periodic symbol, inverse, natural order both ways.
+//   The input rows are the packed half-spectra of k_contig MODE 2, so for q >= 1 the column pair (2q, 2q+1) is the complex line
+//   of kx = q (one 16-byte load per element).  Pair (0, 1) holds two real lines, kx = 0 and kx = Nx/2, with symbols s0 and sn;
+//   as the symbol is even in ky, Z'[k] = ((s0 + sn)/2) Z[k] + ((s0 - sn)/2) conj Z[-k] (one partner read).
 template <class C, int MODE>
-static __global__ void BKF_BOUNDS(C) k_strided(const double* __restrict__ in, double* __restrict__ out, Geom g, Tables tbg, Symbol sy) {
+static __global__ void BKF_BOUNDS(C, MODE == 3) k_strided(const double* __restrict__ in, double* __restrict__ out, Geom g, Tables tbg, Symbol sy) {
   extern __shared__ __align__(128) double2 sm_fast[];
   __shared__ __align__(8) unsigned long long tbar;
   double2* sm = sm_fast;
-  const Tables tb = stage_tables<C, MODE == 2>(tbg, sm, &tbar);
+  const Tables tb = stage_tables<C, MODE == 2 || MODE == 3>(tbg, sm, &tbar);
   const int tid = threadIdx.x, pr = tid % C::PP, tau = tid / C::PP;
   __syncthreads();  // the barrier is initialised before anybody waits on it
   bk_pdl_sync();
   const int col = (blockIdx.x * C::PP + pr) * 2, o = blockIdx.y;
   const bool v0 = col < g.nb, v1 = col + 1 < g.nb;
   const long long off = (long long)o * g.os + col;
-  if (MODE == 2 && sy.tail_n > 0 && blockIdx.x == 0 && blockIdx.y == 0 && tid < sy.tail_n) sy.tail_dst[tid] = sy.tail_src[tid];
+  if ((MODE == 2 || MODE == 3) && sy.tail_n > 0 && blockIdx.x == 0 && blockIdx.y == 0 && tid < sy.tail_n)
+    sy.tail_dst[tid] = sy.tail_src[tid];
   double2 a[C::E];
+  if (MODE == 3) {
+#pragma unroll
+    for (int i = 0; i < C::E; ++i) {
+      const double* p = in + off + (long long)(i * C::T + tau) * g.es;
+      a[i] = v1 ? __ldg(reinterpret_cast<const double2*>(p)) : make_double2(v0 ? __ldg(p) : 0.0, 0.0);
+    }
+    mbar_wait(&tbar, 0);
+    fwd_passes<C, 0>(a, sm, tb, tau, pr);
+    const bool nyq = blockIdx.x == 0 && pr == 0;   // column pair (0, 1): kx = 0 and kx = Nx/2
+    if (blockIdx.x == 0) {                          // CTA-uniform
+      park<C>(a, sm, tau, pr);
+      __syncthreads();
+      if (nyq) {
+        const double l0 = __ldg(sy.lam_b), ln = __ldg(sy.lam_b + (g.nb >> 1));
+#pragma unroll
+        for (int reg = 0; reg < C::E; ++reg) {
+          int k;
+          const double2 z = a[reg], zp = partner<C>(sm, reg_pos<C>(tau, reg), pr, k);
+          const double ly = tb.lam2[reg * C::T + tau].x;
+          const double s0 = per_symbol(sy, l0 + ly), sn = per_symbol(sy, ln + ly);
+          const double hp = 0.5 * (s0 + sn), hm = 0.5 * (s0 - sn);
+          a[reg] = make_double2(fma(hp, z.x, hm * zp.x), fma(hp, z.y, -(hm * zp.y)));
+        }
+      }
+      __syncthreads();
+    }
+    if (!nyq) {
+      const double lq = v0 ? __ldg(sy.lam_b + (col >> 1)) : 0.0;
+#pragma unroll
+      for (int reg = 0; reg < C::E; ++reg) {
+        const double s = per_symbol(sy, lq + tb.lam2[reg * C::T + tau].x);
+        a[reg] = make_double2(s * a[reg].x, s * a[reg].y);
+      }
+    }
+    inv_passes<C, C::NP - 1>(a, sm, tb, tau, pr);
+#pragma unroll
+    for (int i = 0; i < C::E; ++i) {
+      double* p = out + off + (long long)(i * C::T + tau) * g.es;
+      if (v1) *reinterpret_cast<double2*>(p) = a[i];
+      else if (v0) *p = a[i].x;
+    }
+    return;
+  }
   if (MODE != 1) {
     strided_load<C>(a, in + off, g.es, tau, v0, v1);
     mbar_wait(&tbar, 0);
@@ -474,8 +546,30 @@ static __global__ void BKF_BOUNDS(C) k_strided(const double* __restrict__ in, do
 template <class C>
 __device__ __forceinline__ int nslot(int k, int pr) { return C::padn(k) * C::PP + pr; }
 
+__device__ __forceinline__ double pw_c(const PerPw& pw, double u) { return fma(u, fma(-3.0, u, 2.0 * pw.nu), pw.l); }
+__device__ __forceinline__ double pw_d(const PerPw& pw, double u) { return fma(pw.a1, pw.spc + pw_c(pw, u), pw.a0); }
+// epilogue of the periodic c2r pass (PerPw, bk_common.cuh); v / u point at the row, m is the element
+__device__ __forceinline__ double pw_out(const PerPw& pw, double y, const double* v, const double* u, int m, double s) {
+  switch (pw.epi) {
+    case PW_RESID: {
+      const double x = __ldg(v + m);
+      return fma(x, fma(x, pw.nu - x, pw.l), y);
+    }
+    case PW_JVP: return fma(fma(pw.a1, pw_c(pw, __ldg(u + m)), pw.a0), s * __ldg(v + m), y);
+    case PW_FLEFT: return fma(-pw.a1 * s, __ldg(v + m), y);
+    case PW_FRIGHT: return fma(pw_d(pw, __ldg(u + m)), y, -pw.a1 * s * __ldg(v + m));
+    default: return y;
+  }
+}
+
+// MODE 2 / 3: the x passes of BK_SH2D_PERIODIC.  Two neighbouring rows form one complex line z = r_A + i r_B (natural order, no
+// Makhoul reordering), so one length-n FFT gives both real transforms: X_A[k] = (Z[k] + conj Z[n-k]) / 2,
+// X_B[k] = (Z[k] - conj Z[n-k]) / 2i.  A row is stored as its packed half-spectrum [Re X0, Re X_{n/2}, Re X1, Im X1, ...,
+// Re X_{n/2-1}, Im X_{n/2-1}] (n doubles).  MODE 2 (r2c) multiplies the input by the prologue of pw first; MODE 3 (c2r) rebuilds
+// Z[k] = X_A[k] + i X_B[k] (X[n-k] = conj X[k]), inverts (n z) and applies the epilogue of pw.  The caller's vectors are only
+// touched by 8-byte accesses, so they need no 16-byte alignment.
 template <class C, int MODE>
-static __global__ void BKF_BOUNDS(C) k_contig(const double* __restrict__ in, double* __restrict__ out, Geom g, Tables tbg) {
+static __global__ void BKF_BOUNDS(C, MODE == 2) k_contig(const double* __restrict__ in, double* __restrict__ out, Geom g, Tables tbg, PerPw pw) {
   extern __shared__ __align__(128) double2 sm_fast[];
   __shared__ __align__(8) unsigned long long tbar;
   double2* sm = sm_fast;
@@ -490,6 +584,90 @@ static __global__ void BKF_BOUNDS(C) k_contig(const double* __restrict__ in, dou
   double* outA = out + lineA * g.os;
   double* outB = out + lineB * g.os;
   double2 a[C::E];
+  if (MODE == 2) {
+    const double s = pw.sp ? __ldg(pw.sp) : 1.0;
+#pragma unroll
+    for (int i = 0; i < C::E; ++i) {
+      const int m = i * C::T + tau;
+      double xa = vA ? __ldg(inA + m) : 0.0, xb = vB ? __ldg(inB + m) : 0.0;
+      if (pw.pro == PW_D) {
+        xa *= vA ? pw_d(pw, __ldg(pw.u + lineA * g.os + m)) : 0.0;
+        xb *= vB ? pw_d(pw, __ldg(pw.u + lineB * g.os + m)) : 0.0;
+      }
+      a[i] = make_double2(s * xa, s * xb);
+    }
+    mbar_wait(&tbar, 0);
+    fwd_passes<C, 0>(a, sm, tb, tau, pr);
+    park<C>(a, sm, tau, pr);
+    __syncthreads();
+    double2 b[C::E];
+#pragma unroll
+    for (int reg = 0; reg < C::E; ++reg) {
+      int k;
+      const double2 z = a[reg], zp = partner<C>(sm, reg_pos<C>(tau, reg), pr, k);
+      // X_A = (Z + conj Zp) / 2,  X_B = (Z - conj Zp) / 2i;  a = (Re X_A, Re X_B), b = (Im X_A, Im X_B)
+      a[reg] = make_double2(0.5 * (z.x + zp.x), 0.5 * (z.y + zp.y));
+      b[reg] = make_double2(0.5 * (z.y - zp.y), 0.5 * (zp.x - z.x));
+    }
+    __syncthreads();  // every partner read is done: the natural-order array may overwrite the work array
+#pragma unroll
+    for (int reg = 0; reg < C::E; ++reg) {
+      const int k = k_of_pos<C>(reg_pos<C>(tau, reg));
+      if (k == 0) sm[nslot<C>(0, pr)] = a[reg];
+      else if (k == C::N / 2) sm[nslot<C>(1, pr)] = a[reg];
+      else if (k < C::N / 2) {
+        sm[nslot<C>(2 * k, pr)] = a[reg];
+        sm[nslot<C>(2 * k + 1, pr)] = b[reg];
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < C::E; ++i) {
+      const int p = i * C::T + tau;
+      const double2 d = sm[nslot<C>(p, pr)];
+      if (vA) outA[p] = d.x;
+      if (vB) outB[p] = d.y;
+    }
+    return;
+  }
+  if (MODE == 3) {
+#pragma unroll
+    for (int i = 0; i < C::E; ++i) {
+      const int p = i * C::T + tau;
+      sm[nslot<C>(p, pr)] = make_double2(vA ? __ldg(inA + p) : 0.0, vB ? __ldg(inB + p) : 0.0);
+    }
+    mbar_wait(&tbar, 0);
+    __syncthreads();
+#pragma unroll
+    for (int reg = 0; reg < C::E; ++reg) {
+      const int k = k_of_pos<C>(reg_pos<C>(tau, reg)), kk = k <= C::N / 2 ? k : C::N - k;
+      double2 xa, xb;  // X_A[kk], X_B[kk] (x: A, y: B in the packed pairs)
+      if (kk == 0 || kk == C::N / 2) {
+        const double2 d = sm[nslot<C>(kk ? 1 : 0, pr)];
+        xa = make_double2(d.x, 0.0);
+        xb = make_double2(d.y, 0.0);
+      } else {
+        const double2 re = sm[nslot<C>(2 * kk, pr)], im = sm[nslot<C>(2 * kk + 1, pr)];
+        xa = make_double2(re.x, k == kk ? im.x : -im.x);
+        xb = make_double2(re.y, k == kk ? im.y : -im.y);
+      }
+      a[reg] = make_double2(xa.x - xb.y, xa.y + xb.x);  // Z = X_A + i X_B
+    }
+    __syncthreads();  // the natural-order array is dead: the inverse passes reuse the memory
+    inv_passes<C, C::NP - 1>(a, sm, tb, tau, pr);
+    const double s = pw.sp ? __ldg(pw.sp) : 1.0;
+    const double* vrA = pw.v + lineA * g.os;
+    const double* vrB = pw.v + lineB * g.os;
+    const double* urA = pw.u ? pw.u + lineA * g.os : nullptr;
+    const double* urB = pw.u ? pw.u + lineB * g.os : nullptr;
+#pragma unroll
+    for (int i = 0; i < C::E; ++i) {
+      const int m = i * C::T + tau;
+      if (vA) outA[m] = pw_out(pw, a[i].x, vrA, urA, m, s);
+      if (vB) outB[m] = pw_out(pw, a[i].y, vrB, urB, m, s);
+    }
+    return;
+  }
   if (MODE == 0) {
 #pragma unroll
     for (int i = 0; i < C::E; ++i) {

@@ -18,6 +18,9 @@
 //                               Algorithmic traffic 8N(j+2): read w, V_1..V_j, write v'_{j+1}.
 //   k_lincomb                 : x = beta x + sum_i y_i s_i v'_i at restart and at the end.
 //
+// Periodic SH2d (BK_SH2D_PERIODIC) with BK_PC_SH_FFT on either side and fused set (fuses_pc): the preconditioned operator of a
+// step is ONE spectral pipeline (bk_periodic_fused: 3 transform kernels, 64N) in place of apply + preconditioner, then k2_dots.
+//
 // The basis is stored UN-normalised (v'_i) with the scalars s_i = 1/||v'_i|| kept on device, so
 // normalisation costs no memory pass ("deferred as a scalar") and the host never has to be in the
 // loop to launch the next step: Givens rotations run on the host one iteration behind the GPU.
@@ -132,6 +135,13 @@ static bool fuses_jvp(const bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o)
   return o->fused && op.kind == BK_SH2D && op.nx % 2 == 0 && !op.cplx && op.bordered <= 1 && !left;
 }
 
+// Whether the Arnoldi steps of a solve apply the preconditioned operator of BK_SH2D_PERIODIC in ONE spectral pipeline
+// (bk_periodic_fused: P (a0 I + a1 J) = P d - a1 I, (a0 I + a1 J) P = d P - a1 I) instead of precond + apply or apply + precond.
+static bool fuses_pc(const bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o) {
+  const bool side = o->pc_side == BK_SIDE_LEFT || o->pc_side == BK_SIDE_RIGHT;
+  return o->fused && op.kind == BK_SH2D_PERIODIC && c->pc.kind == BK_PC_SH_FFT && side && op.bordered == 0 && !op.cplx;
+}
+
 static int launch_fused(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* w, int j, double* hcol) {
   const int tiles_x = (op.nx + BK2_ROW - 1) / BK2_ROW;
   Plan2 p = plan2(c, (long long)tiles_x * op.ny, sh2_scratch_bytes);
@@ -225,8 +235,9 @@ struct TimerScope {
 };
 
 // One Arnoldi step k (0-based): basis v'_0..v'_k -> v'_{k+1}, H column k on device (+ async copy to pinned host).
-// fuse: fuses_jvp() of the solve.
-static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, long long n, int k, bool fuse, size_t* timer_slot) {
+// fuse: fuses_jvp() of the solve; fuse_pc: fuses_pc() of the solve.
+static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, long long n, int k, bool fuse, bool fuse_pc,
+                        size_t* timer_slot) {
   const int j = k + 1;
   const int mh = c->m + 4;
   // The H column is written by the kernels' last CTA straight into pinned, device-mapped host memory (UVA): no
@@ -237,13 +248,18 @@ static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, lon
   const double* sp = c->scales + k;
   const bool left = o->pc_side == BK_SIDE_LEFT && c->pc.kind != BK_PC_NONE;
   const bool right = o->pc_side == BK_SIDE_RIGHT && c->pc.kind != BK_PC_NONE;
-  if (right) {
+  if (right && !fuse_pc) {
     BK_TRY(bk_precond_apply_dev(c, in, c->z, n));
     in = c->z;
   }
   TimerScope ts(c);
   const double* wfin = c->w;
-  if (fuse) {
+  if (fuse_pc) {
+    BK_TRY(bk_periodic_fused(c, op, in, sp, c->w, left));
+    ts.begin((*timer_slot)++);
+    BK_TRY(launch_dots(c, c->w, n, j, hcol));
+    ts.end();
+  } else if (fuse) {
     ts.begin((*timer_slot)++);
     BK_TRY(launch_fused(c, op, in, sp, c->w, j, hcol));
     ts.end();
@@ -313,6 +329,7 @@ int bk_gmres_dev(bk_ctx* c, const OpDesc& op, const double* rhs, double* x, cons
   const bool right = o->pc_side == BK_SIDE_RIGHT && c->pc.kind != BK_PC_NONE;
   BK_CHECK(c, o->pc_side == BK_SIDE_NONE || c->pc.kind != BK_PC_NONE, "pc_side set but no preconditioner was set up");
   const bool fuse = fuses_jvp(c, op, o);
+  const bool fuse_pc = fuses_pc(c, op, o);
   c->stats.last_fused_bytes = 0;
   c->stats.last_fused_launches = 0;
   c->stats.last_fused_ms = 0.0;
@@ -363,7 +380,7 @@ int bk_gmres_dev(bk_ctx* c, const OpDesc& op, const double* rhs, double* x, cons
     while (true) {
       bool can_launch = kl < restart && (total + (kl - kd)) < maxiter && !stop;
       if (can_launch && (kl - kd) < 2) {
-        BK_TRY(arnoldi_step(c, op, o, n, kl, fuse, &timer_slot));
+        BK_TRY(arnoldi_step(c, op, o, n, kl, fuse, fuse_pc, &timer_slot));
         ++kl;
         continue;
       }

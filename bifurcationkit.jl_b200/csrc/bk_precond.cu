@@ -9,6 +9,8 @@
 //   Power-of-two line lengths 64..2048 run the register-resident FFT kernels of bk_fft_fast.cuh (two lines per complex
 //   FFT, the last dimension fused: forward + symbol + inverse, so an application is 3 kernels in 2-D and 5 in 3-D);
 //   every other length runs the mixed-radix kernel of bk_fft_gen.cuh.  No library on this path.
+// BK_PC_SH_FFT: (L1 + shift I)^-1 on the periodic grid of BK_SH2D_PERIODIC (examples/SH2d-fronts-cuda.jl:55-64), the real 2-D FFT
+//   pipeline of bk_periodic_setup / periodic_pipeline below, which also applies that kind's residual and JVP.
 // BK_PC_CHAN_TRIDIAG: lu(P) of examples/chan.jl:108-111 (Thomas algorithm, one thread: n = 1e3 plumbing).
 // BK_PC_CGL_DST: per-component (a0 I + a1 Lap_dirichlet)^-1 by DST-I (stand-in for the ILU of
 //   examples/cGL2d.jl:209-213); for potrap contexts it is applied slice by slice (block Jacobi, cf.
@@ -192,14 +194,17 @@ static int fast_setup(bk_ctx* c, int d, const double* lam_host) {
   return BK_OK;
 }
 
-// mode 0 forward (2 C), 1 inverse (n x), 2 fused forward + symbol + inverse (strided only)
+// strided: mode 0 forward (2 C), 1 inverse (n x), 2 fused forward + symbol + inverse, 3 periodic fused y pass;
+// contiguous: mode 0 forward, 1 inverse, 2 periodic r2c, 3 periodic c2r (prologue / epilogue pw)
 template <class FC>
 static int fast_launch(bk_ctx* c, int d, bool strided, int mode, const double* in, double* out, const bkf::Geom& g,
-                       const bkf::Symbol* sy) {
+                       const bkf::Symbol* sy, const PerPw* pw = nullptr) {
   Precond& pc = c->pc;
   bkf::Tables tb{pc.ftw[d], pc.fom[d], pc.flam2[d]};
   bkf::Symbol s0{};
   if (sy) s0 = *sy;
+  PerPw p0{};
+  if (pw) p0 = *pw;
   if (strided) {
     dim3 grid((g.nb + 2 * FC::PP - 1) / (2 * FC::PP), g.nouter);
     if (mode == 0) {
@@ -208,19 +213,25 @@ static int fast_launch(bk_ctx* c, int d, bool strided, int mode, const double* i
     } else if (mode == 1) {
       bk_ensure_smem(c, bkf::k_strided<FC, 1>, FC::SMEM);
       BK_CUDA(c, bk_launch_pdl(bkf::k_strided<FC, 1>, grid, dim3(FC::THREADS), FC::SMEM, c->stream, in, out, g, tb, s0));
-    } else {
+    } else if (mode == 2) {
       bk_ensure_smem(c, bkf::k_strided<FC, 2>, FC::SMEM_FUSED);
       BK_CUDA(c, bk_launch_pdl(bkf::k_strided<FC, 2>, grid, dim3(FC::THREADS), FC::SMEM_FUSED, c->stream, in, out, g, tb, s0));
+    } else {
+      bk_ensure_smem(c, bkf::k_strided<FC, 3>, FC::SMEM_FUSED);
+      BK_CUDA(c, bk_launch_pdl(bkf::k_strided<FC, 3>, grid, dim3(FC::THREADS), FC::SMEM_FUSED, c->stream, in, out, g, tb, s0));
     }
   } else {
     dim3 grid((unsigned)((g.nb + 2 * FC::PP - 1) / (2 * FC::PP)));
-    if (mode == 0) {
-      bk_ensure_smem(c, bkf::k_contig<FC, 0>, FC::SMEM);
-      BK_CUDA(c, bk_launch_pdl(bkf::k_contig<FC, 0>, grid, dim3(FC::THREADS), FC::SMEM, c->stream, in, out, g, tb));
-    } else {
-      bk_ensure_smem(c, bkf::k_contig<FC, 1>, FC::SMEM);
-      BK_CUDA(c, bk_launch_pdl(bkf::k_contig<FC, 1>, grid, dim3(FC::THREADS), FC::SMEM, c->stream, in, out, g, tb));
-    }
+#define BKF_CONTIG_GO(M)                                                                                                      \
+  do {                                                                                                                       \
+    bk_ensure_smem(c, bkf::k_contig<FC, M>, FC::SMEM);                                                                        \
+    BK_CUDA(c, bk_launch_pdl(bkf::k_contig<FC, M>, grid, dim3(FC::THREADS), FC::SMEM, c->stream, in, out, g, tb, p0));       \
+  } while (0)
+    if (mode == 0) BKF_CONTIG_GO(0);
+    else if (mode == 1) BKF_CONTIG_GO(1);
+    else if (mode == 2) BKF_CONTIG_GO(2);
+    else BKF_CONTIG_GO(3);
+#undef BKF_CONTIG_GO
   }
   return BK_OK;
 }
@@ -317,6 +328,61 @@ static int setup_dim(bk_ctx* c, int d, long long n, double inv_h2, int type, boo
   return gen_setup(c, d, (int)n, type);  // always available: unaligned vectors fall back to it
 }
 
+// ---- BK_SH2D_PERIODIC: real 2-D FFT pipeline -------------------------------------------------------------------------------
+// Tables for both dimensions are built once at bk_ctx_create: every operator application (residual, JVP, preconditioner, the
+// one-transform preconditioned operator) is  x r2c (k_contig MODE 2) -> y forward * symbol * inverse (k_strided MODE 3) ->
+// x c2r (k_contig MODE 3), through the two work buffers.  Periodic eigenvalues of the Laplacian: lambda[k] = -(pi k / l)^2 with
+// the signed frequency k (examples/SH2d-fronts-cuda.jl:48-50).
+int bk_periodic_setup(bk_ctx* c) {
+  Precond& pc = c->pc;
+  const long double PI = 3.14159265358979323846264338327950288L;
+  for (int d = 0; d < 2; ++d) {
+    const long long n = c->dims[d];
+    int logn = 0;
+    while ((1LL << logn) < n) ++logn;
+    BK_CHECK(c, (1LL << logn) == n && logn >= 6 && logn <= 11, "BK_SH2D_PERIODIC: Nx and Ny must be powers of two from 64 to 2048");
+    std::vector<double> lam(n);
+    for (long long k = 0; k < n; ++k) {
+      const long double ks = (long double)(k <= n / 2 ? k : k - n), w = PI * ks / (long double)c->lengths[d];
+      lam[k] = (double)(-w * w);
+    }
+    BK_TRY(upload(c, (void**)&pc.lam[d], lam.data(), 8 * n));
+    pc.fast[d] = logn;
+    BKF_DISPATCH(logn, BK_TRY(fast_setup<FC>(c, d, lam.data())));
+  }
+  if (!pc.work) BK_CUDA(c, cudaMalloc(&pc.work, 8 * (size_t)c->ld));
+  if (!pc.work2) BK_CUDA(c, cudaMalloc(&pc.work2, 8 * (size_t)c->ld));
+  return BK_OK;
+}
+
+// out = epilogue(F^-1 sigma F prologue(in)), sigma = gain / (Nx Ny) * (neg ? -L1 : 1 / (L1 + shift)); 3 kernels, 64N bytes at most
+static int periodic_pipeline(bk_ctx* c, const double* in, double* out, const PerPw& pw, bool neg, double gain, double shift,
+                             const double* tail_src = nullptr, double* tail_dst = nullptr, int tail_n = 0) {
+  Precond& pc = c->pc;
+  const int nx = (int)c->dims[0], ny = (int)c->dims[1];
+  const bkf::Geom gx{1, nx, ny, 1}, gy{nx, (long long)nx * ny, nx, 1};
+  const bkf::Symbol sy{pc.lam[0], nullptr, shift, gain / ((double)nx * (double)ny), tail_src, tail_dst, tail_n, neg ? 1 : 0};
+  BKF_DISPATCH(pc.fast[0], BK_TRY(fast_launch<FC>(c, 0, false, 2, in, pc.work, gx, nullptr, &pw)));
+  BKF_DISPATCH(pc.fast[1], BK_TRY(fast_launch<FC>(c, 1, true, 3, pc.work, pc.work2, gy, &sy)));
+  BKF_DISPATCH(pc.fast[0], BK_TRY(fast_launch<FC>(c, 0, false, 3, pc.work2, out, gx, nullptr, &pw)));
+  c->stats.kernel_launches += 3;
+  return BK_OK;
+}
+
+int bk_periodic_residual(bk_ctx* c, const OpDesc& op, const double* u, double* out) {
+  const PerPw pw{0, PW_RESID, u, nullptr, nullptr, 0.0, 0.0, op.par[0], op.par[1], 0.0};
+  return periodic_pipeline(c, u, out, pw, true, 1.0, 0.0);
+}
+int bk_periodic_jvp(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* out) {
+  const PerPw pw{0, PW_JVP, in, op.u, sp, op.a0, op.a1, op.par[0], op.par[1], 0.0};
+  return periodic_pipeline(c, in, out, pw, true, op.a1, 0.0);
+}
+int bk_periodic_fused(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* out, bool left) {
+  BK_CHECK(c, c->pc.kind == BK_PC_SH_FFT && !op.bordered && !op.cplx, "internal: one-transform operator needs BK_PC_SH_FFT, unbordered, real");
+  const PerPw pw{left ? PW_D : 0, left ? PW_FLEFT : PW_FRIGHT, in, op.u, sp, op.a0, op.a1, op.par[0], op.par[1], c->pc.a0};
+  return periodic_pipeline(c, in, out, pw, false, 1.0, c->pc.a0);
+}
+
 extern "C" int32_t bk_precond_setup(bk_ctx* c, int32_t kind, double a0, double a1) {
   BK_ENTER(c);
   BK_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -335,6 +401,10 @@ extern "C" int32_t bk_precond_setup(bk_ctx* c, int32_t kind, double a0, double a
       double h = 2 * c->lengths[d] / c->dims[d];
       BK_TRY(setup_dim(c, d, c->dims[d], 1.0 / (h * h), 0, even_nx));
     }
+  } else if (kind == BK_PC_SH_FFT) {
+    BK_CHECK(c, c->kind == BK_SH2D_PERIODIC, "BK_PC_SH_FFT needs a BK_SH2D_PERIODIC context");
+    BK_CHECK(c, a0 > 0, "BK_PC_SH_FFT: a0 must be > 0 (the symbol of L1 vanishes at |k| = 1)");
+    // tables and work buffers are the context's own (bk_periodic_setup)
   } else if (kind == BK_PC_CGL_DST) {
     BK_CHECK(c, c->kind == BK_CGL2D || c->kind == BK_POTRAP_CGL2D, "BK_PC_CGL_DST needs a cGL context");
     for (int d = 0; d < 2; ++d) {
@@ -502,6 +572,18 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
       BK_TRY(transform_pass(c, 1, 1, cur, oth, nx, ny, nz, true));
       BK_TRY(transform_pass(c, 0, 1, oth, out, nx, ny, nz, al));
     }
+  } else if (pc.kind == BK_PC_SH_FFT) {
+    const double* ts = nullptr;
+    double* td = nullptr;
+    int tn = 0;
+    if (n > N && n - N <= 32) {  // border entries ride along with the y pass
+      ts = in + N;
+      td = out + N;
+      tn = (int)(n - N);
+      tail_done = true;
+    }
+    const PerPw pw{0, PW_NONE, in, nullptr, nullptr, 0.0, 0.0, 0.0, 0.0, 0.0};
+    BK_TRY(periodic_pipeline(c, in, out, pw, false, 1.0, pc.a0, ts, td, tn));
   } else if (pc.kind == BK_PC_CGL_DST) {
     const int nx = (int)c->dims[0], ny = (int)c->dims[1];
     const long long nblk = (c->kind == BK_POTRAP_CGL2D) ? 2 * c->dims[2] : 2;  // components x slices

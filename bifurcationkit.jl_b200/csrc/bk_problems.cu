@@ -389,6 +389,8 @@ static int launch_kind(bk_ctx* c, const OpDesc& op, const double* in, const doub
       k_sh_apply<3, MODE><<<sh_num_tiles<3>(op.nx, op.ny, op.nz), BK_THREADS, ShSmem<3>::BYTES, c->stream>>>(op, in, sp, out);
       break;
     }
+    case BK_SH2D_PERIODIC:  // spectral: three transform kernels (bk_precond.cu), which count their own launches
+      return MODE == 1 ? bk_periodic_residual(c, op, in, out) : bk_periodic_jvp(c, op, in, sp, out);
     case BK_CHAN: k_chan_apply<MODE><<<lin_grid(c, op.nx), 256, 0, c->stream>>>(op, in, sp, out); break;
     case BK_CGL2D: k_cgl_apply<MODE><<<lin_grid(c, (long long)op.nx * op.ny), 256, 0, c->stream>>>(op, in, sp, out); break;
     case BK_POTRAP_CGL2D: {
@@ -426,7 +428,9 @@ static __global__ void __launch_bounds__(256) k_cshift(double* __restrict__ out,
 }
 
 int bk_launch_apply(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* out) {
-  if (op.transpose) BK_CHECK(c, op.kind == BK_SH2D || op.kind == BK_SH3D || op.kind == BK_CGL2D, "J' is not available for this problem kind");
+  if (op.transpose)
+    BK_CHECK(c, op.kind == BK_SH2D || op.kind == BK_SH3D || op.kind == BK_SH2D_PERIODIC || op.kind == BK_CGL2D,
+             "J' is not available for this problem kind");
   if (op.cplx) {
     // ((a0 + i a0i) I + a1 J)(x + i y): the real operator on both halves, then the cross terms of the imaginary shift
     OpDesc half = op;
@@ -495,7 +499,8 @@ extern "C" int32_t bk_jac_set_shift_imag(bk_ctx* c, double a0_imag) {
 
 extern "C" int32_t bk_jac_set_transpose(bk_ctx* c, int32_t on) {
   BK_ENTER(c);
-  BK_CHECK(c, !on || c->kind == BK_SH2D || c->kind == BK_SH3D || c->kind == BK_CGL2D, "J' is not available for this problem kind");
+  BK_CHECK(c, !on || c->kind == BK_SH2D || c->kind == BK_SH3D || c->kind == BK_SH2D_PERIODIC || c->kind == BK_CGL2D,
+           "J' is not available for this problem kind");
   c->transpose = on != 0;
   return BK_OK;
 }

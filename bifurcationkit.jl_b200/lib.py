@@ -12,9 +12,9 @@ LIB_PATH = os.path.join(_HERE, "libbk200.so")
 CSRC = os.path.join(_HERE, "csrc")
 
 BK_OK, BK_NOT_CONVERGED = 0, 1
-BK_CHAN, BK_SH2D, BK_SH3D, BK_CGL2D, BK_POTRAP_CGL2D = 1, 2, 3, 4, 5
+BK_CHAN, BK_SH2D, BK_SH3D, BK_CGL2D, BK_POTRAP_CGL2D, BK_SH2D_PERIODIC = 1, 2, 3, 4, 5, 6
 BK_COMPLEX = 0x100  # OR-ed into the kind: complexified context, vectors [re; im]
-BK_PC_NONE, BK_PC_SH_DCT, BK_PC_CHAN_TRIDIAG, BK_PC_CGL_DST, BK_PC_POTRAP_CIRC = 0, 1, 2, 3, 4
+BK_PC_NONE, BK_PC_SH_DCT, BK_PC_CHAN_TRIDIAG, BK_PC_CGL_DST, BK_PC_POTRAP_CIRC, BK_PC_SH_FFT = 0, 1, 2, 3, 4, 5
 BK_SIDE_NONE, BK_SIDE_LEFT, BK_SIDE_RIGHT = 0, 1, 2
 BK_ORTH_CGS, BK_ORTH_CGS2 = 0, 1
 

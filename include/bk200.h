@@ -39,6 +39,11 @@ enum {
   BK_SH3D = 3,   /* examples/SH3d.jl:16-53           params (l, nu)                  dims (Nx,Ny,Nz) */
   BK_CGL2D = 4,  /* examples/cGL2d.jl:6-22,262-318   params (r, mu, nu, c3, c5)      dims (Nx,Ny), N = 2 Nx Ny */
   BK_POTRAP_CGL2D = 5, /* src/periodicorbit/PeriodicOrbitTrapeze.jl:209-330 over BK_CGL2D; dims (Nx,Ny,M), N = 2 Nx Ny M + 1 */
+  /* examples/SH2d-fronts-cuda.jl:46-61,104-108  params (l, nu)  dims (Nx,Ny), N = Nx Ny: periodic Swift-Hohenberg,
+   * F = -L1 u + l u + nu u^2 - u^3 with L1 = (I + Lap_periodic)^2 applied spectrally (symbol (1 - kx^2 - ky^2)^2, kx = pi k / lx;
+   * the example's L is L1 + I).  Same layout and lengths as BK_SH2D: domain [-lx, lx), h = 2 lx / Nx.  Nx and Ny must be powers
+   * of two from 64 to 2048 (BK_ERR_ARG otherwise).  Every operator application is three transform kernels (bk_fft_fast.cuh). */
+  BK_SH2D_PERIODIC = 6,
   /* OR-ed into one of the kinds above (not BK_POTRAP_CGL2D): a COMPLEXIFIED context for the complex shifts of the Hopf
    * minimally augmented system (src/codim2/MinAugHopf.jl:19-40, shift = Complex(0, -omega)) and complex eigenvector work.
    * Unknowns are z = x + i y stored split, [x; y]: bk_problem_size = 2 N0, with N0 = bk_state_size the size of the real
@@ -56,9 +61,11 @@ enum {
   BK_PC_SH_DCT = 1,     /* (L1 + shift I)^-1 by separable DCT-II (exact for the Neumann-closure operator) */
   BK_PC_CHAN_TRIDIAG = 2, /* lu(P), P = tridiagonal Laplacian with identity boundary rows (chan.jl:108-109) */
   BK_PC_CGL_DST = 3,    /* per-component (a0 I + a1 Lap_dirichlet)^-1 by DST-I (block Jacobi over slices) */
-  BK_PC_POTRAP_CIRC = 4 /* Trapeze PO Jacobian of cGL linearised at the trivial state: DST-I in space (mixed-radix FFT of the odd extension, bk_fft_gen.cuh),
+  BK_PC_POTRAP_CIRC = 4,/* Trapeze PO Jacobian of cGL linearised at the trivial state: DST-I in space (mixed-radix FFT of the odd extension, bk_fft_gen.cuh),
                            u1 +- i u2, DFT over the M-1 cyclic slices, scalar symbol; a0 = period T.  Stand-in for the ILU
                            of the assembled PO Jacobian (examples/cGL2d.jl:209-213) */
+  BK_PC_SH_FFT = 5      /* BK_SH2D_PERIODIC only: (L1 + a0 I)^-1 by real 2-D FFT, a0 > 0 (the symbol of L1 vanishes at |k| = 1); the
+                           example's L^-1 is a0 = 1 (examples/SH2d-fronts-cuda.jl:64,77-90) */
 };
 enum { BK_SIDE_NONE = 0, BK_SIDE_LEFT = 1, BK_SIDE_RIGHT = 2 };
 enum { BK_ORTH_CGS = 0, BK_ORTH_CGS2 = 1 };
@@ -72,7 +79,11 @@ typedef struct bk_gmres_opts {
   int32_t pc_side; /* BK_SIDE_*: which of Pl / Pr holds the context's preconditioner */
   int32_t orth;    /* BK_ORTH_CGS (single classical Gram-Schmidt pass) or BK_ORTH_CGS2 */
   int32_t fused;   /* 0: separate kernels; nonzero: JVP fused into the Arnoldi dot kernel where a fused kernel exists, i.e. real
-                      SH2d with an even nx, at most one border (the bordered map), preconditioner not on the left */
+                      SH2d with an even nx, at most one border (the bordered map), preconditioner not on the left.
+                      BK_SH2D_PERIODIC with BK_PC_SH_FFT on either side: operator and preconditioner in ONE transform per
+                      Arnoldi step, P (a0 I + a1 J) v = P (d v) - a1 v or (a0 I + a1 J) P v = d (P v) - a1 v with
+                      d = a0 + a1 (pc a0 + l + 2 nu u - 3 u^2); unbordered real solves only (bordered and BK_COMPLEX solves run
+                      the separate kernels) */
   int32_t reserved;
 } bk_gmres_opts;
 
@@ -129,11 +140,11 @@ int32_t bk_jvp(bk_ctx* ctx, const double* v, double* out, double a0, double a1);
 /* BK_COMPLEX contexts: imaginary part of the shift a0 of every later operator application (default 0) */
 int32_t bk_jac_set_shift_imag(bk_ctx* ctx, double a0_imag);
 /* apply J' instead of J from now on: apply_jacobian(prob, x, par, dx, true) / jacobian_adjoint (src/codim2/MinAugHopf.jl:79-81,
- * 152-155).  SH2d / SH3d are self-adjoint (no-op), cGL2d transposes its 2 x 2 reaction block; BK_CHAN / BK_POTRAP_CGL2D: error */
+ * 152-155).  SH2d / SH3d / periodic SH2d are self-adjoint (no-op), cGL2d transposes its 2 x 2 reaction block; BK_CHAN / BK_POTRAP_CGL2D: error */
 int32_t bk_jac_set_transpose(bk_ctx* ctx, int32_t on);
 
 /* ---- K6: preconditioner --------------------------------------------------------------------- */
-int32_t bk_precond_setup(bk_ctx* ctx, int32_t kind, double a0, double a1); /* SH_DCT: (L1 + a0 I)^-1; CGL_DST: (a0 I + a1 Lap)^-1 */
+int32_t bk_precond_setup(bk_ctx* ctx, int32_t kind, double a0, double a1); /* SH_DCT, SH_FFT: (L1 + a0 I)^-1; CGL_DST: (a0 I + a1 Lap)^-1 */
 int32_t bk_precond_apply(bk_ctx* ctx, const double* in, double* out);  /* ldiv!(out, P, in) (src/Preconditioner.jl:11-37) */
 
 /* ---- S1/S2: GMRES = (l::GMRESIterativeSolvers)(J, rhs; a0, a1) (src/LinearSolver.jl:186-206, 15-19) */
@@ -230,6 +241,7 @@ int32_t bk_palc_run(bk_ctx* ctx, const bk_palc_opts* opts, const bk_gmres_opts* 
  *   BK2_E=1..8          tile height of the TMA-ring Arnoldi kernels instead of the heuristic (bk_krylov.cu::plan2)
  *   BK_NO_PDL=1         launch without programmatic dependent launch (plain stream order)
  *   BK_FFT_LOGE=2..5    complex values per thread (2^e) of the power-of-two transform kernels instead of the per-size default
+ *                       (some non-default choices spill registers in the BK_SH2D_PERIODIC kernels: correct results, not tuned)
  *   BK_FFT_NO_FAST=1    every transform through the general mixed-radix kernel (bk_fft_gen.cuh)
  *   BK_NSM=1..1024      size grids and reductions (read at bk_ctx_create) as for a device with that many SMs: changes the summation
  *                       order of every reduction, so it shows how a result depends on it */

@@ -21,8 +21,8 @@ const BK = BifurcationKit
 const VI = BK.VI
 const lib = get(ENV, "BK200_LIB", joinpath(@__DIR__, "..", "bifurcationkit.jl_b200", "libbk200.so"))
 
-const KINDS = Dict(:CHAN => 1, :SH2D => 2, :SH3D => 3, :CGL2D => 4, :POTRAP_CGL2D => 5)
-const PCS = Dict(:NONE => 0, :SH_DCT => 1, :CHAN_TRIDIAG => 2, :CGL_DST => 3, :POTRAP_CIRC => 4)
+const KINDS = Dict(:CHAN => 1, :SH2D => 2, :SH3D => 3, :CGL2D => 4, :POTRAP_CGL2D => 5, :SH2D_PERIODIC => 6)
+const PCS = Dict(:NONE => 0, :SH_DCT => 1, :CHAN_TRIDIAG => 2, :CGL_DST => 3, :POTRAP_CIRC => 4, :SH_FFT => 5)
 
 struct GmresOpts            # == bk_gmres_opts
     reltol::Cdouble; abstol::Cdouble; restart::Int32; maxiter::Int32

@@ -1,8 +1,11 @@
 """Numbers for the other BASELINE.json configs (kernel-level, CUDA-event timed):
   [1] SH2d 512^2 GMRES(100): fused JVP+Arnoldi GB/s          [4] cGL2d 512^2 Trapeze M=30: po_jvp GB/s, bordered MF GMRES it/s
   [5] SH3d 128^3: Newton to the pattern + shift-invert Arnoldi k=10 eigenpairs, s/eigensolve
+  [6] periodic spectral SH2d, the reference GPU example at its own size (examples/SH2d-fronts-cuda.jl: 512^2, lx = 16 pi,
+      ly = 8 pi / sqrt(3), (l, nu) = (-0.15, 1.3)): Newton to the hexagons, one GMRES(50) with Pl = (L1 + I)^-1 fused (one
+      transform per Arnoldi step) and unfused at equal iteration counts, the same at 1024^2, with the card and its power limit
 Prints one JSON object per config."""
-import json, os, sys, time
+import json, os, subprocess, sys, time
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -146,3 +149,45 @@ if "5" in which:
     print(json.dumps({"config": f"SH3d {n3}^3, shift-invert Arnoldi k=10 (sigma=0.1, krylovdim 40, inner GMRES rtol 1e-9)", "newton_converged": sol.converged,
                       "relax_s": t_relax, "residual_after_relaxation": relax_res, "newton_its": sol.itnewton, "newton_linear_its": sol.itlineartot, "newton_s": t_newton, "residuals": sol.residuals[-3:],
                       "eig_s": t_eig, "eig_converged": cv, "inner_solves": nops, "eigenvalues": [float(v.real) for v in vals]}), flush=True)
+
+if "6" in which:
+    def card():
+        try:
+            q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(torch.cuda.current_device())],
+                               capture_output=True, text=True, timeout=30).stdout.strip()
+        except (OSError, subprocess.TimeoutExpired):
+            q = ""
+        return {"name": torch.cuda.get_device_name(), "nvidia_smi": q}
+
+    PAR6 = (-0.15, 1.3)
+    out = {"config": "periodic SH2d (examples/SH2d-fronts-cuda.jl), GMRES(50) with Pl = (L1 + I)^-1", "card": card(),
+           "operator_bytes_per_arnoldi_step": {"fused": "64N", "unfused": "112N"}}
+    for n in (512, 1024):
+        lx, ly = 16 * np.pi * n / 512, 8 * np.pi / np.sqrt(3) * n / 512   # the example's domain at 512^2, scaled to keep sol0 periodic
+        ctx = bk.Context(bk.BK_SH2D_PERIODIC, (n, n), (lx, ly), krylov_m=50, params=PAR6)
+        ctx.precond_setup(bk.BK_PC_SH_FFT, 1.0)
+        X = -lx + 2 * lx / n * np.arange(n); Y = -ly + 2 * ly / n * np.arange(n)
+        u0 = (0.5 * (np.cos(X)[None, :] + np.cos(X / 2)[None, :] * np.cos(np.sqrt(3.0) * Y / 2)[:, None])).reshape(-1)
+        ls = bk.GMRESB200(reltol=1e-8, restart=50, maxiter=300, Pl=True)
+        prob = P.BifurcationProblemB200(ctx, ctx.to_device(u0), PAR6, lens=0)
+        ctx.sync(); t0 = time.perf_counter()
+        sol = P.newton(prob, prob.u0, PAR6[0], P.NewtonPar(tol=1e-6, max_iterations=10, linsolver=ls), P.norminf)
+        ctx.sync(); t_newton = time.perf_counter() - t0
+        J = ctx.jacobian(sol.u)
+        rhs = ctx.to_device(np.random.default_rng(6).standard_normal(n * n))
+        per = {"fused": {"us_per_iteration_rounds": []}, "unfused": {"us_per_iteration_rounds": []}}
+        for _ in range(3):                # alternate the two variants; reltol 0: exactly 50 iterations (one cycle) either way
+            for fused in (True, False):
+                g50 = bk.GMRESB200(reltol=0.0, restart=50, maxiter=50, Pl=True, fused=fused)
+                its = []
+                ms = ev_time(ctx, lambda: its.append(g50(J, rhs)[2]), reps=10, warm=2)
+                d = per["fused" if fused else "unfused"]
+                d["iterations"] = its[-1]
+                d["us_per_iteration_rounds"].append(ms * 1e3 / its[-1])
+        for d in per.values():
+            d["us_per_iteration"] = float(np.median(d["us_per_iteration_rounds"]))
+        out[f"{n}^2"] = {"newton_converged": sol.converged, "newton_its": sol.itnewton, "newton_linear_its": sol.itlineartot,
+                         "newton_s": t_newton, "norminf_u": float(sol.u.norminf()), "gmres50": per,
+                         "fused_speedup": per["unfused"]["us_per_iteration"] / per["fused"]["us_per_iteration"]}
+        del ctx, J, rhs, sol, prob
+    print(json.dumps(out), flush=True)

@@ -211,6 +211,89 @@ def fused_pair(pl, x1, x2, s1, s2):
     return unmakhoul(v.real), unmakhoul(v.imag)
 
 
+# ---- periodic transforms (BK_SH2D_PERIODIC): k_contig MODE 2 / 3 and k_strided MODE 3 -------------------------------------
+def rfft_pair(pl, x1, x2):
+    """k_contig MODE 2: two real rows form z = x1 + i x2 (natural order, no Makhoul reordering); per position the partner read
+    splits Z into X1 = (Z[k] + conj Z[n-k]) / 2, X2 = (Z[k] - conj Z[n-k]) / 2i, stored as packed half-spectra
+    [Re X0, Re X_{n/2}, Re X1, Im X1, ..., Re X_{n/2-1}, Im X_{n/2-1}]."""
+    n = pl.n
+    A, _ = pl.forward(x1 + 1j * x2)
+    P1, P2 = np.zeros(n), np.zeros(n)
+    for p in range(n):
+        k = pl.k_of_pos[p]
+        Zk, Zc = A[p], np.conj(A[pl.pos_of_k[(n - k) % n]])
+        X1, X2 = (Zk + Zc) / 2, (Zk - Zc) / 2j
+        if k == 0:
+            P1[0], P2[0] = X1.real, X2.real
+        elif k == n // 2:
+            P1[1], P2[1] = X1.real, X2.real
+        elif k < n // 2:
+            P1[2 * k], P1[2 * k + 1] = X1.real, X1.imag
+            P2[2 * k], P2[2 * k + 1] = X2.real, X2.imag
+    return P1, P2
+
+
+def unpack(P, k):
+    """X[k] of a packed half-spectrum, any 0 <= k < n (X[n-k] = conj X[k])"""
+    n = len(P)
+    kk = k if k <= n // 2 else n - k
+    if kk == 0 or kk == n // 2:
+        return complex(P[1 if kk else 0], 0.0)
+    x = complex(P[2 * kk], P[2 * kk + 1])
+    return x if k == kk else np.conj(x)
+
+
+def irfft_pair(pl, P1, P2):
+    """k_contig MODE 3 before its epilogue: Z[k] = X1[k] + i X2[k] at every position, inverse passes -> n x1, n x2"""
+    n = pl.n
+    A = np.zeros(n, dtype=complex)
+    for p in range(n):
+        k = pl.k_of_pos[p]
+        A[p] = unpack(P1, k) + 1j * unpack(P2, k)
+    v = pl.inverse(A)
+    return v.real, v.imag
+
+
+def periodic_y_pair(pl, c0, c1, s0, sn=None):
+    """k_strided MODE 3 on one column pair of length n (s includes every normalisation).  sn is None: the pair is the complex
+    line c0 + i c1 of one kx, multiplied by s0[k].  Otherwise the pair holds the two real lines kx = 0 (symbol s0) and
+    kx = Nx/2 (symbol sn): Z'[k] = ((s0 + sn)/2) Z[k] + ((s0 - sn)/2) conj Z[-k] with the partner read.  Returns n x."""
+    n = pl.n
+    A, _ = pl.forward(c0 + 1j * c1)
+    B = np.zeros(n, dtype=complex)
+    for p in range(n):
+        k = pl.k_of_pos[p]
+        if sn is None:
+            B[p] = s0[k] * A[p]
+        else:
+            Zc = np.conj(A[pl.pos_of_k[(n - k) % n]])
+            B[p] = 0.5 * (s0[k] + sn[k]) * A[p] + 0.5 * (s0[k] - sn[k]) * Zc
+    v = pl.inverse(B)
+    return v.real, v.imag
+
+
+def periodic_apply(u, sym, E):
+    """The whole BK_SH2D_PERIODIC pipeline on a (Ny, Nx) array: x r2c per row pair, y pass per column pair, x c2r per row pair.
+    sym (Ny, Nx // 2 + 1) is the symbol over (ky, kx >= 0); the result is irfft2(rfft2(u) * sym)."""
+    Ny, Nx = u.shape
+    px, py = Plan(Nx, E), Plan(Ny, E)
+    P = np.zeros((Ny, Nx))
+    for j in range(0, Ny, 2):
+        P[j], P[j + 1] = rfft_pair(px, u[j], u[j + 1])
+    Q = np.zeros_like(P)
+    scale = 1.0 / (Nx * Ny)
+    for q in range(Nx // 2):
+        if q == 0:
+            a, b = periodic_y_pair(py, P[:, 0], P[:, 1], sym[:, 0] * scale, sym[:, Nx // 2] * scale)
+        else:
+            a, b = periodic_y_pair(py, P[:, 2 * q], P[:, 2 * q + 1], sym[:, q] * scale)
+        Q[:, 2 * q], Q[:, 2 * q + 1] = a, b
+    out = np.zeros_like(u)
+    for j in range(0, Ny, 2):
+        out[j], out[j + 1] = irfft_pair(px, Q[j], Q[j + 1])
+    return out
+
+
 def wavefronts(slots):
     """128-bit accesses are served per quarter warp (8 lanes x 16 B = 128 B): wavefronts = max lanes on one 16-byte bank group"""
     tot = 0
