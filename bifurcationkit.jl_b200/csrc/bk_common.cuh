@@ -104,6 +104,56 @@ struct Precond {
   double po_r = 0, po_nu = 0, po_T = 0;
 };
 
+// What the host code needs to know about a problem kind.  N0 = fields * dims[0] * ... * dims[ndims - 1] + extra.
+struct BkKindTraits {
+  int ndims;        // grid dimensions that multiply into N0
+  int fields;       // values per grid point
+  int extra;        // unknowns behind the grid (the Trapeze period)
+  bool jac_sym;     // J symmetric: the eigensolver runs its thick-restart branch
+  bool has_jt;      // J' available (bk_jac_set_transpose)
+  bool complex_ok;  // BK_COMPLEX allowed
+  bool pow2_grid;   // Nx and Ny must be powers of two from 64 to 2048
+};
+const BkKindTraits* bk_kind_traits(int kind);  // nullptr for an unknown kind
+
+// CUDA event pairs bracketing intervals on a stream, created on first use and reused from one harvest to the next.
+struct BkEventTimer {
+  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pairs;
+  size_t used = 0;  // pairs begun since the last harvest
+  void begin(cudaStream_t st) {
+    if (used == pairs.size()) {
+      cudaEvent_t a, b;
+      cudaEventCreate(&a);
+      cudaEventCreate(&b);
+      pairs.push_back({a, b});
+    }
+    cudaEventRecord(pairs[used++].first, st);
+  }
+  void end(cudaStream_t st) { cudaEventRecord(pairs[used - 1].second, st); }
+  // adds the milliseconds of every pair begun since the last harvest to ms and returns how many there were; the stream must
+  // be idle.  A pair whose end was never recorded has no time and is not counted.
+  long long harvest(double& ms) {
+    long long k = 0;
+    for (size_t i = 0; i < used; ++i) {
+      float t = 0;
+      if (cudaEventElapsedTime(&t, pairs[i].first, pairs[i].second) == cudaSuccess) {
+        ms += t;
+        ++k;
+      }
+    }
+    used = 0;
+    return k;
+  }
+  void destroy() {
+    for (auto& p : pairs) {
+      cudaEventDestroy(p.first);
+      cudaEventDestroy(p.second);
+    }
+    pairs.clear();
+    used = 0;
+  }
+};
+
 struct bk_ctx {
   int device = 0;
   int nsm = BK_NSM_FALLBACK;
@@ -166,10 +216,8 @@ struct bk_ctx {
   int timing_every = 1;     // ... of every timing_every-th bk_gmres call only (event records sit between PDL launches: sampling keeps the overhead small)
   long long solve_count = 0;
   bool timing_now = false;  // decided per solve
-  cudaEvent_t tev0 = nullptr, tev1 = nullptr;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> tpairs;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pc_pairs;  // one pair per preconditioner application (timing enabled)
-  size_t pc_pairs_used = 0;
+  BkEventTimer fused_timer; // the Arnoldi kernels of one solve (bk_gmres_dev)
+  BkEventTimer pc_timer;    // one pair per preconditioner application, read back at the end of a solve and in bk_get_stats
   // dynamic shared memory this context has already asked for, per kernel (first-level filter in front of bk_grant_smem)
   std::unordered_map<const void*, size_t> smem_attr;
   std::string err;
@@ -201,6 +249,19 @@ int bk_fail(bk_ctx* c, int code, const char* what, const char* file, int line);
   } while (0)
 
 // ---- host-side internal API (cross-TU) ----------------------------------------------------------
+// Grid of the 256-thread grid-stride kernels: one CTA per 256 values, at most 8 per SM.  It fixes the summation order of every
+// k_reduce / k_tail reduction, and with it the rounding of the continuation (DESIGN.md §7).
+static inline int bk_lin_grid(const bk_ctx* c, long long n) {
+  long long g = (n + 255) / 256;
+  long long cap = (long long)c->nsm * 8;
+  return (int)(g < cap ? (g > 0 ? g : 1) : cap);
+}
+// 1/h^2 along dimension d, with h = 2 l / n in every example (SH2d-fronts.jl:14-15, SH3d.jl:18-20, cGL2d.jl:7-8)
+static inline double bk_inv_h2(const bk_ctx* c, int d) {
+  const double h = 2 * c->lengths[d] / c->dims[d];
+  return 1.0 / (h * h);
+}
+
 bool bk_is_device_ptr(const void* p);
 // Returns a device pointer for argument p (n doubles): p itself when device memory, else stage slot `slot`
 // filled by H2D (when `in`).  For outputs call bk_stage_out afterwards.
@@ -215,7 +276,6 @@ int bk_launch_apply(bk_ctx* c, const OpDesc& op, const double* in_dev, const dou
 int bk_potrap_refresh_cache(bk_ctx* c);
 
 int bk_precond_apply_dev(bk_ctx* c, const double* in_dev, double* out_dev, long long n);
-void bk_harvest_pc_timing(bk_ctx* c);
 
 // BK_SH2D_PERIODIC (bk_precond.cu): transform tables and work buffers at bk_ctx_create, then the three-kernel spectral pipeline
 // x r2c -> y (forward, symbol, inverse) -> x c2r for the residual, the JVP and the one-transform preconditioned operator
@@ -277,6 +337,15 @@ static inline cudaError_t bk_launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 
   if (no_pdl < 0) no_pdl = getenv("BK_NO_PDL") ? 1 : 0;
   cfg.numAttrs = no_pdl ? 0 : 1;
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
+}
+// grant `smem` bytes of dynamic shared memory to kern, launch it with PDL on the context's stream, check and count the launch
+template <typename... KArgs, typename... Args>
+static inline int bk_launch(bk_ctx* c, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, Args&&... args) {
+  bk_ensure_smem(c, kern, smem);
+  bk_launch_pdl(kern, grid, block, smem, c->stream, static_cast<Args&&>(args)...);
+  BK_CUDA(c, cudaGetLastError());
+  c->stats.kernel_launches++;
+  return BK_OK;
 }
 // first statement of every kernel launched through bk_launch_pdl: wait for the previous grid's memory, then let the next
 // grid start launching (its CTAs block at their own wait)

@@ -71,6 +71,20 @@ int bk_tmp(bk_ctx* c, int slot, double** out) {
   return BK_OK;
 }
 
+const BkKindTraits* bk_kind_traits(int kind) {
+  //                                   ndims fields extra jac_sym has_jt complex_ok pow2_grid
+  static const BkKindTraits table[] = {{0, 0, 0, false, false, false, false},  // 0: not a kind
+                                       {1, 1, 0, false, false, true, false},   // BK_CHAN
+                                       {2, 1, 0, true, true, true, false},     // BK_SH2D
+                                       {3, 1, 0, true, true, true, false},     // BK_SH3D
+                                       {2, 2, 0, false, true, true, false},    // BK_CGL2D
+                                       {3, 2, 1, false, false, false, false},  // BK_POTRAP_CGL2D
+                                       {2, 1, 0, true, true, true, true}};     // BK_SH2D_PERIODIC
+  static_assert(BK_CHAN == 1 && BK_POTRAP_CGL2D == 5 && BK_SH2D_PERIODIC == 6, "the table is indexed by kind");
+  if (kind < BK_CHAN || kind > BK_SH2D_PERIODIC) return nullptr;
+  return &table[kind];
+}
+
 extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dims[3], const double lengths[3],
                                  int32_t krylov_m, bk_ctx** out) {
   if (!out) return BK_ERR_ARG;
@@ -86,26 +100,20 @@ extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dim
     c->dims[i] = dims ? (dims[i] > 0 ? dims[i] : 1) : 1;
     c->lengths[i] = lengths ? lengths[i] : 1.0;
   }
-  long long n = 0;
-  switch (kind) {
-    case BK_CHAN: n = c->dims[0]; break;
-    case BK_SH2D: n = c->dims[0] * c->dims[1]; break;
-    case BK_SH2D_PERIODIC:
-      for (int d = 0; d < 2; ++d) {
-        const long long v = c->dims[d];
-        BK_CHECK(c, v >= 64 && v <= 2048 && (v & (v - 1)) == 0,
-                 "BK_SH2D_PERIODIC: Nx and Ny must be powers of two from 64 to 2048");
-      }
-      n = c->dims[0] * c->dims[1];
-      break;
-    case BK_SH3D: n = c->dims[0] * c->dims[1] * c->dims[2]; break;
-    case BK_CGL2D: n = 2 * c->dims[0] * c->dims[1]; break;
-    case BK_POTRAP_CGL2D: n = 2 * c->dims[0] * c->dims[1] * c->dims[2] + 1; break;
-    default: return bk_fail(c, BK_ERR_ARG, "unknown problem kind", __FILE__, __LINE__);
-  }
+  const BkKindTraits* kt = bk_kind_traits(kind);
+  if (!kt) return bk_fail(c, BK_ERR_ARG, "unknown problem kind", __FILE__, __LINE__);
+  if (kt->pow2_grid)
+    for (int d = 0; d < 2; ++d) {
+      const long long v = c->dims[d];
+      BK_CHECK(c, v >= 64 && v <= 2048 && (v & (v - 1)) == 0,
+               "BK_SH2D_PERIODIC: Nx and Ny must be powers of two from 64 to 2048");
+    }
+  long long n = kt->fields;
+  for (int d = 0; d < kt->ndims; ++d) n *= c->dims[d];
+  n += kt->extra;
   BK_CHECK(c, n >= 2, "problem too small");
   BK_CHECK(c, krylov_m >= 1 && krylov_m <= 1024, "krylov_m out of range");
-  BK_CHECK(c, !(c->cplx && kind == BK_POTRAP_CGL2D), "BK_COMPLEX is not available for the periodic-orbit functional");
+  BK_CHECK(c, !c->cplx || kt->complex_ok, "BK_COMPLEX is not available for the periodic-orbit functional");
   c->N0 = n;
   if (c->cplx) n *= 2;  // [re; im]
   c->N = n;
@@ -155,8 +163,6 @@ extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dim
   BK_CUDA(c, cudaMallocHost(&c->coef_pinned, 8 * (m + 4)));
   c->events.resize(m + 2);
   for (auto& e : c->events) BK_CUDA(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  BK_CUDA(c, cudaEventCreate(&c->tev0));
-  BK_CUDA(c, cudaEventCreate(&c->tev1));
   if (kind == BK_POTRAP_CGL2D) {
     BK_CUDA(c, cudaMalloc(&c->phi, 8 * ld));
     BK_CUDA(c, cudaMalloc(&c->xpi, 8 * ld));
@@ -182,10 +188,6 @@ extern "C" int32_t bk_ctx_destroy(bk_ctx* c) {
     for (void* t : tabs)
       if (t) cudaFree(t);
   }
-  for (auto& p : c->pc_pairs) {
-    cudaEventDestroy(p.first);
-    cudaEventDestroy(p.second);
-  }
   if (c->pc.tdft) cudaFree(c->pc.tdft);
   if (c->counters) cudaFree(c->counters);
   for (auto& kv : c->vec_live) cudaFree(kv.first);
@@ -200,12 +202,8 @@ extern "C" int32_t bk_ctx_destroy(bk_ctx* c) {
   if (c->eig_pinned) cudaFreeHost(c->eig_pinned);
   for (auto& e : c->events)
     if (e) cudaEventDestroy(e);
-  for (auto& p : c->tpairs) {
-    cudaEventDestroy(p.first);
-    cudaEventDestroy(p.second);
-  }
-  if (c->tev0) cudaEventDestroy(c->tev0);
-  if (c->tev1) cudaEventDestroy(c->tev1);
+  c->fused_timer.destroy();
+  c->pc_timer.destroy();
   if (c->stream) cudaStreamDestroy(c->stream);
   delete c;
   return BK_OK;
@@ -220,24 +218,12 @@ extern "C" int32_t bk_set_params(bk_ctx* c, const double* p, int32_t n) {
   for (int i = 0; i < n; ++i) c->par[i] = p[i];
   return BK_OK;
 }
-// sum the per-application event pairs recorded by bk_precond_apply_dev (timing enabled); the stream must be idle
-void bk_harvest_pc_timing(bk_ctx* c) {
-  for (size_t i = 0; i < c->pc_pairs_used; ++i) {
-    float t = 0;
-    if (cudaEventElapsedTime(&t, c->pc_pairs[i].first, c->pc_pairs[i].second) == cudaSuccess) {
-      c->stats.total_precond_ms += t;
-      c->stats.total_precond_applies++;
-    }
-  }
-  c->pc_pairs_used = 0;
-}
-
 extern "C" int32_t bk_get_stats(bk_ctx* c, bk_stats* out) {
   BK_ENTER(c);
   if (!out) return BK_ERR_ARG;
-  if (c->pc_pairs_used) {
+  if (c->pc_timer.used) {
     BK_CUDA(c, cudaStreamSynchronize(c->stream));
-    bk_harvest_pc_timing(c);
+    c->stats.total_precond_applies += c->pc_timer.harvest(c->stats.total_precond_ms);
   }
   *out = c->stats;
   return BK_OK;
@@ -343,20 +329,14 @@ static __global__ void __launch_bounds__(256) k_scale(double* __restrict__ x, do
   for (; i < n; i += stride) x[i] *= a;
 }
 
-static inline int ew_grid(bk_ctx* c, long long n) {
-  long long g = (n + 255) / 256;
-  long long cap = (long long)c->nsm * 8;
-  return (int)(g < cap ? (g > 0 ? g : 1) : cap);
-}
-
 int bk_dev_axpby(bk_ctx* c, double* y, double a, const double* x, double b, long long n) {
-  k_axpby<<<ew_grid(c, n), 256, 0, c->stream>>>(y, a, x, b, n);
+  k_axpby<<<bk_lin_grid(c, n), 256, 0, c->stream>>>(y, a, x, b, n);
   c->stats.kernel_launches++;
   BK_CUDA(c, cudaGetLastError());
   return BK_OK;
 }
 int bk_dev_scale(bk_ctx* c, double* x, double a, long long n) {
-  k_scale<<<ew_grid(c, n), 256, 0, c->stream>>>(x, a, n);
+  k_scale<<<bk_lin_grid(c, n), 256, 0, c->stream>>>(x, a, n);
   c->stats.kernel_launches++;
   BK_CUDA(c, cudaGetLastError());
   return BK_OK;
@@ -406,7 +386,7 @@ static __global__ void __launch_bounds__(256) k_reduce(const double* __restrict_
 
 template <int MODE>
 static int reduce_launch(bk_ctx* c, const double* x, const double* y, const double* x0, long long n, double* out_host) {
-  int g = ew_grid(c, n);
+  int g = bk_lin_grid(c, n);
   if (g > c->gmax) g = c->gmax;
   k_reduce<MODE><<<g, 256, 0, c->stream>>>(x, y, x0, n, c->partials, c->counters + 8, c->red_out);
   c->stats.kernel_launches++;

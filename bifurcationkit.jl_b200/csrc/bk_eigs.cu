@@ -231,6 +231,64 @@ static __global__ void k_start_vector(double* v, long long n) {
   }
 }
 
+// Arnoldi workspace of the eigensolver: slots of S = m + 4 doubles in c->eig_dev and the pinned host mirror c->eig_pinned
+struct EigWork {
+  int S;
+  double* ones;  // all ones: the basis Q is stored normalised
+  double* hA;    // H column of the first Gram-Schmidt pass, followed by hB
+  double* hB;    // second-pass corrections
+  double* gco;   // dot-product coefficients handed from k2_dots to k2_update
+  double* coef;  // 2 S: lincomb coefficients
+  double* hp;    // pinned host copy of hA | hB
+};
+
+// Q_0 = x / ||x||
+static int arnoldi_start(bk_ctx* c, const EigWork& ws, const double* x, long long n) {
+  BK_TRY(bk_launch_update(c, c->Q, ws.gco, x, n, 0, c->Q, ws.hA, ws.hB));
+  BK_CUDA(c, cudaMemcpyAsync(ws.hp, ws.hA, 8, cudaMemcpyDeviceToHost, c->stream));
+  BK_CUDA(c, cudaStreamSynchronize(c->stream));
+  BK_CHECK(c, ws.hp[0] > 0, "zero start vector");
+  BK_TRY(bk_dev_scale(c, c->Q, 1.0 / ws.hp[0], n));
+  return BK_OK;
+}
+
+// Arnoldi expansion of columns kstart..m-1 of H ((m + 1) x m, column-major): Q_{k+1} from one inner solve x = (J - sigma)^-1 Q_k
+// and two classical Gram-Schmidt passes.  Stops early at an invariant subspace; *keff is the number of columns of H filled.
+// Adds the inner solves to *nops.
+static int arnoldi_expand(bk_ctx* c, const EigWork& ws, const OpDesc& op, const bk_gmres_opts* inner, double* x, long long n,
+                          int m, int kstart, std::vector<double>& H, int* keff, int* nops) {
+  const int S = ws.S;
+  *keff = m;
+  for (int k = kstart; k < m; ++k) {
+    const int j = k + 1;
+    int cv = 0, it = 0;
+    int st = bk_gmres_dev(c, op, c->Q + (size_t)k * c->ld, x, inner, &cv, &it, nullptr);
+    if (st < 0) return st;
+    ++*nops;
+    double* qn = c->Q + (size_t)(k + 1) * c->ld;
+    BK_TRY(bk_launch_dots(c, c->Q, ws.ones, x, n, j, ws.hA, ws.gco));
+    BK_TRY(bk_launch_update(c, c->Q, ws.gco, x, n, j, qn, ws.hA + j, ws.hB + S - 1));
+    BK_TRY(bk_launch_dots(c, c->Q, ws.ones, qn, n, j, ws.hB, ws.gco));
+    BK_TRY(bk_launch_update(c, c->Q, ws.gco, qn, n, j, qn, ws.hA + j, ws.hB + S - 1));
+    BK_CUDA(c, cudaMemcpyAsync(ws.hp, ws.hA, 8 * (size_t)(2 * S), cudaMemcpyDeviceToHost, c->stream));
+    BK_CUDA(c, cudaStreamSynchronize(c->stream));
+    const double* hp = ws.hp;
+    double cn = 0;
+    for (int i = 0; i < j; ++i) {
+      H[i + (size_t)k * (m + 1)] = hp[i] + hp[S + i];
+      cn = fmax(cn, fabs(H[i + (size_t)k * (m + 1)]));
+    }
+    double hk1 = hp[j];
+    H[j + (size_t)k * (m + 1)] = hk1;
+    if (!(hk1 > 1e-14 * fmax(cn, 1e-300))) {  // invariant subspace found
+      *keff = k + 1;
+      return BK_OK;
+    }
+    BK_TRY(bk_dev_scale(c, qn, 1.0 / hk1, n));
+  }
+  return BK_OK;
+}
+
 extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, int32_t krylovdim, double tol,
                                         int32_t maxrestart, const bk_gmres_opts* inner, const double* v0, double* vals_re,
                                         double* vals_im, double* vecs, int32_t* nconv, int32_t* nops) {
@@ -259,12 +317,9 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
   // partial-sum buffer must hold m rows
   BK_CHECK(c, m <= c->m, "krylovdim exceeds the context's krylov_m (partial-sum workspace)");
   const int S = m + 4;
-  double* ones = c->eig_dev;
-  double* hA = c->eig_dev + S;
-  double* hB = c->eig_dev + 2 * S;
-  double* gco = c->eig_dev + 3 * S;
-  double* coef = c->eig_dev + 4 * S;  // 2*S
-  double* hp = c->eig_pinned;
+  const EigWork ws{S, c->eig_dev, c->eig_dev + S, c->eig_dev + 2 * S, c->eig_dev + 3 * S, c->eig_dev + 4 * S, c->eig_pinned};
+  double* coef = ws.coef;
+  double* hp = ws.hp;
   double* x;
   BK_TRY(bk_tmp(c, 3, &x));
   OpDesc op = bk_make_op(c, -sigma, 1.0);  // (a0 I + a1 J) with a0 = -sigma (src/EigSolver.jl:260)
@@ -283,7 +338,7 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
   bool converged = false;
   int keff = m;
   // ---------------- symmetric operators (Swift-Hohenberg): thick-restart (Krylov-Schur with Ritz vectors) ----------------
-  const bool sym = (c->kind == BK_SH2D || c->kind == BK_SH3D || c->kind == BK_SH2D_PERIODIC);
+  const bool sym = bk_kind_traits(c->kind)->jac_sym;
   std::vector<double> Ssym, wsym;
   std::vector<int> order;
   if (sym) {
@@ -294,40 +349,10 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
       c->q2cap = m;
     }
     std::fill(H.begin(), H.end(), 0.0);
-    BK_TRY(bk_launch_update(c, c->Q, gco, x, n, 0, c->Q, hA, hB));
-    BK_CUDA(c, cudaMemcpyAsync(hp, hA, 8, cudaMemcpyDeviceToHost, c->stream));
-    BK_CUDA(c, cudaStreamSynchronize(c->stream));
-    BK_CHECK(c, hp[0] > 0, "zero start vector");
-    BK_TRY(bk_dev_scale(c, c->Q, 1.0 / hp[0], n));
+    BK_TRY(arnoldi_start(c, ws, x, n));
     int kstart = 0;
     for (int rs = 0; rs < maxrestart && !converged; ++rs) {
-      keff = m;
-      for (int k = kstart; k < m; ++k) {
-        const int j = k + 1;
-        int cv = 0, it = 0;
-        int st = bk_gmres_dev(c, op, c->Q + (size_t)k * c->ld, x, inner, &cv, &it, nullptr);
-        if (st < 0) return st;
-        ++total_ops;
-        double* qn = c->Q + (size_t)(k + 1) * c->ld;
-        BK_TRY(bk_launch_dots(c, c->Q, ones, x, n, j, hA, gco));
-        BK_TRY(bk_launch_update(c, c->Q, gco, x, n, j, qn, hA + j, hB + S - 1));
-        BK_TRY(bk_launch_dots(c, c->Q, ones, qn, n, j, hB, gco));
-        BK_TRY(bk_launch_update(c, c->Q, gco, qn, n, j, qn, hA + j, hB + S - 1));
-        BK_CUDA(c, cudaMemcpyAsync(hp, hA, 8 * (size_t)(2 * S), cudaMemcpyDeviceToHost, c->stream));
-        BK_CUDA(c, cudaStreamSynchronize(c->stream));
-        double cn = 0;
-        for (int i = 0; i < j; ++i) {
-          H[i + (size_t)k * (m + 1)] = hp[i] + hp[S + i];
-          cn = fmax(cn, fabs(H[i + (size_t)k * (m + 1)]));
-        }
-        double hk1 = hp[j];
-        H[j + (size_t)k * (m + 1)] = hk1;
-        if (!(hk1 > 1e-14 * fmax(cn, 1e-300))) {
-          keff = k + 1;
-          break;
-        }
-        BK_TRY(bk_dev_scale(c, qn, 1.0 / hk1, n));
-      }
+      BK_TRY(arnoldi_expand(c, ws, op, inner, x, n, m, kstart, H, &keff, &total_ops));
       // symmetrised projected matrix (exactly symmetric in exact arithmetic)
       std::vector<double> A((size_t)keff * keff);
       for (int jj = 0; jj < keff; ++jj)
@@ -384,39 +409,8 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
   }
   for (int rs = 0; !sym && rs < maxrestart && !converged; ++rs) {
     std::fill(H.begin(), H.end(), 0.0);
-    // Q_0 = x / ||x||
-    BK_TRY(bk_launch_update(c, c->Q, gco, x, n, 0, c->Q, hA, hB));
-    BK_CUDA(c, cudaMemcpyAsync(hp, hA, 8, cudaMemcpyDeviceToHost, c->stream));
-    BK_CUDA(c, cudaStreamSynchronize(c->stream));
-    BK_CHECK(c, hp[0] > 0, "zero start vector");
-    BK_TRY(bk_dev_scale(c, c->Q, 1.0 / hp[0], n));
-    keff = m;
-    for (int k = 0; k < m; ++k) {
-      const int j = k + 1;
-      int cv = 0, it = 0;
-      int st = bk_gmres_dev(c, op, c->Q + (size_t)k * c->ld, x, inner, &cv, &it, nullptr);
-      if (st < 0) return st;
-      ++total_ops;
-      double* qn = c->Q + (size_t)(k + 1) * c->ld;
-      BK_TRY(bk_launch_dots(c, c->Q, ones, x, n, j, hA, gco));
-      BK_TRY(bk_launch_update(c, c->Q, gco, x, n, j, qn, hA + j, hB + S - 1));
-      BK_TRY(bk_launch_dots(c, c->Q, ones, qn, n, j, hB, gco));
-      BK_TRY(bk_launch_update(c, c->Q, gco, qn, n, j, qn, hA + j, hB + S - 1));
-      BK_CUDA(c, cudaMemcpyAsync(hp, hA, 8 * (size_t)(2 * S), cudaMemcpyDeviceToHost, c->stream));
-      BK_CUDA(c, cudaStreamSynchronize(c->stream));
-      double cn = 0;
-      for (int i = 0; i < j; ++i) {
-        H[i + (size_t)k * (m + 1)] = hp[i] + hp[S + i];
-        cn = fmax(cn, fabs(H[i + (size_t)k * (m + 1)]));
-      }
-      double hk1 = hp[j];
-      H[j + (size_t)k * (m + 1)] = hk1;
-      if (!(hk1 > 1e-14 * fmax(cn, 1e-300))) {  // invariant subspace found
-        keff = k + 1;
-        break;
-      }
-      BK_TRY(bk_dev_scale(c, qn, 1.0 / hk1, n));
-    }
+    BK_TRY(arnoldi_start(c, ws, x, n));
+    BK_TRY(arnoldi_expand(c, ws, op, inner, x, n, m, 0, H, &keff, &total_ops));
     // Ritz values / vectors of H(keff x keff)
     BK_CHECK(c, hess_eigvals(H, keff, m + 1, ev), "QR iteration on the Hessenberg matrix did not converge");
     std::sort(ev.begin(), ev.end(), [](const cplx& a, const cplx& b) {

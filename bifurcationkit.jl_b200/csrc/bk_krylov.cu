@@ -147,22 +147,11 @@ static int launch_fused(bk_ctx* c, const OpDesc& op, const double* in, const dou
   Plan2 p = plan2(c, (long long)tiles_x * op.ny, sh2_scratch_bytes);
   p.grid = tiles_x * ((op.ny + p.E - 1) / p.E);
   BK_CHECK(c, p.grid <= c->gmax, "partial-sum workspace too small for the fused grid");  // dots_finish indexes partials by CTA
-  if (op.bordered) {
-    BK2_DISPATCH(p.E, {
-      bk_ensure_smem(c, k2_fused<EE, true>, p.smem);
-      bk_launch_pdl(k2_fused<EE, true>, dim3(p.grid), dim3(BK2_THREADS), p.smem, c->stream, op, in, sp, w, c->V, c->ld, j, c->scales, c->partials,
-                                                                     c->counters + 0, hcol, c->gcoef, p.NS, p.sred_off);
-    });
-  } else {
-    BK2_DISPATCH(p.E, {
-      bk_ensure_smem(c, k2_fused<EE, false>, p.smem);
-      bk_launch_pdl(k2_fused<EE, false>, dim3(p.grid), dim3(BK2_THREADS), p.smem, c->stream, op, in, sp, w, c->V, c->ld, j, c->scales, c->partials,
-                                                                      c->counters + 0, hcol, c->gcoef, p.NS, p.sred_off);
-    });
-  }
-  c->stats.kernel_launches++;
-  BK_CUDA(c, cudaGetLastError());
-  return BK_OK;
+  BK2_DISPATCH(p.E, {
+    auto kern = op.bordered ? k2_fused<EE, true> : k2_fused<EE, false>;
+    return bk_launch(c, kern, dim3(p.grid), dim3(BK2_THREADS), p.smem, op, in, sp, w, c->V, c->ld, j, c->scales, c->partials,
+                     c->counters + 0, hcol, c->gcoef, p.NS, p.sred_off);
+  });
 }
 
 // ------------------------------------------------------------------------------------------------ host
@@ -172,14 +161,8 @@ int bk_launch_dots(bk_ctx* c, const double* basis, const double* scales, const d
                    double* gcoef) {
   Plan2 p = plan2(c, (n + BK2_ROW - 1) / BK2_ROW, nullptr);
   BK_CHECK(c, p.grid <= c->gmax, "partial-sum workspace too small");
-  BK2_DISPATCH(p.E, {
-    bk_ensure_smem(c, k2_dots<EE>, p.smem);
-    bk_launch_pdl(k2_dots<EE>, dim3(p.grid), dim3(BK2_THREADS), p.smem, c->stream, w, n, basis, c->ld, j, scales, c->partials, c->counters + 1, hcol,
-                                                            gcoef, p.NS, p.sred_off);
-  });
-  c->stats.kernel_launches++;
-  BK_CUDA(c, cudaGetLastError());
-  return BK_OK;
+  BK2_DISPATCH(p.E, return bk_launch(c, k2_dots<EE>, dim3(p.grid), dim3(BK2_THREADS), p.smem, w, n, basis, c->ld, j, scales,
+                                     c->partials, c->counters + 1, hcol, gcoef, p.NS, p.sred_off));
 }
 static int launch_dots(bk_ctx* c, const double* w, long long n, int j, double* hcol) {
   return bk_launch_dots(c, c->V, c->scales, w, n, j, hcol, c->gcoef);
@@ -189,14 +172,8 @@ int bk_launch_update(bk_ctx* c, const double* basis, const double* gcoef, const 
                      double* h_out, double* scale_out) {
   Plan2 p = plan2(c, (n + BK2_ROW - 1) / BK2_ROW, nullptr);
   BK_CHECK(c, p.grid <= c->gmax, "partial-sum workspace too small");
-  BK2_DISPATCH(p.E, {
-    bk_ensure_smem(c, k2_update<EE>, p.smem);
-    bk_launch_pdl(k2_update<EE>, dim3(p.grid), dim3(BK2_THREADS), p.smem, c->stream, w, n, basis, c->ld, j, gcoef, vout, c->partials,
-                                                              c->counters + 2, h_out, scale_out, p.NS);
-  });
-  c->stats.kernel_launches++;
-  BK_CUDA(c, cudaGetLastError());
-  return BK_OK;
+  BK2_DISPATCH(p.E, return bk_launch(c, k2_update<EE>, dim3(p.grid), dim3(BK2_THREADS), p.smem, w, n, basis, c->ld, j, gcoef, vout,
+                                     c->partials, c->counters + 2, h_out, scale_out, p.NS));
 }
 static int launch_update(bk_ctx* c, const double* w, long long n, int j, double* vout, double* h_out, double* scale_out) {
   return bk_launch_update(c, c->V, c->gcoef, w, n, j, vout, h_out, scale_out);
@@ -213,31 +190,9 @@ static int launch_lincomb(bk_ctx* c, double* x, double beta, long long n, int k,
   return bk_launch_lincomb(c, c->V, use_scales ? c->scales : nullptr, x, beta, n, k, coef_dev);
 }
 
-struct TimerScope {
-  bk_ctx* c;
-  size_t idx;
-  bool on;
-  TimerScope(bk_ctx* c_) : c(c_), idx(0), on(c_->timing_now) {}
-  void begin(size_t i) {
-    if (!on) return;
-    idx = i;
-    while (c->tpairs.size() <= i) {
-      cudaEvent_t a, b;
-      cudaEventCreate(&a);
-      cudaEventCreate(&b);
-      c->tpairs.push_back({a, b});
-    }
-    cudaEventRecord(c->tpairs[i].first, c->stream);
-  }
-  void end() {
-    if (on) cudaEventRecord(c->tpairs[idx].second, c->stream);
-  }
-};
-
 // One Arnoldi step k (0-based): basis v'_0..v'_k -> v'_{k+1}, H column k on device (+ async copy to pinned host).
 // fuse: fuses_jvp() of the solve; fuse_pc: fuses_pc() of the solve.
-static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, long long n, int k, bool fuse, bool fuse_pc,
-                        size_t* timer_slot) {
+static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, long long n, int k, bool fuse, bool fuse_pc) {
   const int j = k + 1;
   const int mh = c->m + 4;
   // The H column is written by the kernels' last CTA straight into pinned, device-mapped host memory (UVA): no
@@ -252,31 +207,24 @@ static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, lon
     BK_TRY(bk_precond_apply_dev(c, in, c->z, n));
     in = c->z;
   }
-  TimerScope ts(c);
+  const bool timed = c->timing_now;
   const double* wfin = c->w;
   if (fuse_pc) {
     BK_TRY(bk_periodic_fused(c, op, in, sp, c->w, left));
-    ts.begin((*timer_slot)++);
-    BK_TRY(launch_dots(c, c->w, n, j, hcol));
-    ts.end();
-  } else if (fuse) {
-    ts.begin((*timer_slot)++);
-    BK_TRY(launch_fused(c, op, in, sp, c->w, j, hcol));
-    ts.end();
-  } else {
+  } else if (!fuse) {
     BK_TRY(bk_launch_apply(c, op, in, sp, c->w));
     if (left) {
       BK_TRY(bk_precond_apply_dev(c, c->w, c->r, n));
       wfin = c->r;
     }
-    ts.begin((*timer_slot)++);
-    BK_TRY(launch_dots(c, wfin, n, j, hcol));
-    ts.end();
   }
+  if (timed) c->fused_timer.begin(c->stream);
+  BK_TRY(fuse ? launch_fused(c, op, in, sp, c->w, j, hcol) : launch_dots(c, wfin, n, j, hcol));
+  if (timed) c->fused_timer.end(c->stream);
   double* vnext = c->V + (size_t)(k + 1) * c->ld;
-  ts.begin((*timer_slot)++);
+  if (timed) c->fused_timer.begin(c->stream);
   BK_TRY(launch_update(c, wfin, n, j, vnext, hcol + j, c->scales + k + 1));
-  ts.end();
+  if (timed) c->fused_timer.end(c->stream);
   if (o->orth == BK_ORTH_CGS2) {
     BK_TRY(launch_dots(c, vnext, n, j, hcol2));
     BK_TRY(launch_update(c, vnext, n, j, vnext, hcol + j, c->scales + k + 1));
@@ -335,7 +283,7 @@ int bk_gmres_dev(bk_ctx* c, const OpDesc& op, const double* rhs, double* x, cons
   c->stats.last_fused_ms = 0.0;
   c->solve_count++;
   c->timing_now = c->timing && (c->solve_count % c->timing_every == 0);
-  size_t timer_slot = 0;
+  c->fused_timer.used = 0;  // drop what a failed solve left behind
 
   BK_CUDA(c, cudaMemsetAsync(x, 0, 8 * (size_t)n, c->stream));  // initially_zero = true (src/LinearSolver.jl:171)
   bool x_zero = true;
@@ -380,7 +328,7 @@ int bk_gmres_dev(bk_ctx* c, const OpDesc& op, const double* rhs, double* x, cons
     while (true) {
       bool can_launch = kl < restart && (total + (kl - kd)) < maxiter && !stop;
       if (can_launch && (kl - kd) < 2) {
-        BK_TRY(arnoldi_step(c, op, o, n, kl, fuse, fuse_pc, &timer_slot));
+        BK_TRY(arnoldi_step(c, op, o, n, kl, fuse, fuse_pc));
         ++kl;
         continue;
       }
@@ -447,13 +395,10 @@ int bk_gmres_dev(bk_ctx* c, const OpDesc& op, const double* rhs, double* x, cons
     if (conv || total >= maxiter || k == 0) break;
   }
   BK_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (c->pc_pairs_used) bk_harvest_pc_timing(c);
+  c->stats.total_precond_applies += c->pc_timer.harvest(c->stats.total_precond_ms);
   if (c->timing_now) {
     double ms = 0;
-    for (size_t i = 0; i < timer_slot && i < c->tpairs.size(); ++i) {
-      float t = 0;
-      if (cudaEventElapsedTime(&t, c->tpairs[i].first, c->tpairs[i].second) == cudaSuccess) ms += t;
-    }
+    c->fused_timer.harvest(ms);
     c->stats.last_fused_ms = ms;
     if (fuse) c->stats.total_fused_ms += ms;
   }

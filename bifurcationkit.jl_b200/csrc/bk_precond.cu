@@ -130,11 +130,6 @@ static __global__ void k_thomas(const double* __restrict__ tri, const double* __
 }
 
 // ------------------------------------------------------------------------------------------------ host
-static inline int lin_grid(bk_ctx* c, long long n) {
-  long long g = (n + 255) / 256, cap = (long long)c->nsm * 8;
-  return (int)(g < cap ? (g > 0 ? g : 1) : cap);
-}
-
 static int upload(bk_ctx* c, void** dst, const void* src, size_t bytes) {
   if (*dst) cudaFree(*dst);
   *dst = nullptr;
@@ -206,34 +201,15 @@ static int fast_launch(bk_ctx* c, int d, bool strided, int mode, const double* i
   PerPw p0{};
   if (pw) p0 = *pw;
   if (strided) {
-    dim3 grid((g.nb + 2 * FC::PP - 1) / (2 * FC::PP), g.nouter);
-    if (mode == 0) {
-      bk_ensure_smem(c, bkf::k_strided<FC, 0>, FC::SMEM);
-      BK_CUDA(c, bk_launch_pdl(bkf::k_strided<FC, 0>, grid, dim3(FC::THREADS), FC::SMEM, c->stream, in, out, g, tb, s0));
-    } else if (mode == 1) {
-      bk_ensure_smem(c, bkf::k_strided<FC, 1>, FC::SMEM);
-      BK_CUDA(c, bk_launch_pdl(bkf::k_strided<FC, 1>, grid, dim3(FC::THREADS), FC::SMEM, c->stream, in, out, g, tb, s0));
-    } else if (mode == 2) {
-      bk_ensure_smem(c, bkf::k_strided<FC, 2>, FC::SMEM_FUSED);
-      BK_CUDA(c, bk_launch_pdl(bkf::k_strided<FC, 2>, grid, dim3(FC::THREADS), FC::SMEM_FUSED, c->stream, in, out, g, tb, s0));
-    } else {
-      bk_ensure_smem(c, bkf::k_strided<FC, 3>, FC::SMEM_FUSED);
-      BK_CUDA(c, bk_launch_pdl(bkf::k_strided<FC, 3>, grid, dim3(FC::THREADS), FC::SMEM_FUSED, c->stream, in, out, g, tb, s0));
-    }
-  } else {
-    dim3 grid((unsigned)((g.nb + 2 * FC::PP - 1) / (2 * FC::PP)));
-#define BKF_CONTIG_GO(M)                                                                                                      \
-  do {                                                                                                                       \
-    bk_ensure_smem(c, bkf::k_contig<FC, M>, FC::SMEM);                                                                        \
-    BK_CUDA(c, bk_launch_pdl(bkf::k_contig<FC, M>, grid, dim3(FC::THREADS), FC::SMEM, c->stream, in, out, g, tb, p0));       \
-  } while (0)
-    if (mode == 0) BKF_CONTIG_GO(0);
-    else if (mode == 1) BKF_CONTIG_GO(1);
-    else if (mode == 2) BKF_CONTIG_GO(2);
-    else BKF_CONTIG_GO(3);
-#undef BKF_CONTIG_GO
+    static decltype(&bkf::k_strided<FC, 0>) const kern[4] = {bkf::k_strided<FC, 0>, bkf::k_strided<FC, 1>, bkf::k_strided<FC, 2>,
+                                                             bkf::k_strided<FC, 3>};
+    const dim3 grid((g.nb + 2 * FC::PP - 1) / (2 * FC::PP), g.nouter);
+    return bk_launch(c, kern[mode], grid, dim3(FC::THREADS), mode >= 2 ? FC::SMEM_FUSED : FC::SMEM, in, out, g, tb, s0);
   }
-  return BK_OK;
+  static decltype(&bkf::k_contig<FC, 0>) const kern[4] = {bkf::k_contig<FC, 0>, bkf::k_contig<FC, 1>, bkf::k_contig<FC, 2>,
+                                                          bkf::k_contig<FC, 3>};
+  const dim3 grid((unsigned)((g.nb + 2 * FC::PP - 1) / (2 * FC::PP)));
+  return bk_launch(c, kern[mode], grid, dim3(FC::THREADS), FC::SMEM, in, out, g, tb, p0);
 }
 
 // ---- general path ----------------------------------------------------------------------------------------------------------
@@ -293,22 +269,9 @@ static int gen_launch(bk_ctx* c, int d, bool strided, int mode, const double* in
   const size_t sm = 32 * (size_t)pl.L * ppg;
   const long long npairs = ((long long)g.nb + 1) / 2;
   dim3 grid((unsigned)((npairs + ppg - 1) / ppg), strided ? g.nouter : 1);
-#define BKG_GO(S, M)                                                                                                       \
-  do {                                                                                                                     \
-    bk_ensure_smem(c, bkg::k_gen<S, M>, sm);                                                                               \
-    BK_CUDA(c, bk_launch_pdl(bkg::k_gen<S, M>, grid, dim3(BKG_THREADS), sm, c->stream, in, out, g, pl, ppg));              \
-  } while (0)
-  if (strided) {
-    if (mode == 0) BKG_GO(true, 0);
-    else if (mode == 1) BKG_GO(true, 1);
-    else BKG_GO(true, 2);
-  } else {
-    if (mode == 0) BKG_GO(false, 0);
-    else if (mode == 1) BKG_GO(false, 1);
-    else BKG_GO(false, 2);
-  }
-#undef BKG_GO
-  return BK_OK;
+  static decltype(&bkg::k_gen<false, 0>) const kern[2][3] = {{bkg::k_gen<false, 0>, bkg::k_gen<false, 1>, bkg::k_gen<false, 2>},
+                                                              {bkg::k_gen<true, 0>, bkg::k_gen<true, 1>, bkg::k_gen<true, 2>}};
+  return bk_launch(c, kern[strided][mode], grid, dim3(BKG_THREADS), sm, in, out, g, pl, ppg);
 }
 
 // transform tables for dimension d of length n. type 0: DCT-II (Neumann), 1: DST-I (Dirichlet)
@@ -340,7 +303,6 @@ int bk_periodic_setup(bk_ctx* c) {
     const long long n = c->dims[d];
     int logn = 0;
     while ((1LL << logn) < n) ++logn;
-    BK_CHECK(c, (1LL << logn) == n && logn >= 6 && logn <= 11, "BK_SH2D_PERIODIC: Nx and Ny must be powers of two from 64 to 2048");
     std::vector<double> lam(n);
     for (long long k = 0; k < n; ++k) {
       const long double ks = (long double)(k <= n / 2 ? k : k - n), w = PI * ks / (long double)c->lengths[d];
@@ -365,7 +327,6 @@ static int periodic_pipeline(bk_ctx* c, const double* in, double* out, const Per
   BKF_DISPATCH(pc.fast[0], BK_TRY(fast_launch<FC>(c, 0, false, 2, in, pc.work, gx, nullptr, &pw)));
   BKF_DISPATCH(pc.fast[1], BK_TRY(fast_launch<FC>(c, 1, true, 3, pc.work, pc.work2, gy, &sy)));
   BKF_DISPATCH(pc.fast[0], BK_TRY(fast_launch<FC>(c, 0, false, 3, pc.work2, out, gx, nullptr, &pw)));
-  c->stats.kernel_launches += 3;
   return BK_OK;
 }
 
@@ -396,30 +357,20 @@ extern "C" int32_t bk_precond_setup(bk_ctx* c, int32_t kind, double a0, double a
   const bool even_nx = (c->dims[0] % 2) == 0;
   if (kind == BK_PC_SH_DCT) {
     BK_CHECK(c, c->kind == BK_SH2D || c->kind == BK_SH3D, "BK_PC_SH_DCT needs a Swift-Hohenberg context");
-    int nd = c->kind == BK_SH3D ? 3 : 2;
-    for (int d = 0; d < nd; ++d) {
-      double h = 2 * c->lengths[d] / c->dims[d];
-      BK_TRY(setup_dim(c, d, c->dims[d], 1.0 / (h * h), 0, even_nx));
-    }
+    for (int d = 0; d < bk_kind_traits(c->kind)->ndims; ++d) BK_TRY(setup_dim(c, d, c->dims[d], bk_inv_h2(c, d), 0, even_nx));
   } else if (kind == BK_PC_SH_FFT) {
     BK_CHECK(c, c->kind == BK_SH2D_PERIODIC, "BK_PC_SH_FFT needs a BK_SH2D_PERIODIC context");
     BK_CHECK(c, a0 > 0, "BK_PC_SH_FFT: a0 must be > 0 (the symbol of L1 vanishes at |k| = 1)");
     // tables and work buffers are the context's own (bk_periodic_setup)
   } else if (kind == BK_PC_CGL_DST) {
     BK_CHECK(c, c->kind == BK_CGL2D || c->kind == BK_POTRAP_CGL2D, "BK_PC_CGL_DST needs a cGL context");
-    for (int d = 0; d < 2; ++d) {
-      double h = 2 * c->lengths[d] / c->dims[d];
-      BK_TRY(setup_dim(c, d, c->dims[d], 1.0 / (h * h), 1, even_nx));
-    }
+    for (int d = 0; d < 2; ++d) BK_TRY(setup_dim(c, d, c->dims[d], bk_inv_h2(c, d), 1, even_nx));
   } else if (kind == BK_PC_POTRAP_CIRC) {
     BK_CHECK(c, c->kind == BK_POTRAP_CGL2D, "BK_PC_POTRAP_CIRC needs a Trapeze (potrap) context");
     const int K = (int)c->dims[2] - 1;
     BK_CHECK(c, K >= 1 && K <= BK_PO_KMAX, "BK_PC_POTRAP_CIRC supports 2 <= M <= 65 time slices");
     BK_CHECK(c, a0 > 0, "BK_PC_POTRAP_CIRC: a0 must be the period T > 0");
-    for (int d = 0; d < 2; ++d) {
-      double h = 2 * c->lengths[d] / c->dims[d];
-      BK_TRY(setup_dim(c, d, c->dims[d], 1.0 / (h * h), 1, even_nx));
-    }
+    for (int d = 0; d < 2; ++d) BK_TRY(setup_dim(c, d, c->dims[d], bk_inv_h2(c, d), 1, even_nx));
     std::vector<double2> tw(K);
     const long double PI = 3.14159265358979323846264338327950288L;
     for (int j = 0; j < K; ++j) tw[j] = make_double2((double)cosl(-2.0L * PI * j / K), (double)sinl(-2.0L * PI * j / K));
@@ -488,7 +439,6 @@ static int transform_pass(bk_ctx* c, int d, int mode, const double* in, double* 
     BK_CHECK(c, !fused, "internal: fused transform on the general path");
     BK_TRY(gen_launch(c, d, strided, pc.ttype[d] == 1 ? 2 : mode, in, out, g));
   }
-  c->stats.kernel_launches++;
   return BK_OK;
 }
 
@@ -510,23 +460,12 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
   Precond& pc = c->pc;
   const long long N = c->N0;
   bool tail_done = false;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  if (c->timing_now) {  // per-application device time for bench.py's breakdown (event pairs are read back in bk_get_stats)
-    if (c->pc_pairs_used >= c->pc_pairs.size()) {
-      cudaEvent_t a, b;
-      cudaEventCreate(&a);
-      cudaEventCreate(&b);
-      c->pc_pairs.push_back({a, b});
-    }
-    ev0 = c->pc_pairs[c->pc_pairs_used].first;
-    ev1 = c->pc_pairs[c->pc_pairs_used].second;
-    c->pc_pairs_used++;
-    cudaEventRecord(ev0, c->stream);
-  }
+  const bool timed = c->timing_now;  // per-application device time for bench.py's breakdown
+  if (timed) c->pc_timer.begin(c->stream);
   const bool al = aligned16(in, out);
   if (pc.kind == BK_PC_SH_DCT) {
-    const int nx = (int)c->dims[0], ny = (int)c->dims[1], nz = c->kind == BK_SH3D ? (int)c->dims[2] : 1;
-    const int nd = c->kind == BK_SH3D ? 3 : 2;
+    const int nd = bk_kind_traits(c->kind)->ndims;
+    const int nx = (int)c->dims[0], ny = (int)c->dims[1], nz = nd == 3 ? (int)c->dims[2] : 1;
     double* A = pc.work;
     double* B = pc.work2;
     const int last = nd - 1;
@@ -561,7 +500,7 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
         cur = A;
         oth = B;
       }
-      k_sh_symbol_div<<<lin_grid(c, N), 256, 0, c->stream>>>(cur, nx, ny, nz, pc.lam[0], pc.lam[1],
+      k_sh_symbol_div<<<bk_lin_grid(c, N), 256, 0, c->stream>>>(cur, nx, ny, nz, pc.lam[0], pc.lam[1],
                                                             nd == 3 ? pc.lam[2] : nullptr, pc.a0, scale);
       c->stats.kernel_launches++;
       BK_CUDA(c, cudaGetLastError());
@@ -591,7 +530,7 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
     double* B = pc.work2;
     BK_TRY(transform_pass(c, 0, 0, in, A, nx, ny, (int)nblk, al));
     BK_TRY(transform_pass(c, 1, 0, A, B, nx, ny, (int)nblk, true));
-    k_helmholtz_symbol_div<<<lin_grid(c, (long long)nx * ny * nblk), 256, 0, c->stream>>>(B, nx, ny, nblk, pc.lam[0], pc.lam[1],
+    k_helmholtz_symbol_div<<<bk_lin_grid(c, (long long)nx * ny * nblk), 256, 0, c->stream>>>(B, nx, ny, nblk, pc.lam[0], pc.lam[1],
                                                                                          pc.a0, pc.a1);
     c->stats.kernel_launches++;
     BK_CUDA(c, cudaGetLastError());
@@ -623,7 +562,7 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
   }
   if (n > N && !tail_done)
     BK_CUDA(c, cudaMemcpyAsync(out + N, in + N, 8 * (size_t)(n - N), cudaMemcpyDeviceToDevice, c->stream));
-  if (ev1) cudaEventRecord(ev1, c->stream);
+  if (timed) c->pc_timer.end(c->stream);
   return BK_OK;
 }
 

@@ -310,10 +310,9 @@ static void fill_grid(bk_ctx* c, OpDesc& op) {
   op.nx = (int)c->dims[0];
   op.ny = (int)c->dims[1];
   op.nz = (int)c->dims[2];
-  // h = 2 l / N in every example (SH2d-fronts.jl:14-15, SH3d.jl:18-20, cGL2d.jl:7-8)
-  op.cx = 1.0 / ((2 * c->lengths[0] / c->dims[0]) * (2 * c->lengths[0] / c->dims[0]));
-  op.cy = 1.0 / ((2 * c->lengths[1] / c->dims[1]) * (2 * c->lengths[1] / c->dims[1]));
-  op.cz = (c->kind == BK_SH3D) ? 1.0 / ((2 * c->lengths[2] / c->dims[2]) * (2 * c->lengths[2] / c->dims[2])) : 0.0;
+  op.cx = bk_inv_h2(c, 0);
+  op.cy = bk_inv_h2(c, 1);
+  op.cz = (c->kind == BK_SH3D) ? bk_inv_h2(c, 2) : 0.0;
   op.N = c->N;
   op.bordered = 0;
   op.ba = op.bb = nullptr;
@@ -348,12 +347,6 @@ OpDesc bk_make_residual_op(bk_ctx* c) {
   op.cplx = 0;
   op.transpose = 0;
   return op;
-}
-
-static inline int lin_grid(bk_ctx* c, long long n) {
-  long long g = (n + 255) / 256;
-  long long cap = (long long)c->nsm * 8;
-  return (int)(g < cap ? (g > 0 ? g : 1) : cap);
 }
 
 template <int MODE>
@@ -391,14 +384,14 @@ static int launch_kind(bk_ctx* c, const OpDesc& op, const double* in, const doub
     }
     case BK_SH2D_PERIODIC:  // spectral: three transform kernels (bk_precond.cu), which count their own launches
       return MODE == 1 ? bk_periodic_residual(c, op, in, out) : bk_periodic_jvp(c, op, in, sp, out);
-    case BK_CHAN: k_chan_apply<MODE><<<lin_grid(c, op.nx), 256, 0, c->stream>>>(op, in, sp, out); break;
-    case BK_CGL2D: k_cgl_apply<MODE><<<lin_grid(c, (long long)op.nx * op.ny), 256, 0, c->stream>>>(op, in, sp, out); break;
+    case BK_CHAN: k_chan_apply<MODE><<<bk_lin_grid(c, op.nx), 256, 0, c->stream>>>(op, in, sp, out); break;
+    case BK_CGL2D: k_cgl_apply<MODE><<<bk_lin_grid(c, (long long)op.nx * op.ny), 256, 0, c->stream>>>(op, in, sp, out); break;
     case BK_POTRAP_CGL2D: {
       long long tot = (long long)op.nx * op.ny * op.nz;
-      k_potrap_apply<MODE><<<lin_grid(c, tot), 256, 0, c->stream>>>(op, in, sp, out);
+      k_potrap_apply<MODE><<<bk_lin_grid(c, tot), 256, 0, c->stream>>>(op, in, sp, out);
       c->stats.kernel_launches++;
       BK_CUDA(c, cudaGetLastError());
-      int g = lin_grid(c, op.N - 1);
+      int g = bk_lin_grid(c, op.N - 1);
       if (g > c->gmax) g = c->gmax;
       k_tail<0><<<g, 256, 0, c->stream>>>(op, in, sp, out, op.N - 1, (MODE == 1) ? c->phi_dot_xpi : 0.0, MODE == 0 ? 1 : 0,
                                           c->partials, c->counters + 9);
@@ -428,9 +421,7 @@ static __global__ void __launch_bounds__(256) k_cshift(double* __restrict__ out,
 }
 
 int bk_launch_apply(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* out) {
-  if (op.transpose)
-    BK_CHECK(c, op.kind == BK_SH2D || op.kind == BK_SH3D || op.kind == BK_SH2D_PERIODIC || op.kind == BK_CGL2D,
-             "J' is not available for this problem kind");
+  if (op.transpose) BK_CHECK(c, bk_kind_traits(op.kind)->has_jt, "J' is not available for this problem kind");
   if (op.cplx) {
     // ((a0 + i a0i) I + a1 J)(x + i y): the real operator on both halves, then the cross terms of the imaginary shift
     OpDesc half = op;
@@ -440,7 +431,7 @@ int bk_launch_apply(bk_ctx* c, const OpDesc& op, const double* in, const double*
     BK_TRY(launch_kind<0>(c, half, in, sp, out));
     BK_TRY(launch_kind<0>(c, half, in + half.N, sp, out + half.N));
     if (op.a0i != 0.0) {
-      k_cshift<<<lin_grid(c, half.N), 256, 0, c->stream>>>(out, in, sp, op.a0i, half.N);
+      k_cshift<<<bk_lin_grid(c, half.N), 256, 0, c->stream>>>(out, in, sp, op.a0i, half.N);
       c->stats.kernel_launches++;
       BK_CUDA(c, cudaGetLastError());
     }
@@ -448,7 +439,7 @@ int bk_launch_apply(bk_ctx* c, const OpDesc& op, const double* in, const double*
     BK_TRY(launch_kind<0>(c, op, in, sp, out));
   }
   if (op.bordered) {
-    int g = lin_grid(c, op.N);
+    int g = bk_lin_grid(c, op.N);
     if (g > c->gmax) g = c->gmax;
     if (op.bordered == 2) k_tail2<<<g, 256, 0, c->stream>>>(op, in, sp, out, op.N, c->partials, c->counters + 9);
     else k_tail<1><<<g, 256, 0, c->stream>>>(op, in, sp, out, op.N, 0.0, 0, c->partials, c->counters + 9);
@@ -462,7 +453,7 @@ int bk_potrap_refresh_cache(bk_ctx* c) {
   if (c->kind != BK_POTRAP_CGL2D) return BK_OK;
   OpDesc op = bk_make_op(c, 0, 1);
   long long tot = (long long)op.nx * op.ny * op.nz;
-  k_potrap_fcache<<<lin_grid(c, tot), 256, 0, c->stream>>>(op, c->u_state, c->fcache);
+  k_potrap_fcache<<<bk_lin_grid(c, tot), 256, 0, c->stream>>>(op, c->u_state, c->fcache);
   c->stats.kernel_launches++;
   BK_CUDA(c, cudaGetLastError());
   return BK_OK;
@@ -499,8 +490,7 @@ extern "C" int32_t bk_jac_set_shift_imag(bk_ctx* c, double a0_imag) {
 
 extern "C" int32_t bk_jac_set_transpose(bk_ctx* c, int32_t on) {
   BK_ENTER(c);
-  BK_CHECK(c, !on || c->kind == BK_SH2D || c->kind == BK_SH3D || c->kind == BK_SH2D_PERIODIC || c->kind == BK_CGL2D,
-           "J' is not available for this problem kind");
+  BK_CHECK(c, !on || bk_kind_traits(c->kind)->has_jt, "J' is not available for this problem kind");
   c->transpose = on != 0;
   return BK_OK;
 }
