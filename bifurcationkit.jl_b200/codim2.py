@@ -271,57 +271,28 @@ class Codim2Point:
 
 def locate_event(it, _st, values_at, labels, indicator=None):
     """locate_event!(event, iter, state) (src/events/EventDetection.jl:28-235) for a ContinuousEvent whose indicator is the number of
-    positive test functions (nb_signs): bisection on ds from the state `_st` just AFTER the event -- first half a step back, then
-    halving, reversing at every change of the indicator -- until contpar.n_inversion reversals (or max_bisection_steps /
-    dsmin_bisection).  On return `_st` holds the located state (just after the event for an even number of reversals) and its
-    predictor.  values_at(st) -> tuple of test-function values at a state.  Returns (status, interval, label)."""
+    positive test functions (nb_signs): the bisection of events.bisection on that number, from the state `_st` just AFTER the
+    event.  On return `_st` holds the located state (just after the event for an even number of reversals) and its predictor.
+    values_at(st) -> tuple of test-function values at a state.  Returns (status, interval, label of the test function that changed
+    at the last reversal)."""
     from . import events as E
-    from .palc import _predict
-    cp = it.contpar
     nb = indicator or (lambda vals: sum(1 for v in vals if v > 0))   # nb_signs: ContinuousEvent -> number of positive values;
-    if abs(_st.ds) < cp.dsmin:                                         # DiscreteEvent -> the value itself (EventDetection.jl:2-3)
+    if abs(_st.ds) < it.contpar.dsmin:                                 # DiscreteEvent -> the value itself (EventDetection.jl:2-3)
         return "none", (0.0, 0.0), None
-    v_after = values_at(_st)
-    after, st, before = E.copy_state(_st), E.copy_state(_st), E.copy_state(_st)
-    st.in_bisection = True
-    before.zold_p, before.z_p = before.z_p, before.zold_p
-    st.ds *= -1
-    st.step = 0
-    st.stepsizecontrol = False
-    nsigns = [nb(v_after)]
-    interval = list(E.getinterval(st.z_p, st.zold_p))
-    indinterval = 0 if interval[0] == st.z_p else 1
-    n_inversion, alive, vals = 0, True, v_after
-    changed = None
-    while True:
-        if not st.converged or not alive:
-            break
-        prev, vals = vals, values_at(st)      # update_event!: on the first pass this is the state the bisection starts from
-        nsigns.append(nb(vals))
-        if nsigns[-1] == nsigns[-2]:
-            st.ds /= 2                        # the event is still ahead of the current state
-        else:
-            st.ds /= -2                       # passed it: reverse
-            n_inversion += 1
-            indinterval = 1 - indinterval
-            changed = [k for k, (a_, b_) in enumerate(zip(prev, vals)) if ((a_ > 0) != (b_ > 0) if indicator is None else a_ != b_)]
-        _predict(st)
-        E.copyto_state(after if n_inversion % 2 == 0 else before, st)
-        if st.step > 0:
-            interval[indinterval] = st.z_p
-        if not (abs(st.ds) >= cp.dsmin_bisection and st.step < cp.max_bisection_steps and n_inversion < cp.n_inversion):
-            break
-        alive = it.iterate(st)
-    if n_inversion % 2 == 0:
-        status, src, interval = ("converged" if n_inversion >= cp.n_inversion else "guess"), st, (st.z_p, before.z_p)
-    else:
-        status, src, interval = "guessL", after, (st.z_p, after.z_p)
-    for k in ("z_u", "zold_u", "tau_u", "zpred_u"):
-        V.copyto(getattr(_st, k), getattr(src, k))
-    _st.z_p, _st.zold_p, _st.tau_p, _st.zpred_p = src.z_p, src.zold_p, src.tau_p, src.zpred_p
-    _st.work_newton, _st.work_linear = st.work_newton, st.work_linear
-    _predict(_st)                             # update_predictor!(_state, iter) with the outer ds
-    return status, E.getinterval(*interval), (labels[min(changed[0], len(labels) - 1)] if changed else None)
+    seen = []                                 # (indicator, test-function values) at every state the bisection compares
+
+    def count(s):
+        vals = values_at(s)
+        seen.append((nb(vals), vals))
+        return seen[-1][0]
+
+    status, interval, _, _ = E.bisection(it, _st, count)
+    flips = [(a[1], b[1]) for a, b in zip(seen, seen[1:]) if a[0] != b[0]]
+    if not flips:
+        return status, interval, None
+    prev, vals = flips[-1]
+    changed = [k for k, (a_, b_) in enumerate(zip(prev, vals)) if ((a_ > 0) != (b_ > 0) if indicator is None else a_ != b_)]
+    return status, interval, (labels[min(changed[0], len(labels) - 1)] if changed else None)
 
 
 @dataclass
@@ -370,7 +341,7 @@ def continuation_fold(prob, x0, p1_0, lens2, eigenvec, eigenvec_ad, contpar, bls
     alg = P.PALC(tangent=alg.tangent, theta=alg.theta, bls=BorderingBLSHost(fls))
     curve = FoldCurve([], [], [], [], [], ma, None, [])
     from . import events as E
-    it = E._Iter(pb, alg, cp, normC)
+    it = P.ContIterable(pb, alg, cp, normC)
     zh_hist = []
 
     def values_at(s):   # test_bt_cusp at a state, the border vectors untouched
@@ -410,7 +381,7 @@ def continuation_fold(prob, x0, p1_0, lens2, eigenvec, eigenvec_ad, contpar, bls
 
     p2_0 = prob.params[lens2]
     try:
-        curve.rows, curve.state = P.continuation(pb, alg, cp, normC=normC, callback=cb)
+        curve.rows, curve.state = P.continuation(pb, alg, cp, normC=normC, callback=cb, it=it)
     finally:
         prob.params[lens2] = p2_0  # the caller's parameter tuple is left as it was
     return curve
@@ -622,7 +593,7 @@ def continuation_hopf(prob, cprob, x0, p1_0, omega0, lens2, eigenvec, eigenvec_a
     curve.specialpoint = []
     cnorm = lambda z: float(np.max(np.abs(z)))
     from . import events as E
-    it = E._Iter(pb, alg, cp, normC)
+    it = P.ContIterable(pb, alg, cp, normC)
     tol_st = max(10 * no.tol, contpar.tol_stability)
     nhist = []
 
@@ -662,7 +633,7 @@ def continuation_hopf(prob, cprob, x0, p1_0, omega0, lens2, eigenvec, eigenvec_a
 
     p2_0, c2_0 = prob.params[lens2], cprob.params[lens2]
     try:
-        curve.rows, curve.state = P.continuation(pb, alg, cp, normC=normC, callback=cb)
+        curve.rows, curve.state = P.continuation(pb, alg, cp, normC=normC, callback=cb, it=it)
     finally:
         prob.params[lens2], cprob.params[lens2] = p2_0, c2_0
     return curve

@@ -4,10 +4,10 @@ What the reference does between two continuation steps when ``detect_bifurcation
 count unstable eigenvalues (``is_stable``, src/Bifurcations.jl:5-18), flag a change (``detect_bifurcation`` :21-28),
 optionally locate it by bisection on the step size (``locate_bifurcation!`` :159-349, ``detect_bifurcation = 3``), classify
 it from the change of (n_unstable, n_imag) (``get_bifurcation_type`` :70-150) and record a special point; folds by
-parameter monotony when eigenvalues are not used (``locate_fold!`` :33-66).  The continuation step itself (``iterate``,
-src/Continuation.jl:458-504) is assembled from the same pieces as ``palc.continuation`` -- corrector = ``newton_palc`` with
-the context's bordered solver, tangent, predictor -- so every linear solve and eigen-solve still goes through the C ABI
-(``MatrixFreeBLSB200`` / ``BorderingBLSB200`` / ``ShiftInvertB200``); ``palc.continuation`` is left untouched.
+parameter monotony when eigenvalues are not used (``locate_fold!`` :33-66).  The continuation steps, of the branch and of
+the bisection, are those of ``palc.ContIterable`` -- the iterator ``palc.continuation`` runs -- so every linear solve and
+eigen-solve still goes through the C ABI (``MatrixFreeBLSB200`` / ``BorderingBLSB200`` / ``ShiftInvertB200``).  The
+bisection loop (``bisection``) also locates the events of codim-2 curves (``codim2.locate_event``).
 
 State vectors are ``DeviceVec`` or ndarray through the ``V`` interface of palc.py; the three state copies the bisection keeps
 (`before`, `after`, current) are device copies (4 vectors each).
@@ -17,21 +17,10 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-from .palc import (V, ContState, newton, newton_palc, step_size_control, _secant, _bordered_tangent, _predict)
+from .palc import V, ContIterable, is_stable, _predict
 
 
 # ------------------------------------------------------------------------------------------------ stability bookkeeping
-def is_stable(contpar, eigvals):
-    """src/Bifurcations.jl:5-18 -> (isstable, n_unstable, n_imag)"""
-    if eigvals is None:
-        return True, 0, 0
-    ev = np.asarray(eigvals, dtype=complex)
-    tol = contpar.tol_stability
-    n_unstable = int(np.sum(ev.real > tol))
-    n_imag = int(np.sum((np.abs(ev.imag) > tol) & (ev.real > tol)))
-    return n_unstable == 0, n_unstable, n_imag
-
-
 def detect_bifurcation(st):
     """src/Bifurcations.jl:21-28"""
     n1, n2 = st.n_unstable
@@ -94,69 +83,8 @@ def copyto_state(dst, src):
     return dst
 
 
-def _done(contpar, st):
-    """src/Continuation.jl:254-257"""
-    return (st.step <= contpar.max_steps) and ((contpar.p_min < st.z_p < contpar.p_max) or st.step == 0) and not st.stop
-
-
 def _is_on_boundary(contpar, p):
     return p == contpar.p_min or p == contpar.p_max
-
-
-class _Iter:
-    """ContIterable: everything `iterate` needs (src/Continuation.jl:27-60)."""
-
-    def __init__(self, prob, alg, contpar, normC):
-        self.prob, self.alg, self.contpar, self.normC = prob, alg, contpar, normC
-
-    # compute_eigenvalues! (src/Utils.jl:70-104) + update_stability! (src/Continuation.jl:274-278)
-    def eigen(self, st):
-        cp = self.contpar
-        eig = cp.newton_options.eigsolver
-        if cp.detect_bifurcation <= 0 or eig is None:
-            return
-        n = st.n_unstable[1]
-        nev_ = max(n + 5, cp.nev)
-        out = eig(self.prob.J(st.z_u, st.z_p), nev_)
-        vals = np.asarray(out[0])
-        _, nu, ni = is_stable(cp, vals)
-        st.n_unstable = (nu, st.n_unstable[0])
-        st.n_imag = (ni, st.n_imag[0])
-        st.eigvals = vals
-        st.eigvecs = out[1] if len(out) > 1 else None
-
-    # iterate (src/Continuation.jl:458-504); returns False when the reference returns `nothing`
-    def iterate(self, st):
-        cp, alg, prob = self.contpar, self.alg, self.prob
-        if not _done(cp, st):
-            return False
-        if st.zpred_p <= cp.p_min or st.zpred_p >= cp.p_max:  # Palc.jl:157-160 -> Natural corrector
-            st.zpred_p = min(max(st.zpred_p, cp.p_min), cp.p_max)
-            sol = newton(prob, st.zpred_u, st.zpred_p, cp.newton_options, self.normC)
-            sol.p = st.zpred_p
-        else:
-            sol = newton_palc(prob, st.z_u, st.z_p, st.tau_u, st.tau_p, st.zpred_u, st.zpred_p, st.ds, alg.theta, cp, alg.bls,
-                              self.normC)
-        st.converged, st.itnewton, st.itlinear = sol.converged, sol.itnewton, sol.itlineartot
-        st.work_newton += sol.itnewton
-        st.work_linear += sol.itlineartot
-        st.nfail += 0 if sol.converged else 1
-        if sol.converged:
-            st.zold_u, st.z_u = st.z_u, st.zold_u
-            st.zold_p = st.z_p
-            V.copyto(st.z_u, sol.u)
-            st.z_p = sol.p
-            self.eigen(st)
-            st.step += 1
-        if not st.stop and st.stepsizecontrol:            # step_size_control! (Contbase.jl:69-76)
-            st.ds, st.stop = step_size_control(st.ds, st.converged, st.itnewton, cp)
-        if st.converged:                                  # getpredictor! (Palc.jl:133-146)
-            if alg.tangent == "secant":
-                _secant(st, alg.theta)
-            else:
-                _bordered_tangent(prob, st, alg.theta, alg.bls)
-        _predict(st)
-        return True
 
 
 # ------------------------------------------------------------------------------------------------ classification
@@ -198,36 +126,30 @@ def locate_fold(rows, specialpoints, it, st):
 
 
 # ------------------------------------------------------------------------------------------------ bisection
-def locate_bifurcation(it, _st):
-    """locate_bifurcation!(iter, state) (src/Bifurcations.jl:159-349): bisection on ds; on return `_st` sits just after
-    the bifurcation point (or is restored to `after`), status in {guess, guessL, converged, none}."""
-    assert detect_bifurcation(_st), "No bifurcation detected for the state"
+def bisection(it, _st, indicator, located=None):
+    """The bisection on ds of locate_bifurcation! (src/Bifurcations.jl:159-349) and locate_event! (src/events/
+    EventDetection.jl:28-235) from the state `_st` just after a change of `indicator(state)`: half a step back, then ds halved
+    at every step and reversed at every change of the indicator, until contpar.n_inversion reversals, max_bisection_steps,
+    dsmin_bisection or `located(state)`.  The steps are it.iterate without step-size control.  On return `_st` holds the
+    located state (just after the point for an even number of reversals) and its predictor.  Returns (status in {converged,
+    guess, guessL}, interval, the located state, the state on the other side of the point)."""
     cp = it.contpar
-    n2, n1 = _st.n_unstable
-    if n1 == -1 or n2 == -1 or abs(_st.ds) < cp.dsmin:
-        return "none", (0.0, 0.0)
+    marks = [indicator(_st)]
     after, st, before = copy_state(_st), copy_state(_st), copy_state(_st)
     st.in_bisection = True
-    before.n_unstable = (before.n_unstable[1], before.n_unstable[0])
+    before.n_unstable = (before.n_unstable[1], before.n_unstable[0])   # `before` is the previous point until a reversal
     before.n_imag = (before.n_imag[1], before.n_imag[0])
     before.zold_p, before.z_p = before.z_p, before.zold_p
     st.ds *= -1
     st.step = 0
     st.stepsizecontrol = False
-    alive = True                       # `next !== nothing`
-    nunstbls, nimags = [n2], [st.n_imag[0]]
     interval = list(getinterval(st.z_p, st.zold_p))
     indinterval = 0 if interval[0] == st.z_p else 1
-    n_inversion = 0
-    while True:
-        if not st.converged:
-            break                      # Newton failed to fully locate the point with the bisection parameters
-        if not alive:
-            break
-        nunstbls.append(st.n_unstable[0])
-        nimags.append(st.n_imag[0])
-        if nunstbls[-1] == nunstbls[-2]:
-            st.ds /= 2                 # bifurcation point still after the current state, keep going
+    n_inversion, alive = 0, True
+    while st.converged and alive:      # a failed Newton step or the end of the branch ends the bisection
+        marks.append(indicator(st))
+        if marks[-1] == marks[-2]:
+            st.ds /= 2                 # the point is still before the current state, keep going
         else:
             st.ds /= -2                # passed it: reverse
             n_inversion += 1
@@ -236,31 +158,37 @@ def locate_bifurcation(it, _st):
         copyto_state(after if n_inversion % 2 == 0 else before, st)
         if st.step > 0:
             interval[indinterval] = st.z_p
-        ev = rightmost(st.eigvals)
-        biflocated = abs(ev.real[0]) < cp.tol_bisection_eigenvalue
         if not (abs(st.ds) >= cp.dsmin_bisection and st.step < cp.max_bisection_steps and n_inversion < cp.n_inversion
-                and not biflocated):
+                and not (located is not None and located(st))):
             break
         alive = it.iterate(st)
     if n_inversion % 2 == 0:
-        status = "converged" if n_inversion >= cp.n_inversion else "guess"
-        src = st
-        _st.n_unstable = (st.n_unstable[0], before.n_unstable[0])
-        _st.n_imag = (st.n_imag[0], before.n_imag[0])
-        interval = (st.z_p, before.z_p)
+        status, here, there = ("converged" if n_inversion >= cp.n_inversion else "guess"), st, before
     else:
-        status = "guessL"
-        src = after
-        _st.n_unstable = (after.n_unstable[0], st.n_unstable[0])
-        _st.n_imag = (after.n_imag[0], st.n_imag[0])
-        interval = (st.z_p, after.z_p)
+        status, here, there = "guessL", after, st
     for k in _VEC:
-        V.copyto(getattr(_st, k), getattr(src, k))
-    _st.z_p, _st.zold_p, _st.tau_p, _st.zpred_p = src.z_p, src.zold_p, src.tau_p, src.zpred_p
-    _st.eigvals, _st.eigvecs = src.eigvals, getattr(src, "eigvecs", None)
+        V.copyto(getattr(_st, k), getattr(here, k))
+    _st.z_p, _st.zold_p, _st.tau_p, _st.zpred_p = here.z_p, here.zold_p, here.tau_p, here.zpred_p
     _st.work_newton, _st.work_linear = st.work_newton, st.work_linear   # the bisection's corrector work is real work
     _predict(_st)                      # update_predictor!(_state, iter) with the outer ds
-    return status, getinterval(*interval)
+    return status, getinterval(st.z_p, (after if n_inversion % 2 else before).z_p), here, there
+
+
+def locate_bifurcation(it, _st):
+    """locate_bifurcation!(iter, state) (src/Bifurcations.jl:159-349): bisection on the number of unstable eigenvalues, which
+    also stops at an eigenvalue within tol_bisection_eigenvalue of the imaginary axis; on return `_st` sits just after the
+    bifurcation point (or is restored to `after`), status in {guess, guessL, converged, none}."""
+    assert detect_bifurcation(_st), "No bifurcation detected for the state"
+    cp = it.contpar
+    n2, n1 = _st.n_unstable
+    if n1 == -1 or n2 == -1 or abs(_st.ds) < cp.dsmin:
+        return "none", (0.0, 0.0)
+    status, interval, here, there = bisection(it, _st, lambda s: s.n_unstable[0],
+                                              lambda s: abs(rightmost(s.eigvals).real[0]) < cp.tol_bisection_eigenvalue)
+    _st.n_unstable = (here.n_unstable[0], there.n_unstable[0])
+    _st.n_imag = (here.n_imag[0], there.n_imag[0])
+    _st.eigvals, _st.eigvecs = here.eigvals, here.eigvecs
+    return status, interval
 
 
 # ------------------------------------------------------------------------------------------------ driver
@@ -274,26 +202,13 @@ class Branch:
 
 def continuation(prob, alg, contpar, normC=V.norm2, verbose=False, callback=None, floquet=False):
     """continuation(prob, PALC(...), ContinuationPar(detect_bifurcation = 0..3)) with special points
-    (src/Continuation.jl:349-400 start-up, :506-575 loop).  Returns a Branch (rows as palc.continuation + `stable`,
-    `n_imag`; specialpoint list ends with the :endpoint)."""
-    cp, opts = contpar, contpar.newton_options
-    it = _Iter(prob, alg, cp, normC)
-    p0 = prob.p0
-    assert cp.p_min <= p0 <= cp.p_max
-    sol0 = newton(prob, prob.u0, p0, opts, normC)
-    if not sol0.converged:
-        raise RuntimeError(f"Newton failed to converge for the initial guess: {sol0.residuals}")
-    p1 = p0 + cp.ds / cp.eta
-    sol1 = newton(prob, sol0.u, p1, opts, normC)
-    if not sol1.converged:
-        raise RuntimeError("Newton failed to converge for the initial tangent")
-    u0, u1 = sol0.u, sol1.u
-    st = ContState(z_u=u1, z_p=p1, zold_u=u0, zold_p=p0, tau_u=V.zeros_like(u0), tau_p=0.0, zpred_u=V.zeros_like(u0),
-                   zpred_p=0.0, ds=cp.ds)
-    st.eigvecs = None
-    _secant(st, alg.theta)
-    st.z_u, st.z_p = V.copy(u0), p0
-    _predict(st)
+    (src/Continuation.jl:349-400 start-up, :506-575 loop): the loop of palc.continuation with the detection before each
+    row is saved.  Returns a Branch (rows as palc.continuation + `n_imag`, `stable`; specialpoint list ends with the
+    :endpoint)."""
+    cp = contpar
+    it = ContIterable(prob, alg, cp, normC)
+    st = it.start()
+    it.eigen(st)
     br = Branch(state=st)
 
     def save():
@@ -302,35 +217,29 @@ def continuation(prob, alg, contpar, normC=V.norm2, verbose=False, callback=None
                             step=st.step, n_unstable=st.n_unstable[0], n_imag=st.n_imag[0], stable=stable))
         if st.eigvals is not None:
             br.eig.append(dict(eigenvals=np.array(st.eigvals), step=st.step))
+        if callback is not None and callback(st) is False:
+            st.stop = True
 
-    it.eigen(st)
     save()
-    if callback is not None and callback(st) is False:
-        st.stop = True
     status = "guess"
-    alive = True
-    first = True
-    while alive:
-        if not first and st.converged and st.step <= cp.max_steps and st.step > 0:
-            if cp.detect_fold and cp.detect_bifurcation < 2:
-                locate_fold(br.rows, br.specialpoint, it, st)
-            if cp.detect_bifurcation > 1 and detect_bifurcation(st):
-                interval = getinterval(st.zold_p, st.z_p)
-                if cp.detect_bifurcation > 2 and not _is_on_boundary(cp, st.z_p):
-                    status, interval = locate_bifurcation(it, st)
-                if detect_bifurcation(st):   # the bisection may have moved the state before the point
-                    bp = get_bifurcation_type(it, st, status, interval, floquet)
-                    if bp.type != "none":
-                        br.specialpoint.append(bp)
-                    if verbose:
-                        print(f"--> {bp.type} bifurcation point at p ~ {bp.param:.8g} in {bp.interval}, delta = {bp.delta}, {bp.status}", flush=True)
-            save()
-            if callback is not None and callback(st) is False:
-                st.stop = True
-        first = False
-        alive = it.iterate(st)
-        if verbose and alive:
+    while it.iterate(st):
+        if verbose:
             print(f"step {st.step} p={st.z_p:.6e} ds={st.ds:.3e} conv={st.converged} itn={st.itnewton} n_unstable={st.n_unstable}", flush=True)
+        if not (st.converged and st.step <= cp.max_steps):
+            continue
+        if cp.detect_fold and cp.detect_bifurcation < 2:
+            locate_fold(br.rows, br.specialpoint, it, st)
+        if cp.detect_bifurcation > 1 and detect_bifurcation(st):
+            interval = getinterval(st.zold_p, st.z_p)
+            if cp.detect_bifurcation > 2 and not _is_on_boundary(cp, st.z_p):
+                status, interval = locate_bifurcation(it, st)
+            if detect_bifurcation(st):   # the bisection may have moved the state before the point
+                bp = get_bifurcation_type(it, st, status, interval, floquet)
+                if bp.type != "none":
+                    br.specialpoint.append(bp)
+                if verbose:
+                    print(f"--> {bp.type} bifurcation point at p ~ {bp.param:.8g} in {bp.interval}, delta = {bp.delta}, {bp.status}", flush=True)
+        save()
     br.specialpoint.append(SpecialPoint(type="endpoint", idx=len(br.rows) - 1, param=st.z_p, norm=normC(st.z_u), step=st.step,
                                         status="converged", delta=(0, 0), ind_ev=0, interval=(st.z_p, st.z_p)))
     return br

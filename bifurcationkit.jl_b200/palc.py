@@ -276,11 +276,12 @@ class ContState:
     stop: bool = False
     n_unstable: tuple = (-1, -1)
     eigvals: object = None
+    eigvecs: object = None
     nfail: int = 0
     work_newton: int = 0
     work_linear: int = 0
-    n_imag: tuple = (-1, -1)       # events.py: unstable eigenvalues with nonzero imaginary part (current, previous)
-    stepsizecontrol: bool = True   # events.py: switched off inside the bisection
+    n_imag: tuple = (-1, -1)       # unstable eigenvalues with nonzero imaginary part (current, previous)
+    stepsizecontrol: bool = True   # switched off inside the bisection (events.bisection)
     in_bisection: bool = False
 
 
@@ -316,94 +317,143 @@ def _predict(st):
     st.zpred_p = st.z_p + st.ds * st.tau_p
 
 
-def continuation(prob, alg, contpar, normC=V.norm2, u1=None, p1=None, verbose=False, callback=None):
-    """src/Continuation.jl:349-504,506-601.  Returns (rows, state); rows mirror ContResult.branch
-    (param, x = record_from_solution, itnewton, itlinear, ds, step, n_unstable; src/Continuation.jl:259-272).
-    With (u1, p1) the branch starts from two points (iterate_from_two_points, :408-456) -- used to seed
-    branch segments on other GPUs."""
-    opts = contpar.newton_options
-    theta, bls = alg.theta, alg.bls
-    p0 = prob.p0
-    if u1 is None:
-        assert contpar.p_min <= p0 <= contpar.p_max
-        sol0 = newton(prob, prob.u0, p0, opts, normC)
-        if not sol0.converged:
-            raise RuntimeError(f"Newton failed to converge for the initial guess: {sol0.residuals}")
-        p1 = p0 + contpar.ds / contpar.eta
-        sol1 = newton(prob, sol0.u, p1, opts, normC)
-        if not sol1.converged:
-            raise RuntimeError("Newton failed to converge for the initial tangent")
-        u0, u1 = sol0.u, sol1.u
-    else:
-        u0 = V.copy(prob.u0)
-    # state.z = z1, z_old = z0 -> secant tangent; then z <- z0 (initialize!, Palc.jl:112-123)
-    st = ContState(z_u=u1, z_p=p1, zold_u=u0, zold_p=p0, tau_u=V.zeros_like(u0), tau_p=0.0,
-                   zpred_u=V.zeros_like(u0), zpred_p=0.0, ds=contpar.ds)
-    _secant(st, theta)
-    st.z_u, st.z_p = V.copy(u0), p0
-    _predict(st)
-    rows = []
+def is_stable(contpar, eigvals):
+    """src/Bifurcations.jl:5-18 -> (isstable, n_unstable, n_imag)"""
+    if eigvals is None:
+        return True, 0, 0
+    ev = np.asarray(eigvals, dtype=complex)
+    tol = contpar.tol_stability
+    n_unstable = int(np.sum(ev.real > tol))
+    n_imag = int(np.sum((np.abs(ev.imag) > tol) & (ev.real > tol)))
+    return n_unstable == 0, n_unstable, n_imag
 
-    def eig_update():
-        if contpar.detect_bifurcation > 0 and opts.eigsolver is not None:
-            nprev = st.n_unstable[1]
-            nev_ = max(nprev + 5, contpar.nev) if nprev >= 0 else contpar.nev  # src/Utils.jl:78-79
-            J = prob.J(st.z_u, st.z_p)
-            vals = opts.eigsolver(J, nev_)[0]
-            nun = int(np.sum(np.real(vals) > contpar.tol_stability))  # src/Bifurcations.jl:5-18
-            st.n_unstable = (nun, st.n_unstable[0])
-            st.eigvals = vals
 
-    def save():
-        rows.append(dict(param=st.z_p, x=prob.record(st.z_u), itnewton=st.itnewton, itlinear=st.itlinear,
-                         ds=st.ds, step=st.step, n_unstable=st.n_unstable[0]))
+class ContIterable:
+    """ContIterable (src/Continuation.jl:27-60): what a continuation step needs.  `start` makes the first state and `iterate`
+    advances a state by one step; `correct`, `accept` and `advance` are the parts of that step a caller choosing its own step
+    sizes (segments.continuation_speculative) runs itself."""
 
-    eig_update()
-    save()
-    if callback is not None and callback(st) is False:  # step 0 (lets callers mark the start of the continuation! loop)
-        st.stop = True
+    def __init__(self, prob, alg, contpar, normC=V.norm2):
+        self.prob, self.alg, self.contpar, self.normC = prob, alg, contpar, normC
 
-    def done():  # src/Continuation.jl:254-257
-        return (st.step <= contpar.max_steps) and ((contpar.p_min < st.z_p < contpar.p_max) or st.step == 0) and not st.stop
-
-    first = True
-    while True:
-        if not first and st.converged and st.step <= contpar.max_steps and st.step > 0:
-            save()
-            if callback is not None and callback(st) is False:
-                st.stop = True
-        first = False
-        if not done():
-            break
-        if st.zpred_p <= contpar.p_min or st.zpred_p >= contpar.p_max:  # Palc.jl:157-160 -> Natural corrector
-            st.zpred_p = min(max(st.zpred_p, contpar.p_min), contpar.p_max)
-            sol = newton(prob, st.zpred_u, st.zpred_p, opts, normC)
-            sol.p = st.zpred_p
+    def start(self, u1=None, p1=None):
+        """start-up (src/Continuation.jl:349-405): z0 by Newton from prob.u0, z1 by Newton at p0 + ds / eta -- or the given
+        second point (u1, p1) (iterate_from_two_points, :408-456) -- then the secant through them, z <- z0 and the predictor
+        (initialize!, Palc.jl:112-123)."""
+        prob, cp = self.prob, self.contpar
+        p0 = prob.p0
+        if u1 is None:
+            assert cp.p_min <= p0 <= cp.p_max
+            sol0 = newton(prob, prob.u0, p0, cp.newton_options, self.normC)
+            if not sol0.converged:
+                raise RuntimeError(f"Newton failed to converge for the initial guess: {sol0.residuals}")
+            p1 = p0 + cp.ds / cp.eta
+            sol1 = newton(prob, sol0.u, p1, cp.newton_options, self.normC)
+            if not sol1.converged:
+                raise RuntimeError("Newton failed to converge for the initial tangent")
+            u0, u1 = sol0.u, sol1.u
         else:
-            sol = newton_palc(prob, st.z_u, st.z_p, st.tau_u, st.tau_p, st.zpred_u, st.zpred_p, st.ds, theta, contpar,
-                              bls, normC)
+            u0 = V.copy(prob.u0)
+        st = ContState(z_u=u1, z_p=p1, zold_u=u0, zold_p=p0, tau_u=V.zeros_like(u0), tau_p=0.0,
+                       zpred_u=V.zeros_like(u0), zpred_p=0.0, ds=cp.ds)
+        _secant(st, self.alg.theta)
+        st.z_u, st.z_p = V.copy(u0), p0
+        _predict(st)
+        return st
+
+    def eigen(self, st):
+        """compute_eigenvalues! (src/Utils.jl:70-104) + update_stability! (src/Continuation.jl:274-278)"""
+        cp = self.contpar
+        eig = cp.newton_options.eigsolver
+        if cp.detect_bifurcation <= 0 or eig is None:
+            return
+        out = eig(self.prob.J(st.z_u, st.z_p), max(st.n_unstable[1] + 5, cp.nev))  # src/Utils.jl:78-79
+        vals = np.asarray(out[0])
+        _, nu, ni = is_stable(cp, vals)
+        st.n_unstable = (nu, st.n_unstable[0])
+        st.n_imag = (ni, st.n_imag[0])
+        st.eigvals = vals
+        st.eigvecs = out[1] if len(out) > 1 else None
+
+    def done(self, st):
+        """src/Continuation.jl:254-257"""
+        cp = self.contpar
+        return (st.step <= cp.max_steps) and ((cp.p_min < st.z_p < cp.p_max) or st.step == 0) and not st.stop
+
+    def correct(self, st, zpred_p, ds):
+        """corrector! from the predictor (st.zpred_u, zpred_p) of a step ds: Newton at fixed parameter (the Natural corrector)
+        when zpred_p reaches a bound (Palc.jl:157-160), newton_palc otherwise"""
+        prob, alg, cp = self.prob, self.alg, self.contpar
+        if zpred_p <= cp.p_min or zpred_p >= cp.p_max:
+            zpred_p = min(max(zpred_p, cp.p_min), cp.p_max)
+            sol = newton(prob, st.zpred_u, zpred_p, cp.newton_options, self.normC)
+            sol.p = zpred_p
+            return sol
+        return newton_palc(prob, st.z_u, st.z_p, st.tau_u, st.tau_p, st.zpred_u, zpred_p, ds, alg.theta, cp, alg.bls, self.normC)
+
+    def accept(self, st, u, p):
+        """move to the corrected point (u, p): z_old <- z by swapping the buffers, z <- (u, p), one more step"""
+        st.zold_u, st.z_u = st.z_u, st.zold_u
+        st.zold_p = st.z_p
+        V.copyto(st.z_u, u)
+        st.z_p = p
+        st.step += 1
+
+    def advance(self, st):
+        """getpredictor! (Palc.jl:133-146): the tangent at a converged point, then the predictor z + ds tau"""
+        alg = self.alg
+        if st.converged:
+            if alg.tangent == "secant":
+                _secant(st, alg.theta)
+            else:
+                _bordered_tangent(self.prob, st, alg.theta, alg.bls)
+        _predict(st)
+
+    def iterate(self, st):
+        """iterate (src/Continuation.jl:458-504): one continuation step on `st`; False where the reference returns `nothing`"""
+        if not self.done(st):
+            return False
+        sol = self.correct(st, st.zpred_p, st.ds)
         st.converged, st.itnewton, st.itlinear = sol.converged, sol.itnewton, sol.itlineartot
         st.work_newton += sol.itnewton      # all corrector work, including rejected attempts
         st.work_linear += sol.itlineartot
         st.nfail += 0 if sol.converged else 1
         if sol.converged:
-            st.zold_u, st.z_u = st.z_u, st.zold_u  # swap buffers: z_old <- z
-            st.zold_p = st.z_p
-            V.copyto(st.z_u, sol.u)
-            st.z_p = sol.p
-            eig_update()
-            st.step += 1
+            self.accept(st, sol.u, sol.p)
+            self.eigen(st)
+        if not st.stop and st.stepsizecontrol:  # step_size_control! (Contbase.jl:69-76)
+            st.ds, st.stop = step_size_control(st.ds, st.converged, st.itnewton, self.contpar)
+        self.advance(st)
+        return True
+
+
+def continuation(prob, alg, contpar, normC=V.norm2, u1=None, p1=None, verbose=False, callback=None, it=None):
+    """src/Continuation.jl:349-504,506-601.  Returns (rows, state); rows mirror ContResult.branch
+    (param, x = record_from_solution, itnewton, itlinear, ds, step, n_unstable; src/Continuation.jl:259-272).
+    With (u1, p1) the branch starts from two points (iterate_from_two_points, :408-456) -- used to seed
+    branch segments on other GPUs.  `it`: the ContIterable over (prob, alg, contpar, normC) to run, for a callback that
+    steps it itself (the event bisection on codim-2 curves)."""
+    it = it or ContIterable(prob, alg, contpar, normC)
+    st = it.start(u1, p1)
+    it.eigen(st)
+    rows = []
+
+    def save():
+        rows.append(dict(param=st.z_p, x=it.prob.record(st.z_u), itnewton=st.itnewton, itlinear=st.itlinear,
+                         ds=st.ds, step=st.step, n_unstable=st.n_unstable[0]))
+        if callback is not None and callback(st) is False:
+            st.stop = True
+
+    save()  # step 0 (lets callers mark the start of the continuation! loop)
+    while True:
+        ds = st.ds  # the step size this step tries
+        if not it.iterate(st):
+            break
         if verbose:
-            print(f"step {st.step} p={st.z_p:.6e} ds={st.ds:.3e} conv={st.converged} itn={st.itnewton} itl={st.itlinear}",
+            print(f"step {st.step} p={st.z_p:.6e} ds={ds:.3e} conv={st.converged} itn={st.itnewton} itl={st.itlinear}",
                   flush=True)
-        if not st.stop:
-            st.ds, st.stop = step_size_control(st.ds, st.converged, st.itnewton, contpar)
-        if st.converged:
-            if alg.tangent == "secant":
-                _secant(st, theta)
-            else:
-                _bordered_tangent(prob, st, theta, bls)
-        _predict(st)
+        if st.converged and st.step <= it.contpar.max_steps:
+            save()
     return rows, st
 
 

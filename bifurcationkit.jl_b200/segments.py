@@ -6,8 +6,6 @@ reference's two-point start (iterate_from_two_points, src/Continuation.jl:408-45
 switching, src/bifdiagram/BranchSwitching.jl:8-44).  State vectors are replicated; the only collective is an
 all_gather of the per-step rows (lambda, ||u||, itnewton, itlinear), 32 B per step.
 """
-import math
-
 import numpy as np
 
 ROW = ("param", "x", "itnewton", "itlinear")
@@ -311,14 +309,6 @@ def continuation_bothside(P, make_prob, alg, contpar, normC, dist=None, torch=No
 # size the sequential loop would have had.  Accepted points, rows and counters equal the single-process run exactly (same
 # inputs, deterministic kernels); what changes is the wall time of the rejected attempts.
 # ======================================================================================================================
-def _halve(ds, contpar):
-    """the failure branch of step_size_control (Contbase.jl:80-86, 100): -> (new ds, stop)"""
-    if abs(ds) <= contpar.dsmin:
-        return ds, True
-    d = math.copysign(max(abs(ds) / 2, contpar.dsmin), ds)
-    return math.copysign(min(max(abs(d), contpar.dsmin), contpar.dsmax), d), False
-
-
 def continuation_speculative(P, prob, alg, contpar, normC, dist, torch, device="cpu", callback=None, to_host=None, from_host=None):
     """palc.continuation(prob, alg, contpar, normC) over the ranks of `dist` with speculative step sizes.  Every rank returns the
     same (rows, state, info); info = dict(rounds, attempts, wasted): corrector rounds actually waited for, corrector attempts the
@@ -328,21 +318,8 @@ def continuation_speculative(P, prob, alg, contpar, normC, dist, torch, device="
     world, rank = dist.get_world_size(), dist.get_rank()
     to_host = to_host or (lambda v: v.numpy() if hasattr(v, "numpy") else np.asarray(v))
     from_host = from_host or (lambda a, like: like.ctx.to_device(a) if hasattr(like, "ctx") else np.array(a))
-    opts, theta, bls = contpar.newton_options, alg.theta, alg.bls
-    p0 = prob.p0
-    assert contpar.p_min <= p0 <= contpar.p_max
-    sol0 = P.newton(prob, prob.u0, p0, opts, normC)           # start-up: replicated, deterministic
-    if not sol0.converged:
-        raise RuntimeError(f"Newton failed to converge for the initial guess: {sol0.residuals}")
-    p1 = p0 + contpar.ds / contpar.eta
-    sol1 = P.newton(prob, sol0.u, p1, opts, normC)
-    if not sol1.converged:
-        raise RuntimeError("Newton failed to converge for the initial tangent")
-    st = P.ContState(z_u=sol1.u, z_p=p1, zold_u=sol0.u, zold_p=p0, tau_u=V.zeros_like(sol0.u), tau_p=0.0, zpred_u=V.zeros_like(sol0.u),
-                     zpred_p=0.0, ds=contpar.ds)
-    P._secant(st, theta)
-    st.z_u, st.z_p = V.copy(sol0.u), p0
-    P._predict(st)
+    it = P.ContIterable(prob, alg, contpar, normC)
+    st = it.start()                                              # start-up: replicated, deterministic
     rows, info = [], dict(rounds=0, attempts=0, wasted=0)
 
     def save():
@@ -353,26 +330,20 @@ def continuation_speculative(P, prob, alg, contpar, normC, dist, torch, device="
 
     save()
     n = len(st.z_u)
-    while (st.step <= contpar.max_steps) and ((contpar.p_min < st.z_p < contpar.p_max) or st.step == 0) and not st.stop:
+    while it.done(st):
         # the step sizes the sequential loop would try one after the other from this point: d_0 = ds, d_{r+1} = halve(d_r)
         trial, d, dead = [], st.ds, False
         for _ in range(world):
             trial.append(None if dead else d)
             if not dead:
-                d, dead = _halve(d, contpar)
+                d, dead = P.step_size_control(d, False, 0, contpar)
         mine = trial[rank]
         res = np.zeros(4)                                        # (valid, converged, itnewton, itlinear)
         sol = None
         if mine is not None:
             V.copyto(st.zpred_u, st.z_u)
             V.axpby(st.zpred_u, mine, st.tau_u, 1.0)
-            zp = st.z_p + mine * st.tau_p
-            if zp <= contpar.p_min or zp >= contpar.p_max:       # Natural corrector at the bound (Palc.jl:157-160)
-                zp = min(max(zp, contpar.p_min), contpar.p_max)
-                sol = P.newton(prob, st.zpred_u, zp, opts, normC)
-                sol.p = zp
-            else:
-                sol = P.newton_palc(prob, st.z_u, st.z_p, st.tau_u, st.tau_p, st.zpred_u, zp, mine, theta, contpar, bls, normC)
+            sol = it.correct(st, st.z_p + mine * st.tau_p, mine)
             res[:] = (1.0, float(sol.converged), sol.itnewton, sol.itlineartot)
         t = torch.tensor(res, dtype=torch.float64, device=device)
         allr = [torch.zeros_like(t) for _ in range(world)]
@@ -391,7 +362,7 @@ def continuation_speculative(P, prob, alg, contpar, normC, dist, torch, device="
         if win is None:
             st.converged = False
             st.itnewton, st.itlinear = int(allr[last, 2]), int(allr[last, 3])
-            st.ds, st.stop = _halve(trial[last], contpar)        # the failed attempt with d_last: halve again or stop at dsmin
+            st.ds, st.stop = P.step_size_control(trial[last], False, 0, contpar)  # the failed attempt with d_last: halve or stop
             continue
         # the winner's corrected point to every rank
         buf = np.zeros(n + 1)
@@ -400,18 +371,10 @@ def continuation_speculative(P, prob, alg, contpar, normC, dist, torch, device="
         tb = torch.tensor(buf, dtype=torch.float64, device=device)
         dist.broadcast(tb, src=win)
         buf = tb.cpu().numpy()
-        st.zold_u, st.z_u = st.z_u, st.zold_u
-        st.zold_p = st.z_p
-        V.copyto(st.z_u, sol.u if rank == win else from_host(buf[:n], st.z_u))
-        st.z_p = float(buf[n])
+        it.accept(st, sol.u if rank == win else from_host(buf[:n], st.z_u), float(buf[n]))
         st.converged, st.itnewton, st.itlinear = True, int(allr[win, 2]), int(allr[win, 3])
-        st.step += 1
         st.ds, st.stop = P.step_size_control(trial[win], True, st.itnewton, contpar)
-        if alg.tangent == "secant":
-            P._secant(st, theta)
-        else:
-            P._bordered_tangent(prob, st, theta, bls)
-        P._predict(st)
+        it.advance(st)
         if st.step <= contpar.max_steps:
             save()
     return rows, st, info

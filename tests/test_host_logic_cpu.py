@@ -340,6 +340,27 @@ def test_bifurcation_detection_and_bisection_known_answers():
     _check_branch(E.continuation(prob(0.95), alg, cp4), cp4, E)
 
 
+def test_eigen_request_follows_the_reference_from_the_first_step():
+    """compute_eigenvalues (src/Utils.jl:78-79) asks for max(n_unstable + 5, nev) eigenvalues, also while n_unstable is still
+    -1: with nev = 1, palc.continuation asks for 4 at the start, as events.continuation does, and fills n_imag alike."""
+    bk = g.load_package()
+    P, E = bk.palc, bk.events
+    F, J = _fold_problem()
+    asked = {"palc": [], "events": []}
+
+    def mk(who):
+        eig = lambda Jm, nev: asked[who].append(nev) or _default_eig(Jm, nev)
+        return P.ContinuationPar(dsmin=0.001, dsmax=0.07, ds=-0.02, p_max=4.1, p_min=-1.0, max_steps=30, nev=1, detect_bifurcation=1,
+                                 newton_options=P.NewtonPar(tol=1e-8, linsolver=krylov.DefaultLS(), eigsolver=eig))
+
+    alg = P.PALC(bls=BlsAdapter(obls.MatrixBLS()))
+    rows, st = P.continuation(NumpyProblem(F, J, np.array([0.8]), 1.0), alg, mk("palc"))
+    br = E.continuation(NumpyProblem(F, J, np.array([0.8]), 1.0), alg, mk("events"))
+    assert asked["palc"][:2] == [4, 4] and asked["palc"] == asked["events"]
+    assert [r["n_unstable"] for r in rows] == [r["n_unstable"] for r in br.rows]
+    assert st.n_imag == br.state.n_imag == (0, 0)
+
+
 def test_fold_and_hopf_detection_two_dimensional_field():
     """test/continuation/test_bif_detection.jl:113-143: 2-d field with folds and Hopf points; detect_bifurcation = 3,
     n_inversion = 6.  The branch invariants of `testBranch` hold and a Hopf point is found with a complex pair crossing."""
