@@ -17,3 +17,4 @@ from . import floquet
 from . import events
 from . import deflation
 from . import codim2
+from . import normalform

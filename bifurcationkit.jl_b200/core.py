@@ -152,6 +152,18 @@ class Context:
         _chk(self, self.lib.bk_jvp(self.handle, _l.ptr(v), _l.ptr(out), a0, a1))
         return out
 
+    def d2f(self, u, dx1, dx2, out=None):
+        """d2F(u; params)[dx1, dx2] at the current params (prob.VF.d2F, src/Problems.jl:165)"""
+        out = self._like(u) if out is None else out
+        _chk(self, self.lib.bk_d2f(self.handle, _l.ptr(u), _l.ptr(dx1), _l.ptr(dx2), _l.ptr(out)))
+        return out
+
+    def d3f(self, u, dx1, dx2, dx3, out=None):
+        """d3F(u; params)[dx1, dx2, dx3] at the current params (prob.VF.d3F, src/Problems.jl:180)"""
+        out = self._like(u) if out is None else out
+        _chk(self, self.lib.bk_d3f(self.handle, _l.ptr(u), _l.ptr(dx1), _l.ptr(dx2), _l.ptr(dx3), _l.ptr(out)))
+        return out
+
     def precond_setup(self, kind, a0=1.0, a1=1.0):
         _chk(self, self.lib.bk_precond_setup(self.handle, kind, a0, a1))
 

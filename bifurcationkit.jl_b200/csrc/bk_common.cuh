@@ -113,6 +113,7 @@ struct BkKindTraits {
   bool has_jt;      // J' available (bk_jac_set_transpose)
   bool complex_ok;  // BK_COMPLEX allowed
   bool pow2_grid;   // Nx and Ny must be powers of two from 64 to 2048
+  bool has_jets;    // d2F / d3F available (bk_d2f, bk_d3f)
 };
 const BkKindTraits* bk_kind_traits(int kind);  // nullptr for an unknown kind
 

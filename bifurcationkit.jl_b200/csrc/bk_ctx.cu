@@ -72,14 +72,14 @@ int bk_tmp(bk_ctx* c, int slot, double** out) {
 }
 
 const BkKindTraits* bk_kind_traits(int kind) {
-  //                                   ndims fields extra jac_sym has_jt complex_ok pow2_grid
-  static const BkKindTraits table[] = {{0, 0, 0, false, false, false, false},  // 0: not a kind
-                                       {1, 1, 0, false, false, true, false},   // BK_CHAN
-                                       {2, 1, 0, true, true, true, false},     // BK_SH2D
-                                       {3, 1, 0, true, true, true, false},     // BK_SH3D
-                                       {2, 2, 0, false, true, true, false},    // BK_CGL2D
-                                       {3, 2, 1, false, false, false, false},  // BK_POTRAP_CGL2D
-                                       {2, 1, 0, true, true, true, true}};     // BK_SH2D_PERIODIC
+  //                                   ndims fields extra jac_sym has_jt complex_ok pow2_grid has_jets
+  static const BkKindTraits table[] = {{0, 0, 0, false, false, false, false, false},  // 0: not a kind
+                                       {1, 1, 0, false, false, true, false, true},     // BK_CHAN
+                                       {2, 1, 0, true, true, true, false, true},       // BK_SH2D
+                                       {3, 1, 0, true, true, true, false, true},       // BK_SH3D
+                                       {2, 2, 0, false, true, true, false, true},      // BK_CGL2D
+                                       {3, 2, 1, false, false, false, false, false},   // BK_POTRAP_CGL2D
+                                       {2, 1, 0, true, true, true, true, true}};       // BK_SH2D_PERIODIC
   static_assert(BK_CHAN == 1 && BK_POTRAP_CGL2D == 5 && BK_SH2D_PERIODIC == 6, "the table is indexed by kind");
   if (kind < BK_CHAN || kind > BK_SH2D_PERIODIC) return nullptr;
   return &table[kind];

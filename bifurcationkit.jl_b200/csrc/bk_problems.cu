@@ -199,6 +199,81 @@ static __global__ void __launch_bounds__(256) k_potrap_fcache(OpDesc op, const d
   }
 }
 
+// ------------------------------------------------------------------------------------------ jets d2F / d3F
+// Second and third differentials of F in u (src/Problems.jl:107-110,165-183).  The linear parts of F (Laplacians, L1, the
+// spectral symbol) drop out, so both are pointwise; the boundary rows of chan are linear too.  ORDER 2: out = d2F(u)[a, b],
+// ORDER 3: out = d3F(u)[a, b, c].  One thread per grid point; cGL2d points carry the pair (u1, u2) = Re, Im of A.
+// chan_Nl = 1 + g / h with g = x + x^2 / 2, h = 1 + b x^2 (examples/chan.jl:5-7, b = beta as chan_F):
+//   Nl'' = (1 - 6 b x - 3 b x^2 + 2 b^2 x^3) / h^3,   Nl''' = (-6 b - 12 b x + 36 b^2 x^2 + 12 b^2 x^3 - 6 b^3 x^4) / h^4
+__device__ __forceinline__ double chan_d2Nl(double x, double b) {
+  const double h = 1.0 + b * x * x;
+  return (1.0 - 6.0 * b * x - 3.0 * b * x * x + 2.0 * b * b * x * x * x) / (h * h * h);
+}
+__device__ __forceinline__ double chan_d3Nl(double x, double b) {
+  const double h = 1.0 + b * x * x, x2 = x * x;
+  return (-6.0 * b - 12.0 * b * x + 36.0 * b * b * x2 + 12.0 * b * b * x2 * x - 6.0 * b * b * b * x2 * x2) / (h * h * h * h);
+}
+// cGL2d: NL(A) = (r + i nu) A - (c3 + i mu) |A|^2 A - c5 |A|^4 A (examples/cGL2d.jl:262-279).  With s = |A|^2 and
+// s_xy = 2 Re(x conj y), the forms are real-multilinear (s is not holomorphic):
+//   d2(s A)[a,b]     = s_ab A + s_A(a) b + s_A(b) a,                   s_A(x) = 2 Re(A conj x)
+//   d2(s^2 A)[a,b]   = 2 (s_A(a) s_A(b) + s s_ab) A + 2 s (s_A(a) b + s_A(b) a)
+//   d3(s A)[a,b,c]   = s_ab c + s_ac b + s_bc a
+//   d3(s^2 A)[a,b,c] = 2 (s_ab s_A(c) + s_ac s_A(b) + s_bc s_A(a)) A + 2 (s_A(a) s_A(b) + s s_ab) c
+//                      + 2 (s_A(a) s_A(c) + s s_ac) b + 2 (s_A(b) s_A(c) + s s_bc) a
+template <int ORDER>
+__device__ __forceinline__ void cgl_jet(const CglPar& p, double2 A, double2 a, double2 b, double2 c, double& o1, double& o2) {
+  auto sdot = [](double2 x, double2 y) { return 2.0 * (x.x * y.x + x.y * y.y); };
+  double2 t3, t5;  // the jets of |A|^2 A and |A|^4 A
+  const double sab = sdot(a, b);
+  if (ORDER == 2) {
+    const double s = sdot(A, A) * 0.5, sa = sdot(A, a), sb = sdot(A, b);
+    t3.x = sab * A.x + sa * b.x + sb * a.x;
+    t3.y = sab * A.y + sa * b.y + sb * a.y;
+    const double k = 2.0 * (sa * sb + s * sab);
+    t5.x = k * A.x + 2.0 * s * (sa * b.x + sb * a.x);
+    t5.y = k * A.y + 2.0 * s * (sa * b.y + sb * a.y);
+  } else {
+    const double s = sdot(A, A) * 0.5, sa = sdot(A, a), sb = sdot(A, b), sc = sdot(A, c);
+    const double sac = sdot(a, c), sbc = sdot(b, c);
+    t3.x = sab * c.x + sac * b.x + sbc * a.x;
+    t3.y = sab * c.y + sac * b.y + sbc * a.y;
+    const double k = 2.0 * (sab * sc + sac * sb + sbc * sa);
+    const double kc = 2.0 * (sa * sb + s * sab), kb = 2.0 * (sa * sc + s * sac), ka = 2.0 * (sb * sc + s * sbc);
+    t5.x = k * A.x + kc * c.x + kb * b.x + ka * a.x;
+    t5.y = k * A.y + kc * c.y + kb * b.y + ka * a.y;
+  }
+  o1 = -(p.c3 * t3.x - p.mu * t3.y) - p.c5 * t5.x;
+  o2 = -(p.c3 * t3.y + p.mu * t3.x) - p.c5 * t5.y;
+}
+template <int ORDER>
+static __global__ void __launch_bounds__(256) k_jet(OpDesc op, const double* u, const double* a, const double* b,
+                                                    const double* c, double* out, long long n) {
+  bk_pdl_sync();
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < n; g += (long long)gridDim.x * blockDim.x) {
+    if (op.kind == BK_CGL2D) {
+      const CglPar p = cgl_par(op);
+      const double2 A = make_double2(u[g], u[g + n]);
+      const double2 da = make_double2(a[g], a[g + n]), db = make_double2(b[g], b[g + n]);
+      const double2 dc = ORDER == 3 ? make_double2(c[g], c[g + n]) : make_double2(0.0, 0.0);
+      double o1, o2;
+      cgl_jet<ORDER>(p, A, da, db, dc, o1, o2);
+      out[g] = o1;
+      out[g + n] = o2;
+    } else if (op.kind == BK_CHAN) {
+      const double x = u[g];
+      const bool interior = g > 0 && g < n - 1;
+      const double ab = a[g] * b[g];
+      double r;
+      if (ORDER == 2) r = op.par[0] * chan_d2Nl(x, op.par[1]) * ab;
+      else r = op.par[0] * chan_d3Nl(x, op.par[1]) * ab * c[g];
+      out[g] = interior ? r : 0.0;
+    } else {  // BK_SH2D, BK_SH3D, BK_SH2D_PERIODIC: F = -L1 u + l u + nu u^2 - u^3
+      const double ab = a[g] * b[g];
+      out[g] = ORDER == 2 ? (2.0 * op.par[1] - 6.0 * u[g]) * ab : -6.0 * ab * c[g];
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------ tail reductions
 // out[N_tail] = alpha * sum_i x[i]*(scale) * y[i] + beta0   (+ optional elementwise border fix)
 //   potrap phase condition:   out[n] = s * <in, phi> - <xpi, phi>(residual only)
@@ -506,6 +581,37 @@ extern "C" int32_t bk_jvp(bk_ctx* c, const double* v, double* out, double a0, do
   OpDesc op = bk_make_op(c, a0, a1);
   BK_TRY(bk_launch_apply(c, op, dv, nullptr, dout));
   return bk_stage_out(c, out, c->N, dout);
+}
+
+// d2F (dx3 == nullptr) or d3F at the context's current params; every vector N0 doubles, host or device
+static int jet(bk_ctx* c, const double* u, const double* dx1, const double* dx2, const double* dx3, double* out) {
+  BK_CHECK(c, bk_kind_traits(c->kind)->has_jets, "d2F / d3F are not available for this problem kind");
+  BK_CHECK(c, !c->cplx, "d2F / d3F act on real states: not available in a BK_COMPLEX context");
+  const long long n = c->N0;
+  double *du, *d1, *d2, *d3 = nullptr, *dout;
+  BK_TRY(bk_stage_in(c, u, n, 0, true, &du));
+  BK_TRY(bk_stage_in(c, dx1, n, 2, true, &d1));
+  BK_TRY(bk_stage_in(c, dx2, n, 3, true, &d2));
+  if (dx3) BK_TRY(bk_stage_in(c, dx3, n, 4, true, &d3));
+  BK_TRY(bk_stage_in(c, out, n, 1, false, &dout));
+  const OpDesc op = bk_make_residual_op(c);
+  const long long pts = n / bk_kind_traits(c->kind)->fields;
+  if (dx3) BK_TRY(bk_launch(c, k_jet<3>, bk_lin_grid(c, pts), 256, 0, op, du, d1, d2, d3, dout, pts));
+  else BK_TRY(bk_launch(c, k_jet<2>, bk_lin_grid(c, pts), 256, 0, op, du, d1, d2, d3, dout, pts));
+  return bk_stage_out(c, out, n, dout);
+}
+
+extern "C" int32_t bk_d2f(bk_ctx* c, const double* u, const double* dx1, const double* dx2, double* out) {
+  BK_ENTER(c);
+  BkRange nvtx_range("bk_d2f");
+  return jet(c, u, dx1, dx2, nullptr, out);
+}
+
+extern "C" int32_t bk_d3f(bk_ctx* c, const double* u, const double* dx1, const double* dx2, const double* dx3, double* out) {
+  BK_ENTER(c);
+  BkRange nvtx_range("bk_d3f");
+  BK_CHECK(c, dx3 != nullptr, "null vector argument");
+  return jet(c, u, dx1, dx2, dx3, out);
 }
 
 extern "C" int32_t bk_bls_map(bk_ctx* c, const double* a, const double* b, double bc, int32_t has_shift, double shift,

@@ -59,6 +59,7 @@ class SpecialPoint:
     x: object = None
     tau_p: float = 0.0
     precision: float = -1.0
+    tau_u: object = None   # tangent at x (bifpt.τ.u), read by the Transcritical predictor (src/NormalForms.jl:410)
 
 
 # ------------------------------------------------------------------------------------------------ state helpers
@@ -111,7 +112,7 @@ def get_bifurcation_type(it, st, status, interval, floquet=False):
         raise RuntimeError(f"We could not detect/identify the bifurcation point. (dn_unstable, dn_imag) = ({dn}, {di})")
     return SpecialPoint(type=tp, idx=st.step, param=st.z_p, norm=it.normC(st.z_u), step=st.step, status=status,
                         delta=(n_unstable - n_unstable_prev, n_imag - n_imag_prev), ind_ev=ind_ev, interval=tuple(interval),
-                        x=V.copy(st.z_u), tau_p=st.tau_p, precision=abs(interval[1] - interval[0]))
+                        x=V.copy(st.z_u), tau_p=st.tau_p, precision=abs(interval[1] - interval[0]), tau_u=V.copy(st.tau_u))
 
 
 def locate_fold(rows, specialpoints, it, st):
@@ -200,14 +201,15 @@ class Branch:
     state: object = None
 
 
-def continuation(prob, alg, contpar, normC=V.norm2, verbose=False, callback=None, floquet=False):
+def continuation(prob, alg, contpar, normC=V.norm2, verbose=False, callback=None, floquet=False, u1=None, p1=None):
     """continuation(prob, PALC(...), ContinuationPar(detect_bifurcation = 0..3)) with special points
     (src/Continuation.jl:349-400 start-up, :506-575 loop): the loop of palc.continuation with the detection before each
-    row is saved.  Returns a Branch (rows as palc.continuation + `n_imag`, `stable`; specialpoint list ends with the
-    :endpoint)."""
+    row is saved.  With (u1, p1) the branch starts from the two points (prob.u0, prob.p0), (u1, p1) (iterate_from_two_points,
+    src/Continuation.jl:408-456), as branch switching does.  Returns a Branch (rows as palc.continuation + `n_imag`, `stable`;
+    specialpoint list ends with the :endpoint)."""
     cp = contpar
     it = ContIterable(prob, alg, cp, normC)
-    st = it.start()
+    st = it.start(u1, p1)
     it.eigen(st)
     br = Branch(state=st)
 

@@ -23,7 +23,7 @@ SYMBOLS = [
     "bk_set_timing", "bk_sync", "bk_stream",
     "bk_vec_alloc", "bk_vec_free", "bk_host_alloc", "bk_host_free", "bk_vec_upload", "bk_vec_download", "bk_vec_copy", "bk_vec_zero", "bk_vec_scale",
     "bk_vec_axpby", "bk_vec_dot", "bk_vec_norm2", "bk_vec_norminf", "bk_vec_diffdot",
-    "bk_residual", "bk_jac_set_state", "bk_jvp", "bk_jac_set_shift_imag", "bk_jac_set_transpose", "bk_precond_setup", "bk_precond_apply",
+    "bk_residual", "bk_jac_set_state", "bk_jvp", "bk_jac_set_shift_imag", "bk_jac_set_transpose", "bk_d2f", "bk_d3f", "bk_precond_setup", "bk_precond_apply",
     "bk_gmres", "bk_gmres2", "bk_bls_bordering", "bk_bls_matrixfree", "bk_bls_map",
     "bk_bls_block_bordering", "bk_bls_block_matrixfree", "bk_bls_block_map",
     "bk_eigs_shift_invert", "bk_potrap_set_section", "bk_hessenberg_eig", "bk_palc_run",
@@ -116,6 +116,8 @@ def load():
         "bk_jvp": [C.c_void_p, vp, vp, dbl, dbl],
         "bk_jac_set_shift_imag": [C.c_void_p, dbl],
         "bk_jac_set_transpose": [C.c_void_p, i32],
+        "bk_d2f": [C.c_void_p, vp, vp, vp, vp],
+        "bk_d3f": [C.c_void_p, vp, vp, vp, vp, vp],
         "bk_precond_setup": [C.c_void_p, i32, dbl, dbl],
         "bk_precond_apply": [C.c_void_p, vp, vp],
         "bk_gmres": [C.c_void_p, vp, vp, dbl, dbl, C.POINTER(GmresOpts), C.POINTER(i32), C.POINTER(i32), dp],

@@ -172,6 +172,22 @@ class BifurcationProblemB200:
         self._set(p)
         return self.ctx.jacobian(x)
 
+    def d2F(self, x, p, dx1, dx2, out=None):
+        """second differential of F in x (src/Problems.jl:165)"""
+        self._set(p)
+        return self.ctx.d2f(x, dx1, dx2, out)
+
+    def d3F(self, x, p, dx1, dx2, dx3, out=None):
+        """third differential of F in x (src/Problems.jl:180)"""
+        self._set(p)
+        return self.ctx.d3f(x, dx1, dx2, dx3, out)
+
+    @property
+    def symmetric(self):
+        """is_symmetric(prob) (src/Problems.jl:126): J' = J for the Swift-Hohenberg kinds"""
+        from . import lib as _l
+        return (self.ctx.kind & ~_l.BK_COMPLEX) in (_l.BK_SH2D, _l.BK_SH3D, _l.BK_SH2D_PERIODIC)
+
 
 @dataclass
 class NonLinearSolution:

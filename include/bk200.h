@@ -142,6 +142,16 @@ int32_t bk_jac_set_shift_imag(bk_ctx* ctx, double a0_imag);
 /* apply J' instead of J from now on: apply_jacobian(prob, x, par, dx, true) / jacobian_adjoint (src/codim2/MinAugHopf.jl:79-81,
  * 152-155).  SH2d / SH3d / periodic SH2d are self-adjoint (no-op), cGL2d transposes its 2 x 2 reaction block; BK_CHAN / BK_POTRAP_CGL2D: error */
 int32_t bk_jac_set_transpose(bk_ctx* ctx, int32_t on);
+/* d2F(u; params)[dx1, dx2] and d3F(u; params)[dx1, dx2, dx3]: second / third differential of F in u at the
+ * context's current params (bk_set_params, as bk_residual).  Host or device pointers, N0 doubles each.
+ * (prob.VF.d2F / d3F, src/Problems.jl:107-110,165-183.)  The linear parts of F drop out, so both are pointwise:
+ *   SH2d / SH3d / periodic SH2d: (2 nu - 6 u) a b  and  -6 a b c
+ *   chan: alpha Nl''(u) a b  and  alpha Nl'''(u) a b c on interior rows (chan.jl:7 with b = beta, as F), 0 on the boundary rows
+ *   cGL2d: the real-multilinear 2nd / 3rd derivative of NL(A) = (r + i nu) A - (c3 + i mu) |A|^2 A - c5 |A|^4 A, A = u1 + i u2
+ * BK_POTRAP_CGL2D and BK_COMPLEX contexts: BK_ERR_ARG, nothing launched (a complex form is composed from four real calls,
+ * src/Problems.jl:171-178). */
+int32_t bk_d2f(bk_ctx* ctx, const double* u, const double* dx1, const double* dx2, double* out);
+int32_t bk_d3f(bk_ctx* ctx, const double* u, const double* dx1, const double* dx2, const double* dx3, double* out);
 
 /* ---- K6: preconditioner --------------------------------------------------------------------- */
 int32_t bk_precond_setup(bk_ctx* ctx, int32_t kind, double a0, double a1); /* SH_DCT, SH_FFT: (L1 + a0 I)^-1; CGL_DST: (a0 I + a1 Lap)^-1 */

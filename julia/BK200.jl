@@ -14,6 +14,12 @@
 #   ls   = BK200.GMRESB200(ctx; reltol = 1e-5, Pr = true)
 #   opts = ContinuationPar(...; newton_options = NewtonPar(linsolver = ls, eigsolver = BK200.ShiftInvertB200(ctx, 0.1, ls)))
 #   br   = continuation(prob, PALC(bls = BK200.BorderingBLSB200(ls)), opts; normC = norminf)
+# Branch switching (get_normal_form / continuation(br, ind_bif, ...), cf. examples/SH2d-fronts.jl:59,95,137) also needs the second
+# and third differentials; they come from the same context, and SH's Jacobian is symmetric:
+#   prob = BifurcationProblem(F, u0, (l = -0.1, ν = 1.3), (@optic _.l); J = ...,
+#                             d2F = (u, p, dx1, dx2) -> BK200.d2F(ctx, u, (p.l, p.ν), dx1, dx2),
+#                             d3F = (u, p, dx1, dx2, dx3) -> BK200.d3F(ctx, u, (p.l, p.ν), dx1, dx2, dx3), issymmetric = true)
+#   bp   = get_normal_form(br, 1; autodiff = false, bls = BK200.MatrixFreeBLSB200(ls))
 module BK200
 
 using BifurcationKit, LinearAlgebra
@@ -129,6 +135,24 @@ end
 function (J::Jac)(dx; a₀ = 0.0, a₁ = 1.0)
     out = like(J.ctx, dx)
     check(J.ctx, ccall((:bk_jvp, lib), Int32, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Float64, Float64), J.ctx.handle, ptr(dx), ptr(out), a₀, a₁))
+    out
+end
+
+"d2F(u, p)[dx1, dx2]: prob.VF.d2F (src/Problems.jl:107-110,165), pointwise on the device (bk_d2f)"
+function d2F(c::Context, u, params, dx1, dx2)
+    setparams!(c, params)
+    out = like(c, u)
+    check(c, ccall((:bk_d2f, lib), Int32, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                   c.handle, ptr(u), ptr(dx1), ptr(dx2), ptr(out)))
+    out
+end
+
+"d3F(u, p)[dx1, dx2, dx3]: prob.VF.d3F (src/Problems.jl:107-110,180), pointwise on the device (bk_d3f)"
+function d3F(c::Context, u, params, dx1, dx2, dx3)
+    setparams!(c, params)
+    out = like(c, u)
+    check(c, ccall((:bk_d3f, lib), Int32, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                   c.handle, ptr(u), ptr(dx1), ptr(dx2), ptr(dx3), ptr(out)))
     out
 end
 
