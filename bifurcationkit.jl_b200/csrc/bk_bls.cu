@@ -84,58 +84,11 @@ extern "C" int32_t bk_bls_bordering(bk_ctx* c, const double* dR, const double* d
   return cv ? BK_OK : BK_NOT_CONVERGED;
 }
 
-static __global__ void k_set_tail(double* v, long long idx, double val) { v[idx] = val; }
-
-extern "C" int32_t bk_bls_matrixfree(bk_ctx* c, const double* dR, const double* dzu, double dzp, const double* R, double n,
-                                     double xiu, double xip, int32_t has_shift, double shift, double dotscale,
-                                     const bk_gmres_opts* opts, double* dX, double* dl, int32_t* converged, int32_t* iters) {
-  BK_ENTER(c);
-  BkRange nvtx_range("bk_bls_matrixfree");
-  BK_CHECK(c, c->have_state, "bk_jac_set_state must be called first");
-  BK_CHECK(c, opts != nullptr, "opts required");
-  const long long N = c->N;
-  double *d_dR, *d_dzu, *d_R;
-  BK_TRY(bk_stage_in(c, dR, N, 6, true, &d_dR));
-  BK_TRY(bk_stage_in(c, dzu, N, 7, true, &d_dzu));
-  BK_TRY(bk_stage_in(c, R, N, 8, true, &d_R));
-  double *rhs, *sol;
-  BK_TRY(bk_tmp(c, 0, &rhs));
-  BK_TRY(bk_tmp(c, 1, &sol));
-  BK_TRY(bk_dev_copy(c, rhs, d_R, N));
-  k_set_tail<<<1, 1, 0, c->stream>>>(rhs, N, n);
-  c->stats.kernel_launches++;
-  // linearmap = MatrixFreeBLSmap(J, dR, xiu*dzu, dzp*xip, shift, dotp)  (:433)
-  OpDesc op = bk_make_op(c, 0.0, 1.0);
-  op.bordered = 1;
-  op.ba = d_dR;
-  op.bb = d_dzu;
-  op.bscale = dotscale * xiu;
-  op.bc = dzp * xip;
-  op.bshift = has_shift ? shift : 0.0;
-  int cv = 0, it = 0;
-  int st = bk_gmres_dev(c, op, rhs, sol, opts, &cv, &it, nullptr);
-  if (st < 0) return st;
-  double tail = 0;
-  BK_CUDA(c, cudaMemcpyAsync(c->red_pinned + 1, sol + N, 8, cudaMemcpyDeviceToHost, c->stream));
-  BK_CUDA(c, cudaStreamSynchronize(c->stream));
-  tail = c->red_pinned[1];
-  if (dl) *dl = tail;
-  if (converged) *converged = cv;
-  if (iters) *iters = it;
-  if (bk_is_device_ptr(dX)) {
-    BK_TRY(bk_dev_copy(c, dX, sol, N));
-    BK_CUDA(c, cudaStreamSynchronize(c->stream));
-  } else {
-    BK_TRY(bk_stage_out(c, dX, N, sol));
-  }
-  return cv ? BK_OK : BK_NOT_CONVERGED;
-}
-
 // ------------------------------------------------------------------------------------------------ block / tuple borders
 // solve_bls_block (src/LinearBorderSolver.jl:168-206 BorderingBLS, :440-450 MatrixFreeBLS over the tuple form of
 // MatrixFreeBLSmap :338-389):   [ shift I + J   a_1 .. a_m ] [u]   [rhst]
 //                               [ dotp(b_i, .)      c      ] [p] = [rhsb]       m = 1 or 2 (the Hopf / codim-2 systems)
-// cmat is m x m, column-major (Julia layout).
+// cmat is m x m, column-major (Julia layout).  One border (MatrixFreeBLS :404-437, MatrixFreeBLSmap :299-335) is m = 1.
 static int stage_borders(bk_ctx* c, int m, const double* const* a, const double* const* b, double* da[2], double* db[2]) {
   static const int slot_a[2] = {6, 12}, slot_b[2] = {7, 13};
   for (int i = 0; i < m; ++i) {
@@ -161,12 +114,8 @@ static void set_block_borders(OpDesc& op, int m, double* const da[2], double* co
   op.bscale = dotscale;
 }
 
-extern "C" int32_t bk_bls_block_map(bk_ctx* c, int32_t m, const double* const* a, const double* const* b, const double* cmat,
-                                    int32_t has_shift, double shift, double dotscale, const double* x, double* out) {
-  BK_ENTER(c);
-  BK_CHECK(c, c->have_state, "bk_jac_set_state must be called first");
-  BK_CHECK(c, m == 1 || m == 2, "block borders: m must be 1 or 2");
-  BK_CHECK(c, a && b && cmat, "null border");
+static int block_map(bk_ctx* c, int m, const double* const* a, const double* const* b, const double* cmat, int has_shift,
+                     double shift, double dotscale, const double* x, double* out) {
   double *da[2], *db[2], *dx, *dout;
   BK_TRY(stage_borders(c, m, a, b, da, db));
   BK_TRY(bk_stage_in(c, x, c->N + m, 0, true, &dx));
@@ -177,16 +126,32 @@ extern "C" int32_t bk_bls_block_map(bk_ctx* c, int32_t m, const double* const* a
   return bk_stage_out(c, out, c->N + m, dout);
 }
 
-extern "C" int32_t bk_bls_block_matrixfree(bk_ctx* c, int32_t m, const double* const* a, const double* const* b,
-                                           const double* cmat, const double* rhst, const double* rhsb, int32_t has_shift,
-                                           double shift, double dotscale, const bk_gmres_opts* opts, double* solu, double* solp,
-                                           int32_t* converged, int32_t* iters) {
+extern "C" int32_t bk_bls_map(bk_ctx* c, const double* a, const double* b, double bc, int32_t has_shift, double shift,
+                              double dotscale, const double* x, double* out) {
   BK_ENTER(c);
-  BkRange nvtx_range("bk_bls_block_matrixfree");
   BK_CHECK(c, c->have_state, "bk_jac_set_state must be called first");
-  BK_CHECK(c, opts != nullptr, "opts required");
+  return block_map(c, 1, &a, &b, &bc, has_shift, shift, dotscale, x, out);
+}
+
+extern "C" int32_t bk_bls_block_map(bk_ctx* c, int32_t m, const double* const* a, const double* const* b, const double* cmat,
+                                    int32_t has_shift, double shift, double dotscale, const double* x, double* out) {
+  BK_ENTER(c);
+  BK_CHECK(c, c->have_state, "bk_jac_set_state must be called first");
   BK_CHECK(c, m == 1 || m == 2, "block borders: m must be 1 or 2");
-  BK_CHECK(c, a && b && cmat && rhsb && solp, "null border");
+  BK_CHECK(c, a && b && cmat, "null border");
+  return block_map(c, m, a, b, cmat, has_shift, shift, dotscale, x, out);
+}
+
+// the border entries of the right-hand side: v[0] = p0 (, v[1] = p1)
+static __global__ void k_set_tail(double* v, int m, double p0, double p1) {
+  v[0] = p0;
+  if (m == 2) v[1] = p1;
+}
+
+// rhs = vcat(rhst, rhsb) (use_bordered_array = false, :414,:434), one GMRES on the (N + m)-system; rhsb and solp on the host
+static int block_matrixfree(bk_ctx* c, int m, const double* const* a, const double* const* b, const double* cmat,
+                            const double* rhst, const double* rhsb, int has_shift, double shift, double dotscale,
+                            const bk_gmres_opts* opts, double* solu, double* solp, int32_t* converged, int32_t* iters) {
   const long long N = c->N;
   double *da[2], *db[2], *d_R;
   BK_TRY(stage_borders(c, m, a, b, da, db));
@@ -195,7 +160,7 @@ extern "C" int32_t bk_bls_block_matrixfree(bk_ctx* c, int32_t m, const double* c
   BK_TRY(bk_tmp(c, 0, &rhs));
   BK_TRY(bk_tmp(c, 1, &sol));
   BK_TRY(bk_dev_copy(c, rhs, d_R, N));
-  BK_CUDA(c, cudaMemcpyAsync(rhs + N, rhsb, 8 * (size_t)m, cudaMemcpyHostToDevice, c->stream));  // rhs = vcat(rhst, rhsb)
+  BK_TRY(bk_launch_ordered(c, k_set_tail, 1, 1, 0, rhs + N, m, rhsb[0], m == 2 ? rhsb[1] : 0.0));
   OpDesc op = bk_make_op(c, 0.0, 1.0);
   set_block_borders(op, m, da, db, cmat, has_shift, shift, dotscale);
   int cv = 0, it = 0;
@@ -213,6 +178,34 @@ extern "C" int32_t bk_bls_block_matrixfree(bk_ctx* c, int32_t m, const double* c
     BK_TRY(bk_stage_out(c, solu, N, sol));
   }
   return cv ? BK_OK : BK_NOT_CONVERGED;
+}
+
+extern "C" int32_t bk_bls_matrixfree(bk_ctx* c, const double* dR, const double* dzu, double dzp, const double* R, double n,
+                                     double xiu, double xip, int32_t has_shift, double shift, double dotscale,
+                                     const bk_gmres_opts* opts, double* dX, double* dl, int32_t* converged, int32_t* iters) {
+  BK_ENTER(c);
+  BkRange nvtx_range("bk_bls_matrixfree");
+  BK_CHECK(c, c->have_state, "bk_jac_set_state must be called first");
+  BK_CHECK(c, opts != nullptr, "opts required");
+  // linearmap = MatrixFreeBLSmap(J, dR, xiu*dzu, dzp*xip, shift, dotp)  (:433)
+  const double cm = dzp * xip;
+  double p = 0;
+  const int st = block_matrixfree(c, 1, &dR, &dzu, &cm, R, &n, has_shift, shift, dotscale * xiu, opts, dX, &p, converged, iters);
+  if (st >= 0 && dl) *dl = p;
+  return st;
+}
+
+extern "C" int32_t bk_bls_block_matrixfree(bk_ctx* c, int32_t m, const double* const* a, const double* const* b,
+                                           const double* cmat, const double* rhst, const double* rhsb, int32_t has_shift,
+                                           double shift, double dotscale, const bk_gmres_opts* opts, double* solu, double* solp,
+                                           int32_t* converged, int32_t* iters) {
+  BK_ENTER(c);
+  BkRange nvtx_range("bk_bls_block_matrixfree");
+  BK_CHECK(c, c->have_state, "bk_jac_set_state must be called first");
+  BK_CHECK(c, opts != nullptr, "opts required");
+  BK_CHECK(c, m == 1 || m == 2, "block borders: m must be 1 or 2");
+  BK_CHECK(c, a && b && cmat && rhsb && solp, "null border");
+  return block_matrixfree(c, m, a, b, cmat, rhst, rhsb, has_shift, shift, dotscale, opts, solu, solp, converged, iters);
 }
 
 extern "C" int32_t bk_bls_block_bordering(bk_ctx* c, int32_t m, const double* const* a, const double* const* b,

@@ -250,12 +250,17 @@ int bk_fail(bk_ctx* c, int code, const char* what, const char* file, int line);
   } while (0)
 
 // ---- host-side internal API (cross-TU) ----------------------------------------------------------
-// Grid of the 256-thread grid-stride kernels: one CTA per 256 values, at most 8 per SM.  It fixes the summation order of every
-// k_reduce / k_tail reduction, and with it the rounding of the continuation (DESIGN.md §7).
+// Grid of the 256-thread grid-stride kernels: one CTA per 256 values, at most 8 per SM.
 static inline int bk_lin_grid(const bk_ctx* c, long long n) {
   long long g = (n + 255) / 256;
   long long cap = (long long)c->nsm * 8;
   return (int)(g < cap ? (g > 0 ? g : 1) : cap);
+}
+// Grid of the bk_grid_reduce kernels (k_reduce, k_tail, k_potrap_phase): bk_lin_grid, at most one CTA per partial-sum column.
+// It fixes the summation order of every such reduction, and with it the rounding of the continuation (DESIGN.md §7).
+static inline int bk_reduce_grid(const bk_ctx* c, long long n) {
+  const int g = bk_lin_grid(c, n);
+  return g < c->gmax ? g : c->gmax;
 }
 // 1/h^2 along dimension d, with h = 2 l / n in every example (SH2d-fronts.jl:14-15, SH3d.jl:18-20, cGL2d.jl:7-8)
 static inline double bk_inv_h2(const bk_ctx* c, int d) {
@@ -320,10 +325,11 @@ static inline void bk_ensure_smem(bk_ctx* c, K kern, size_t bytes) {
   }
 }
 
-// ---- programmatic dependent launch (PDL): the next kernel of the stream is launched while this one drains ---------
+// ---- kernel launches on the context's stream ------------------------------------------------------------------------
 #ifdef __CUDACC__
+// launch kern on stream st.  With pdl (programmatic dependent launch) the kernel is launched while the previous one drains.
 template <typename... KArgs, typename... Args>
-static inline cudaError_t bk_launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+static inline cudaError_t bk_launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl,
                                         Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
@@ -336,19 +342,30 @@ static inline cudaError_t bk_launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 
   cfg.attrs = at;
   static int no_pdl = -1;  // BK_NO_PDL=1: plain stream order (diagnostics)
   if (no_pdl < 0) no_pdl = getenv("BK_NO_PDL") ? 1 : 0;
-  cfg.numAttrs = no_pdl ? 0 : 1;
+  cfg.numAttrs = pdl && !no_pdl ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
-// grant `smem` bytes of dynamic shared memory to kern, launch it with PDL on the context's stream, check and count the launch
+// grant `smem` bytes of dynamic shared memory to kern, launch it on the context's stream, check and count the launch
 template <typename... KArgs, typename... Args>
-static inline int bk_launch(bk_ctx* c, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, Args&&... args) {
-  bk_ensure_smem(c, kern, smem);
-  bk_launch_pdl(kern, grid, block, smem, c->stream, static_cast<Args&&>(args)...);
+static inline int bk_launch_ex(bk_ctx* c, bool pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
+                               Args&&... args) {
+  if (smem) bk_ensure_smem(c, kern, smem);
+  bk_launch_pdl(kern, grid, block, smem, c->stream, pdl, static_cast<Args&&>(args)...);
   BK_CUDA(c, cudaGetLastError());
   c->stats.kernel_launches++;
   return BK_OK;
 }
-// first statement of every kernel launched through bk_launch_pdl: wait for the previous grid's memory, then let the next
+// PDL launch: kern must begin with bk_pdl_sync
+template <typename... KArgs, typename... Args>
+static inline int bk_launch(bk_ctx* c, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, Args&&... args) {
+  return bk_launch_ex(c, true, kern, grid, block, smem, static_cast<Args&&>(args)...);
+}
+// stream-ordered launch: kern starts once the previous kernel of the stream has finished
+template <typename... KArgs, typename... Args>
+static inline int bk_launch_ordered(bk_ctx* c, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, Args&&... args) {
+  return bk_launch_ex(c, false, kern, grid, block, smem, static_cast<Args&&>(args)...);
+}
+// first statement of every kernel launched through bk_launch: wait for the previous grid's memory, then let the next
 // grid start launching (its CTAs block at their own wait)
 __device__ __forceinline__ void bk_pdl_sync() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -386,5 +403,48 @@ __device__ __forceinline__ bool bk_last_block(unsigned int* counter, int* s_flag
   bool last = (*s_flag != 0);
   if (last) __threadfence();
   return last;
+}
+template <bool MAX>
+__device__ __forceinline__ double bk_red(double a, double b) { return MAX ? bk_nanmax(a, b) : a + b; }
+// Deterministic two-level reduction of K <= 2 values per thread over a grid of 256-thread CTAs: sums, or bk_nanmax (MAX).
+// Each CTA reduces its warps by shuffles, then folds the 8 warp results in order, starting from 0.0, into the partial
+// partials[k * gridDim.x + blockIdx.x]; the last CTA to arrive folds the gridDim.x partials the same way.  Returns true in
+// thread 0 of that CTA only, with the grid totals in v.  The order depends on the grid alone (bk_reduce_grid).
+template <int K, bool MAX = false>
+__device__ __forceinline__ bool bk_grid_reduce(double (&v)[K], double* __restrict__ partials, unsigned int* counter) {
+  __shared__ double s_w[K][8];
+  __shared__ int s_flag;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    const double t = MAX ? bk_warp_max(v[k]) : bk_warp_sum(v[k]);
+    if (lane == 0) s_w[k][wid] = t;
+  }
+  __syncthreads();
+  if (threadIdx.x < K) {
+    double t = 0.0;
+    for (int w = 0; w < 8; ++w) t = bk_red<MAX>(t, s_w[threadIdx.x][w]);
+    partials[(size_t)threadIdx.x * gridDim.x + blockIdx.x] = t;
+  }
+  if (!bk_last_block(counter, &s_flag)) return false;
+  double t[K];
+#pragma unroll
+  for (int k = 0; k < K; ++k) t[k] = 0.0;
+  for (int i = threadIdx.x; i < (int)gridDim.x; i += blockDim.x)
+#pragma unroll
+    for (int k = 0; k < K; ++k) t[k] = bk_red<MAX>(t[k], __ldcg(partials + (size_t)k * gridDim.x + i));
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    t[k] = MAX ? bk_warp_max(t[k]) : bk_warp_sum(t[k]);
+    if (lane == 0) s_w[k][wid] = t[k];
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return false;
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    v[k] = 0.0;
+    for (int w = 0; w < 8; ++w) v[k] = bk_red<MAX>(v[k], s_w[k][w]);
+  }
+  return true;
 }
 #endif

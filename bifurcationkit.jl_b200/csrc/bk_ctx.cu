@@ -330,16 +330,10 @@ static __global__ void __launch_bounds__(256) k_scale(double* __restrict__ x, do
 }
 
 int bk_dev_axpby(bk_ctx* c, double* y, double a, const double* x, double b, long long n) {
-  k_axpby<<<bk_lin_grid(c, n), 256, 0, c->stream>>>(y, a, x, b, n);
-  c->stats.kernel_launches++;
-  BK_CUDA(c, cudaGetLastError());
-  return BK_OK;
+  return bk_launch_ordered(c, k_axpby, bk_lin_grid(c, n), 256, 0, y, a, x, b, n);
 }
 int bk_dev_scale(bk_ctx* c, double* x, double a, long long n) {
-  k_scale<<<bk_lin_grid(c, n), 256, 0, c->stream>>>(x, a, n);
-  c->stats.kernel_launches++;
-  BK_CUDA(c, cudaGetLastError());
-  return BK_OK;
+  return bk_launch_ordered(c, k_scale, bk_lin_grid(c, n), 256, 0, x, a, n);
 }
 
 // mode 0: sum x*y ; 1: max |x| ; 2: sum (x - x0)*y
@@ -348,49 +342,21 @@ static __global__ void __launch_bounds__(256) k_reduce(const double* __restrict_
                                                        const double* __restrict__ x0, long long n,
                                                        double* __restrict__ partials, unsigned int* counter,
                                                        double* __restrict__ out) {
-  __shared__ double s_w[8];
-  __shared__ int s_flag;
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   long long stride = (long long)gridDim.x * blockDim.x;
-  double acc = 0.0;
+  double acc[1] = {0.0};
   for (; i < n; i += stride) {
-    if (MODE == 0) acc = fma(x[i], y[i], acc);
-    if (MODE == 1) acc = bk_nanmax(acc, fabs(x[i]));
-    if (MODE == 2) acc = fma(x[i] - x0[i], y[i], acc);
+    if (MODE == 0) acc[0] = fma(x[i], y[i], acc[0]);
+    if (MODE == 1) acc[0] = bk_nanmax(acc[0], fabs(x[i]));
+    if (MODE == 2) acc[0] = fma(x[i] - x0[i], y[i], acc[0]);
   }
-  acc = (MODE == 1) ? bk_warp_max(acc) : bk_warp_sum(acc);
-  int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) s_w[wid] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = s_w[0];
-    for (int k = 1; k < 8; ++k) t = (MODE == 1) ? bk_nanmax(t, s_w[k]) : t + s_w[k];
-    partials[blockIdx.x] = t;
-  }
-  if (bk_last_block(counter, &s_flag)) {
-    double t = 0.0;
-    for (int k = threadIdx.x; k < (int)gridDim.x; k += blockDim.x) {
-      double v = __ldcg(partials + k);
-      t = (MODE == 1) ? bk_nanmax(t, v) : t + v;
-    }
-    t = (MODE == 1) ? bk_warp_max(t) : bk_warp_sum(t);
-    if (lane == 0) s_w[wid] = t;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double r = s_w[0];
-      for (int k = 1; k < 8; ++k) r = (MODE == 1) ? bk_nanmax(r, s_w[k]) : r + s_w[k];
-      out[0] = r;
-    }
-  }
+  if (bk_grid_reduce<1, MODE == 1>(acc, partials, counter)) out[0] = acc[0];
 }
 
 template <int MODE>
 static int reduce_launch(bk_ctx* c, const double* x, const double* y, const double* x0, long long n, double* out_host) {
-  int g = bk_lin_grid(c, n);
-  if (g > c->gmax) g = c->gmax;
-  k_reduce<MODE><<<g, 256, 0, c->stream>>>(x, y, x0, n, c->partials, c->counters + 8, c->red_out);
-  c->stats.kernel_launches++;
-  BK_CUDA(c, cudaGetLastError());
+  BK_TRY(bk_launch_ordered(c, k_reduce<MODE>, bk_reduce_grid(c, n), 256, 0, x, y, x0, n, c->partials, c->counters + 8,
+                           c->red_out));
   BK_CUDA(c, cudaMemcpyAsync(c->red_pinned, c->red_out, 8, cudaMemcpyDeviceToHost, c->stream));
   BK_CUDA(c, cudaStreamSynchronize(c->stream));
   *out_host = c->red_pinned[0];

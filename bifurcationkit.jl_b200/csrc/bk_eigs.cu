@@ -312,7 +312,7 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
     BK_CUDA(c, cudaMalloc(&c->eig_dev, 8 * (size_t)(m + 4) * 6));
     BK_CUDA(c, cudaMallocHost(&c->eig_pinned, 8 * (size_t)(m + 4) * 6));
     c->qcap = m;
-    k_fill_ones<<<(m + 4 + 255) / 256, 256, 0, c->stream>>>(c->eig_dev, m + 4);
+    BK_TRY(bk_launch_ordered(c, k_fill_ones, (m + 4 + 255) / 256, 256, 0, c->eig_dev, m + 4));
   }
   // partial-sum buffer must hold m rows
   BK_CHECK(c, m <= c->m, "krylovdim exceeds the context's krylov_m (partial-sum workspace)");
@@ -329,7 +329,7 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
     cudaMemcpyKind kd = bk_is_device_ptr(v0) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     BK_CUDA(c, cudaMemcpyAsync(x, v0, 8 * (size_t)n, kd, c->stream));
   } else {
-    k_start_vector<<<c->nsm * 4, 256, 0, c->stream>>>(x, n);
+    BK_TRY(bk_launch_ordered(c, k_start_vector, c->nsm * 4, 256, 0, x, n));
   }
   int total_ops = 0;
   std::vector<double> H((size_t)(m + 1) * m);

@@ -181,10 +181,7 @@ static int launch_update(bk_ctx* c, const double* w, long long n, int j, double*
 
 int bk_launch_lincomb(bk_ctx* c, const double* basis, const double* scales, double* x, double beta, long long n, int k,
                       const double* coef_dev) {
-  k_lincomb<<<chunk_grid(n), BK_THREADS, 0, c->stream>>>(x, beta, n, basis, c->ld, k, coef_dev, scales);
-  c->stats.kernel_launches++;
-  BK_CUDA(c, cudaGetLastError());
-  return BK_OK;
+  return bk_launch_ordered(c, k_lincomb, chunk_grid(n), BK_THREADS, 0, x, beta, n, basis, c->ld, k, coef_dev, scales);
 }
 static int launch_lincomb(bk_ctx* c, double* x, double beta, long long n, int k, const double* coef_dev, bool use_scales) {
   return bk_launch_lincomb(c, c->V, use_scales ? c->scales : nullptr, x, beta, n, k, coef_dev);

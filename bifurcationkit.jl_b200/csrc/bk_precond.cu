@@ -500,10 +500,8 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
         cur = A;
         oth = B;
       }
-      k_sh_symbol_div<<<bk_lin_grid(c, N), 256, 0, c->stream>>>(cur, nx, ny, nz, pc.lam[0], pc.lam[1],
-                                                            nd == 3 ? pc.lam[2] : nullptr, pc.a0, scale);
-      c->stats.kernel_launches++;
-      BK_CUDA(c, cudaGetLastError());
+      BK_TRY(bk_launch_ordered(c, k_sh_symbol_div, bk_lin_grid(c, N), 256, 0, cur, nx, ny, nz, pc.lam[0], pc.lam[1],
+                               nd == 3 ? pc.lam[2] : nullptr, pc.a0, scale));
       if (nd == 3) {
         BK_TRY(transform_pass(c, 2, 1, cur, oth, nx, ny, nz, true));
         std::swap(cur, oth);
@@ -530,10 +528,8 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
     double* B = pc.work2;
     BK_TRY(transform_pass(c, 0, 0, in, A, nx, ny, (int)nblk, al));
     BK_TRY(transform_pass(c, 1, 0, A, B, nx, ny, (int)nblk, true));
-    k_helmholtz_symbol_div<<<bk_lin_grid(c, (long long)nx * ny * nblk), 256, 0, c->stream>>>(B, nx, ny, nblk, pc.lam[0], pc.lam[1],
-                                                                                         pc.a0, pc.a1);
-    c->stats.kernel_launches++;
-    BK_CUDA(c, cudaGetLastError());
+    BK_TRY(bk_launch_ordered(c, k_helmholtz_symbol_div, bk_lin_grid(c, (long long)nx * ny * nblk), 256, 0, B, nx, ny, nblk,
+                             pc.lam[0], pc.lam[1], pc.a0, pc.a1));
     BK_TRY(transform_pass(c, 1, 1, B, A, nx, ny, (int)nblk, true));
     BK_TRY(transform_pass(c, 0, 1, A, out, nx, ny, (int)nblk, al));
     if (c->kind == BK_POTRAP_CGL2D) BK_CUDA(c, cudaMemcpyAsync(out + N - 1, in + N - 1, 8, cudaMemcpyDeviceToDevice, c->stream));
@@ -547,18 +543,13 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
     // solve in time per spatial mode, DST-I back
     BK_TRY(transform_pass(c, 0, 0, in, A, nx, ny, nf, al));
     BK_TRY(transform_pass(c, 1, 0, A, Bf, nx, ny, nf, true));
-    k_potrap_time<<<(unsigned)((nn + 127) / 128), 128, 0, c->stream>>>(Bf, nn, nx, M - 1, pc.lam[0], pc.lam[1], pc.po_T / M,
-                                                                    pc.po_r, pc.po_nu, pc.tdft);
-    BK_CUDA(c, cudaGetLastError());
+    BK_TRY(bk_launch_ordered(c, k_potrap_time, (unsigned)((nn + 127) / 128), 128, 0, Bf, nn, nx, M - 1, pc.lam[0], pc.lam[1],
+                             pc.po_T / M, pc.po_r, pc.po_nu, pc.tdft));
     BK_TRY(transform_pass(c, 1, 1, Bf, A, nx, ny, nf, true));
     BK_TRY(transform_pass(c, 0, 1, A, out, nx, ny, nf, al));
-    k_potrap_close<<<(unsigned)((Ns + 255) / 256), 256, 0, c->stream>>>(in, out, Ns, M);
-    c->stats.kernel_launches += 2;
-    BK_CUDA(c, cudaGetLastError());
+    BK_TRY(bk_launch_ordered(c, k_potrap_close, (unsigned)((Ns + 255) / 256), 256, 0, in, out, Ns, M));
   } else if (pc.kind == BK_PC_CHAN_TRIDIAG) {
-    k_thomas<<<1, 32, 0, c->stream>>>(pc.tri, in, out, (int)N);
-    c->stats.kernel_launches++;
-    BK_CUDA(c, cudaGetLastError());
+    BK_TRY(bk_launch_ordered(c, k_thomas, 1, 32, 0, pc.tri, in, out, (int)N));
   }
   if (n > N && !tail_done)
     BK_CUDA(c, cudaMemcpyAsync(out + N, in + N, 8 * (size_t)(n - N), cudaMemcpyDeviceToDevice, c->stream));

@@ -275,108 +275,48 @@ static __global__ void __launch_bounds__(256) k_jet(OpDesc op, const double* u, 
 }
 
 // ------------------------------------------------------------------------------------------ tail reductions
-// out[N_tail] = alpha * sum_i x[i]*(scale) * y[i] + beta0   (+ optional elementwise border fix)
-//   potrap phase condition:   out[n] = s * <in, phi> - <xpi, phi>(residual only)
-//   bordered map (K2'):       out[i] += xp * a[i] + shift * s * in[i];   out[N] = s * (bscale <b, in> + c in[N])
-// mode 0: phase condition; mode 1: border fix.
-template <int MODE>
+// Bordered map with NB = 1 or 2 borders (MatrixFreeBLSmap, src/LinearBorderSolver.jl:299-335; tuple form :338-389), one pass
+// after the operator has written out.u = Op(s x.u):   xp = s x.p,
+//   out.u[i] += xp0 a[i] (+ xp1 a2[i]) + bshift s x.u[i];   out.p = s bscale [<b, x.u>; <b2, x.u>] + [bc bc01; bc10 bc11] xp
+template <int NB>
 static __global__ void __launch_bounds__(256) k_tail(OpDesc op, const double* __restrict__ in,
                                                      const double* __restrict__ in_scale_ptr, double* __restrict__ out,
-                                                     long long n, double beta0, int jvp_mode, double* __restrict__ partials,
-                                                     unsigned int* counter) {
-  __shared__ double s_w[8];
-  __shared__ int s_flag;
+                                                     long long n, double* __restrict__ partials, unsigned int* counter) {
   const double s = in_scale_ptr ? __ldg(in_scale_ptr) : 1.0;
-  double acc = 0.0;
-  const double xp = (MODE == 1) ? s * in[n] : 0.0;
+  const double xp0 = s * in[n], xp1 = NB == 2 ? s * in[n + 1] : 0.0;
+  double acc[NB] = {};
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    double v = in[i];
-    if (MODE == 0) {
-      acc = fma(v, op.phi[i], acc);
+    const double v = in[i];
+    acc[0] = fma(v, op.bb[i], acc[0]);
+    if constexpr (NB == 2) {
+      acc[1] = fma(v, op.bb2[i], acc[1]);
+      out[i] += xp0 * op.ba[i] + xp1 * op.ba2[i] + op.bshift * s * v;
     } else {
-      acc = fma(v, op.bb[i], acc);
-      out[i] += xp * op.ba[i] + op.bshift * s * v;
+      out[i] += xp0 * op.ba[i] + op.bshift * s * v;
     }
   }
-  acc = bk_warp_sum(acc);
-  int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) s_w[wid] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0;
-    for (int k = 0; k < 8; ++k) t += s_w[k];
-    partials[blockIdx.x] = t;
-  }
-  if (bk_last_block(counter, &s_flag)) {
-    double t = 0.0;
-    for (int k = threadIdx.x; k < (int)gridDim.x; k += blockDim.x) t += __ldcg(partials + k);
-    t = bk_warp_sum(t);
-    if (lane == 0) s_w[wid] = t;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double r = 0;
-      for (int k = 0; k < 8; ++k) r += s_w[k];
-      if (MODE == 0) {
-        double ph = s * r - beta0;
-        out[n] = jvp_mode ? op.a0 * s * in[n] + op.a1 * ph : ph;
-      } else {
-        out[n] = s * op.bscale * r + op.bc * xp;
-      }
-    }
+  if (!bk_grid_reduce<NB>(acc, partials, counter)) return;
+  if constexpr (NB == 2) {
+    out[n] = s * op.bscale * acc[0] + op.bc * xp0 + op.bc01 * xp1;
+    out[n + 1] = s * op.bscale * acc[1] + op.bc10 * xp0 + op.bc11 * xp1;
+  } else {
+    out[n] = s * op.bscale * acc[0] + op.bc * xp0;
   }
 }
 
-// two borders (block / tuple MatrixFreeBLSmap, src/LinearBorderSolver.jl:338-389): the same pass with two dot products
-static __global__ void __launch_bounds__(256) k_tail2(OpDesc op, const double* __restrict__ in,
-                                                      const double* __restrict__ in_scale_ptr, double* __restrict__ out,
-                                                      long long n, double* __restrict__ partials, unsigned int* counter) {
-  __shared__ double s_w[16];
-  __shared__ int s_flag;
+// potrap phase condition, the last row: out[n] = s <in, phi> - beta0 (residual, beta0 = <xpi, phi>), or a0 s in[n] + a1 s
+// <in, phi> (JVP)
+static __global__ void __launch_bounds__(256) k_potrap_phase(OpDesc op, const double* __restrict__ in,
+                                                             const double* __restrict__ in_scale_ptr, double* __restrict__ out,
+                                                             long long n, double beta0, int jvp_mode,
+                                                             double* __restrict__ partials, unsigned int* counter) {
   const double s = in_scale_ptr ? __ldg(in_scale_ptr) : 1.0;
-  const double xp0 = s * in[n], xp1 = s * in[n + 1];
-  double acc0 = 0.0, acc1 = 0.0;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const double v = in[i];
-    acc0 = fma(v, op.bb[i], acc0);
-    acc1 = fma(v, op.bb2[i], acc1);
-    out[i] += xp0 * op.ba[i] + xp1 * op.ba2[i] + op.bshift * s * v;
-  }
-  acc0 = bk_warp_sum(acc0);
-  acc1 = bk_warp_sum(acc1);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) {
-    s_w[wid] = acc0;
-    s_w[8 + wid] = acc1;
-  }
-  __syncthreads();
-  if (threadIdx.x < 2) {
-    double t = 0;
-    for (int k = 0; k < 8; ++k) t += s_w[8 * threadIdx.x + k];
-    partials[(size_t)threadIdx.x * gridDim.x + blockIdx.x] = t;
-  }
-  if (bk_last_block(counter, &s_flag)) {
-    double t0 = 0.0, t1 = 0.0;
-    for (int k = threadIdx.x; k < (int)gridDim.x; k += blockDim.x) {
-      t0 += __ldcg(partials + k);
-      t1 += __ldcg(partials + gridDim.x + k);
-    }
-    t0 = bk_warp_sum(t0);
-    t1 = bk_warp_sum(t1);
-    if (lane == 0) {
-      s_w[wid] = t0;
-      s_w[8 + wid] = t1;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double r0 = 0, r1 = 0;
-      for (int k = 0; k < 8; ++k) {
-        r0 += s_w[k];
-        r1 += s_w[8 + k];
-      }
-      out[n] = s * op.bscale * r0 + op.bc * xp0 + op.bc01 * xp1;
-      out[n + 1] = s * op.bscale * r1 + op.bc10 * xp0 + op.bc11 * xp1;
-    }
-  }
+  double acc[1] = {0.0};
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    acc[0] = fma(in[i], op.phi[i], acc[0]);
+  if (!bk_grid_reduce<1>(acc, partials, counter)) return;
+  const double ph = s * acc[0] - beta0;
+  out[n] = jvp_mode ? op.a0 * s * in[n] + op.a1 * ph : ph;
 }
 
 // ------------------------------------------------------------------------------------------ host side
@@ -424,59 +364,38 @@ OpDesc bk_make_residual_op(bk_ctx* c) {
   return op;
 }
 
+// SH2d on the TMA-staged tile (bk_krylov_tma.cuh): the tallest of the tiles E = 8, 4, 2, 1 that still gives every SM about
+// two CTAs
+template <int E, int MODE>
+static int launch_k2_apply(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* out) {
+  const int grid = ((op.nx + BK2_ROW - 1) / BK2_ROW) * ((op.ny + E - 1) / E);
+  if constexpr (E > 1)
+    if (grid < 2LL * c->nsm) return launch_k2_apply<E / 2, MODE>(c, op, in, sp, out);
+  return bk_launch_ordered(c, k2_apply<E, MODE>, grid, BK2_THREADS, Sh2Scratch<E>::BYTES, op, in, sp, out);
+}
+
 template <int MODE>
 static int launch_kind(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* out) {
   switch (op.kind) {
-    case BK_SH2D: {
-      const bool aligned = (op.nx % 2 == 0) && ((((uintptr_t)in) & 15) == 0);
-      if (aligned) {
-        // TMA-staged tile (bk_krylov_tma.cuh): tallest tile that still gives every SM about two CTAs
-        const int tiles_x = (op.nx + BK2_ROW - 1) / BK2_ROW;
-        int E = BK2_EMAX;
-        while (E > 1 && (long long)tiles_x * ((op.ny + E - 1) / E) < 2LL * c->nsm) E >>= 1;
-        const int grid = tiles_x * ((op.ny + E - 1) / E);
-#define BK2A_GO(EE)                                                                                        \
-  do {                                                                                                     \
-    const size_t sm = Sh2Scratch<EE>::BYTES;                                                               \
-    bk_ensure_smem(c, k2_apply<EE, MODE>, sm);                                                             \
-    k2_apply<EE, MODE><<<grid, BK2_THREADS, sm, c->stream>>>(op, in, sp, out);                             \
-  } while (0)
-        if (E == 8) BK2A_GO(8);
-        else if (E == 4) BK2A_GO(4);
-        else if (E == 2) BK2A_GO(2);
-        else BK2A_GO(1);
-#undef BK2A_GO
-        break;
-      }
-      bk_ensure_smem(c, k_sh_apply<2, MODE>, ShSmem<2>::BYTES);
-      k_sh_apply<2, MODE><<<sh_num_tiles<2>(op.nx, op.ny, 1), BK_THREADS, ShSmem<2>::BYTES, c->stream>>>(op, in, sp, out);
-      break;
-    }
-    case BK_SH3D: {
-      bk_ensure_smem(c, k_sh_apply<3, MODE>, ShSmem<3>::BYTES);
-      k_sh_apply<3, MODE><<<sh_num_tiles<3>(op.nx, op.ny, op.nz), BK_THREADS, ShSmem<3>::BYTES, c->stream>>>(op, in, sp, out);
-      break;
-    }
-    case BK_SH2D_PERIODIC:  // spectral: three transform kernels (bk_precond.cu), which count their own launches
+    case BK_SH2D:
+      if ((op.nx % 2 == 0) && ((((uintptr_t)in) & 15) == 0)) return launch_k2_apply<BK2_EMAX, MODE>(c, op, in, sp, out);
+      return bk_launch_ordered(c, k_sh_apply<2, MODE>, sh_num_tiles<2>(op.nx, op.ny, 1), BK_THREADS, ShSmem<2>::BYTES, op, in,
+                               sp, out);
+    case BK_SH3D:
+      return bk_launch_ordered(c, k_sh_apply<3, MODE>, sh_num_tiles<3>(op.nx, op.ny, op.nz), BK_THREADS, ShSmem<3>::BYTES, op,
+                               in, sp, out);
+    case BK_SH2D_PERIODIC:  // spectral: three transform kernels (bk_precond.cu)
       return MODE == 1 ? bk_periodic_residual(c, op, in, out) : bk_periodic_jvp(c, op, in, sp, out);
-    case BK_CHAN: k_chan_apply<MODE><<<bk_lin_grid(c, op.nx), 256, 0, c->stream>>>(op, in, sp, out); break;
-    case BK_CGL2D: k_cgl_apply<MODE><<<bk_lin_grid(c, (long long)op.nx * op.ny), 256, 0, c->stream>>>(op, in, sp, out); break;
-    case BK_POTRAP_CGL2D: {
-      long long tot = (long long)op.nx * op.ny * op.nz;
-      k_potrap_apply<MODE><<<bk_lin_grid(c, tot), 256, 0, c->stream>>>(op, in, sp, out);
-      c->stats.kernel_launches++;
-      BK_CUDA(c, cudaGetLastError());
-      int g = bk_lin_grid(c, op.N - 1);
-      if (g > c->gmax) g = c->gmax;
-      k_tail<0><<<g, 256, 0, c->stream>>>(op, in, sp, out, op.N - 1, (MODE == 1) ? c->phi_dot_xpi : 0.0, MODE == 0 ? 1 : 0,
-                                          c->partials, c->counters + 9);
-      break;
-    }
+    case BK_CHAN: return bk_launch_ordered(c, k_chan_apply<MODE>, bk_lin_grid(c, op.nx), 256, 0, op, in, sp, out);
+    case BK_CGL2D:
+      return bk_launch_ordered(c, k_cgl_apply<MODE>, bk_lin_grid(c, (long long)op.nx * op.ny), 256, 0, op, in, sp, out);
+    case BK_POTRAP_CGL2D:
+      BK_TRY(bk_launch_ordered(c, k_potrap_apply<MODE>, bk_lin_grid(c, (long long)op.nx * op.ny * op.nz), 256, 0, op, in, sp,
+                               out));
+      return bk_launch_ordered(c, k_potrap_phase, bk_reduce_grid(c, op.N - 1), 256, 0, op, in, sp, out, op.N - 1,
+                               (MODE == 1) ? c->phi_dot_xpi : 0.0, MODE == 0 ? 1 : 0, c->partials, c->counters + 9);
     default: return bk_fail(c, BK_ERR_ARG, "unknown kind", __FILE__, __LINE__);
   }
-  c->stats.kernel_launches++;
-  BK_CUDA(c, cudaGetLastError());
-  return BK_OK;
 }
 
 int bk_launch_residual(bk_ctx* c, const double* u, double* out) {
@@ -505,33 +424,20 @@ int bk_launch_apply(bk_ctx* c, const OpDesc& op, const double* in, const double*
     half.bordered = 0;
     BK_TRY(launch_kind<0>(c, half, in, sp, out));
     BK_TRY(launch_kind<0>(c, half, in + half.N, sp, out + half.N));
-    if (op.a0i != 0.0) {
-      k_cshift<<<bk_lin_grid(c, half.N), 256, 0, c->stream>>>(out, in, sp, op.a0i, half.N);
-      c->stats.kernel_launches++;
-      BK_CUDA(c, cudaGetLastError());
-    }
+    if (op.a0i != 0.0) BK_TRY(bk_launch_ordered(c, k_cshift, bk_lin_grid(c, half.N), 256, 0, out, in, sp, op.a0i, half.N));
   } else {
     BK_TRY(launch_kind<0>(c, op, in, sp, out));
   }
-  if (op.bordered) {
-    int g = bk_lin_grid(c, op.N);
-    if (g > c->gmax) g = c->gmax;
-    if (op.bordered == 2) k_tail2<<<g, 256, 0, c->stream>>>(op, in, sp, out, op.N, c->partials, c->counters + 9);
-    else k_tail<1><<<g, 256, 0, c->stream>>>(op, in, sp, out, op.N, 0.0, 0, c->partials, c->counters + 9);
-    c->stats.kernel_launches++;
-    BK_CUDA(c, cudaGetLastError());
-  }
-  return BK_OK;
+  if (!op.bordered) return BK_OK;
+  return bk_launch_ordered(c, op.bordered == 2 ? k_tail<2> : k_tail<1>, bk_reduce_grid(c, op.N), 256, 0, op, in, sp, out, op.N,
+                           c->partials, c->counters + 9);
 }
 
 int bk_potrap_refresh_cache(bk_ctx* c) {
   if (c->kind != BK_POTRAP_CGL2D) return BK_OK;
   OpDesc op = bk_make_op(c, 0, 1);
-  long long tot = (long long)op.nx * op.ny * op.nz;
-  k_potrap_fcache<<<bk_lin_grid(c, tot), 256, 0, c->stream>>>(op, c->u_state, c->fcache);
-  c->stats.kernel_launches++;
-  BK_CUDA(c, cudaGetLastError());
-  return BK_OK;
+  return bk_launch_ordered(c, k_potrap_fcache, bk_lin_grid(c, (long long)op.nx * op.ny * op.nz), 256, 0, op, c->u_state,
+                           c->fcache);
 }
 
 // ------------------------------------------------------------------------------------------ C ABI
@@ -612,26 +518,6 @@ extern "C" int32_t bk_d3f(bk_ctx* c, const double* u, const double* dx1, const d
   BkRange nvtx_range("bk_d3f");
   BK_CHECK(c, dx3 != nullptr, "null vector argument");
   return jet(c, u, dx1, dx2, dx3, out);
-}
-
-extern "C" int32_t bk_bls_map(bk_ctx* c, const double* a, const double* b, double bc, int32_t has_shift, double shift,
-                              double dotscale, const double* x, double* out) {
-  BK_ENTER(c);
-  BK_CHECK(c, c->have_state, "bk_jac_set_state must be called first");
-  double *da, *db, *dx, *dout;
-  BK_TRY(bk_stage_in(c, a, c->N, 2, true, &da));
-  BK_TRY(bk_stage_in(c, b, c->N, 3, true, &db));
-  BK_TRY(bk_stage_in(c, x, c->N + 1, 0, true, &dx));
-  BK_TRY(bk_stage_in(c, out, c->N + 1, 1, false, &dout));
-  OpDesc op = bk_make_op(c, 0.0, 1.0);
-  op.bordered = 1;
-  op.ba = da;
-  op.bb = db;
-  op.bc = bc;
-  op.bshift = has_shift ? shift : 0.0;
-  op.bscale = dotscale;
-  BK_TRY(bk_launch_apply(c, op, dx, nullptr, dout));
-  return bk_stage_out(c, out, c->N + 1, dout);
 }
 
 extern "C" int32_t bk_potrap_set_section(bk_ctx* c, const double* phi, const double* xpi) {

@@ -322,7 +322,7 @@ def test_two_contexts_with_different_krylov_dimensions_interleaved(bk):
 def test_block_bordered_solvers(bk, kind):
     """solve_bls_block with two borders (src/LinearBorderSolver.jl:173-206 BorderingBLS, :440-450 MatrixFreeBLS over the tuple
     map :366-389; exercised with random borders by test/linear_solvers/test_linear.jl:300-320): device path vs the oracle's
-    restatement and vs the explicit (N + 2) x (N + 2) dense solve; also m = 1 against the scalar-border entry points."""
+    restatement and vs the explicit (N + 2) x (N + 2) dense solve; also m = 1 against the scalar-border entry points, bit for bit."""
     rng = np.random.default_rng(31)
     # bordering: residual tolerance 1e-12 x cond(J) = 3e3 (Swift-Hohenberg near its pattern-forming modes), Schur elimination on top.
     # matrix-free: cond of the bordered matrix is 2e4, a relative residual of 1e-12 is below what fp64 attains there (the solve
@@ -356,6 +356,10 @@ def test_block_bordered_solvers(bk, kind):
         x = rng.standard_normal(N + 2)
         assert _rel(bk.bls_map_block(J, a, b, c, x, shift=shift), A @ x) < 1e-12
         assert _rel(bk.bls_map_block(J, a, b, c, x, shift=shift), obls.MatrixFreeBLSmapBlock(Jd, a, b, c, shift, np.dot)(x)) < 1e-12
+        # one border is the block form with m = 1, bit for bit
+        x1 = x[:N + 1]
+        assert np.array_equal(bk.bls_map(J, a[0], b[0], c[0, 0], x1, shift=shift, dotscale=1.0 / N),
+                              bk.bls_map_block(J, (a[0],), (b[0],), [[c[0, 0]]], x1, shift=shift, dotscale=1.0 / N))
         ub, pb, cvb, itb = bk.BorderingBLSB200(ls).solve_block(J, a, b, c, rhst, rhsb, shift=shift)
         assert cvb and _rel(ub, ex[:N]) < TOLB and _rel(pb, ex[N:]) < TOLB and len(itb) == 3, (cvb, itb, _rel(ub, ex[:N]), _rel(pb, ex[N:]))
         um, pm, cvm, itm = bk.MatrixFreeBLSB200(lm).solve_block(J, a, b, c, rhst, rhsb, shift=shift)
@@ -369,7 +373,7 @@ def test_block_bordered_solvers(bk, kind):
     # m = 1 block form == scalar-border entry points
     u1, p1, cv1, _ = bk.MatrixFreeBLSB200(lm).solve_block(J, (a[0],), (b[0],), [[0.7]], rhst, [rhsb[0]])
     us, ps, cvs, _ = bk.MatrixFreeBLSB200(lm)(J, a[0], b[0], 0.7, rhst, rhsb[0])
-    assert cv1 and cvs and _rel(u1, us) < TOLM and abs(p1[0] - ps) < TOLM * max(1.0, abs(ps))
+    assert cv1 and cvs and np.array_equal(u1, us) and p1[0] == ps
     # device-resident vectors give the same result
     ad, bd = tuple(ctx.to_device(v) for v in a), tuple(ctx.to_device(v) for v in b)
     ud, pd_, cvd, _ = bk.MatrixFreeBLSB200(lm).solve_block(J, ad, bd, c, ctx.to_device(rhst), rhsb)
