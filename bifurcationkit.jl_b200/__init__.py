@@ -4,7 +4,8 @@ continuation.  The directory name carries a dot (bifurcationkit.jl_b200), so imp
 
 Contents: csrc/ (CUDA kernels + C ABI -> libbk200.so), lib.py (ctypes binding), core.py (mirror of
 the reference's AbstractLinearSolver / AbstractBorderedLinearSolver / AbstractEigenSolver surfaces),
-palc.py (host-side Newton / newton_palc / continuation loop driving the device kernels).
+palc.py (host-side Newton / newton_palc / continuation loop driving the device kernels), periodic.py (periodic-orbit
+branches with the Trapeze functional and branch switching to them from a Hopf point).
 """
 from . import lib
 from .lib import (BK200Error, BK_CHAN, BK_SH2D, BK_SH3D, BK_CGL2D, BK_POTRAP_CGL2D, BK_SH2D_PERIODIC, BK_COMPLEX, BK_PC_NONE,
@@ -18,3 +19,4 @@ from . import events
 from . import deflation
 from . import codim2
 from . import normalform
+from . import periodic

@@ -175,6 +175,11 @@ class Context:
     def potrap_set_section(self, phi, xpi=None):
         _chk(self, self.lib.bk_potrap_set_section(self.handle, _l.ptr(phi), _l.ptr(xpi)))
 
+    def potrap_update_section(self, x, scale):
+        """phi_i = scale F(x_i), xpi = x without the period, at the current params (bk_potrap_update_section):
+        scale = 1/M is updatesection!, scale = 1 the orbit form of re_make"""
+        _chk(self, self.lib.bk_potrap_update_section(self.handle, _l.ptr(x), float(scale)))
+
 
 class DeviceVec:
     """Device-resident fp64 vector with the VectorInterface subset used by the continuation host loop."""

@@ -198,6 +198,24 @@ static __global__ void __launch_bounds__(256) k_potrap_fcache(OpDesc op, const d
     f[(long long)sl * Ns + g + n] = a2;
   }
 }
+// The section of the phase condition from an orbit x, in one pass over x: phi_i = scale F(x_i) for every slice, xpi = x
+// without the period (updatesection!, PeriodicOrbitTrapeze.jl:665-679: scale = 1/M; re_make :1077-1080: scale = 1)
+static __global__ void __launch_bounds__(256) k_potrap_section(OpDesc op, const double* __restrict__ x, double scale,
+                                                               double* __restrict__ phi, double* __restrict__ xpi) {
+  bk_pdl_sync();
+  const int nx = op.nx, ny = op.ny, M = op.nz;
+  const long long n = (long long)nx * ny, Ns = 2 * n, total = n * M;
+  const CglPar p = cgl_par(op);
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
+    const long long g = q % n, o = (q / n) * Ns + g;
+    double a1, a2;
+    cgl_point<1>(p, nullptr, x + (o - g), 1.0, (int)(g % nx), (int)(g / nx), nx, ny, op.cx, op.cy, a1, a2);
+    phi[o] = scale * a1;
+    phi[o + n] = scale * a2;
+    xpi[o] = x[o];
+    xpi[o + n] = x[o + n];
+  }
+}
 
 // ------------------------------------------------------------------------------------------ jets d2F / d3F
 // Second and third differentials of F in u (src/Problems.jl:107-110,165-183).  The linear parts of F (Laplacians, L1, the
@@ -532,5 +550,18 @@ extern "C" int32_t bk_potrap_set_section(bk_ctx* c, const double* phi, const dou
   } else {
     BK_CUDA(c, cudaMemsetAsync(c->xpi, 0, 8 * (size_t)n, c->stream));
   }
+  return bk_dev_dot(c, c->xpi, c->phi, n, &c->phi_dot_xpi);
+}
+
+extern "C" int32_t bk_potrap_update_section(bk_ctx* c, const double* x, double scale) {
+  BK_ENTER(c);
+  BkRange nvtx_range("bk_potrap_update_section");
+  BK_CHECK(c, c->kind == BK_POTRAP_CGL2D, "not a potrap context");
+  BK_CHECK(c, x != nullptr, "null orbit");
+  const long long n = c->N - 1;
+  double* dx;
+  BK_TRY(bk_stage_in(c, x, n, 0, true, &dx));
+  const OpDesc op = bk_make_residual_op(c);  // F at the context's current params, as the residual
+  BK_TRY(bk_launch(c, k_potrap_section, bk_lin_grid(c, (long long)op.nx * op.ny * op.nz), 256, 0, op, dx, scale, c->phi, c->xpi));
   return bk_dev_dot(c, c->xpi, c->phi, n, &c->phi_dot_xpi);
 }

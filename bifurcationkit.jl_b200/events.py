@@ -219,6 +219,8 @@ def continuation(prob, alg, contpar, normC=V.norm2, verbose=False, callback=None
                             step=st.step, n_unstable=st.n_unstable[0], n_imag=st.n_imag[0], stable=stable))
         if st.eigvals is not None:
             br.eig.append(dict(eigenvals=np.array(st.eigvals), step=st.step))
+            if cp.save_eigenvectors and st.eigvecs is not None:
+                br.eig[-1]["eigenvecs"] = np.array(st.eigvecs)
         if callback is not None and callback(st) is False:
             st.stop = True
 

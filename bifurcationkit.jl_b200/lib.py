@@ -26,7 +26,7 @@ SYMBOLS = [
     "bk_residual", "bk_jac_set_state", "bk_jvp", "bk_jac_set_shift_imag", "bk_jac_set_transpose", "bk_d2f", "bk_d3f", "bk_precond_setup", "bk_precond_apply",
     "bk_gmres", "bk_gmres2", "bk_bls_bordering", "bk_bls_matrixfree", "bk_bls_map",
     "bk_bls_block_bordering", "bk_bls_block_matrixfree", "bk_bls_block_map",
-    "bk_eigs_shift_invert", "bk_potrap_set_section", "bk_hessenberg_eig", "bk_palc_run",
+    "bk_eigs_shift_invert", "bk_potrap_set_section", "bk_potrap_update_section", "bk_hessenberg_eig", "bk_palc_run",
 ]
 
 
@@ -135,6 +135,7 @@ def load():
         "bk_eigs_shift_invert": [C.c_void_p, dbl, i32, i32, dbl, i32, C.POINTER(GmresOpts), vp, dp, dp, vp,
                                  C.POINTER(i32), C.POINTER(i32)],
         "bk_potrap_set_section": [C.c_void_p, vp, vp],
+        "bk_potrap_update_section": [C.c_void_p, vp, dbl],
         "bk_hessenberg_eig": [dp, i32, i32, dp, dp, dp, dp],
         "bk_palc_run": [C.c_void_p, C.POINTER(PalcOpts), C.POINTER(GmresOpts), vp, dbl, vp, dbl, dp, i32, PalcCallback, C.c_void_p,
                         vp, C.POINTER(PalcResult)],

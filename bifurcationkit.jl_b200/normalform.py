@@ -8,11 +8,19 @@ Mirror of the reference:
   (adjoint eigenvector)  <->  get_adjoint_basis(L★, λ::Number, eigsolver)    src/NormalForms.jl:31-49
   predictor              <->  predictor(::Transcritical / ::Pitchfork / ::Fold, ds)  src/NormalForms.jl:389-493
   continuation_from_bp   <->  continuation(br, ind_bif, options_cont)       src/bifdiagram/BranchSwitching.jl:74-198, :8-44
+  hopf_normal_form       <->  hopf_normal_form(prob, br, ind_hopf; autodiff = false)  src/NormalForms.jl:1102-1204
+  hopf_normal_form_at    <->  __hopf_normal_form(prob, pt::Hopf, ls; autodiff = false) src/NormalForms.jl:1009-1076
+  predictor (Hopf)       <->  predictor(hp::Hopf, ds)                       src/NormalForms.jl:1227-1281
+  d2Fc / d3Fc            <->  d2Fc (src/Problems.jl:171-178): complex forms composed from real bk_d2f / bk_d3f calls
+
+The Hopf normal form keeps its complex vectors (ζ, ζ★, Ψ200) as host arrays: it is a handful of solves at one point.
+Branch switching from a Hopf point to periodic orbits is in periodic.py.
 
 Not here: kernels of dimension > 1 (get_normal_formNd, multicontinuation), the generic BranchPoint predictor (_predictor,
-src/NormalForms.jl:496-535), usedeflation, bothside and bifurcationdiagram; Hopf and higher codimension normal forms.
+src/NormalForms.jl:496-535), usedeflation, bothside and bifurcationdiagram; higher codimension normal forms.
 """
 import copy
+import itertools
 from dataclasses import dataclass, replace
 import math
 import types
@@ -65,22 +73,51 @@ def _E(x, zeta, zeta_ad):
     return V.axpby(x, -V.dot(x, zeta_ad), zeta, 1.0)
 
 
+def _host(x):
+    """a vector as a host array"""
+    return x.numpy() if isinstance(x, DeviceVec) else np.asarray(x)
+
+
+def _capply(J, z):
+    """apply(J, z) for a complex host vector z: J on the real and the imaginary part"""
+    re = _host(_apply(J, np.ascontiguousarray(np.real(z), dtype=np.float64)))
+    im = _host(_apply(J, np.ascontiguousarray(np.imag(z), dtype=np.float64)))
+    return re + 1j * im
+
+
+def _eigvec(J, vals, vecs, k):
+    """geteigenvector(eigsolver, vecs, k) as a host array: a complex column as it is; a real-stored one (ShiftInvertB200 keeps a
+    complex pair as real columns) is completed from one of its columns v, which lies in the pair's invariant subspace: with
+    λ = α + iβ, v = Re(w) for an eigenvector w of λ, and J v = α Re(w) - β Im(w) gives Im(w) = (α v - J v) / β."""
+    v = np.asarray(vecs)[:, k]
+    lam = complex(vals[k])
+    if np.iscomplexobj(v) or lam.imag == 0:
+        return v
+    return v + 1j * (lam.real * v - _host(_apply(J, np.ascontiguousarray(v)))) / lam.imag
+
+
 def _adjoint_vector(prob, x0, p, lam, eigsolver, nev):
     """get_adjoint_basis(L★, conj(λ), eigsolver; nev) (src/NormalForms.jl:31-49): the eigenvector of J' whose eigenvalue is
-    closest to conj(λ).  J' is prob.Jt for host problems and J under bk_jac_set_transpose on the device."""
+    closest to conj(λ).  J' is prob.Jt for host problems and J under bk_jac_set_transpose on the device.  A real λ gives a
+    real vector of the container of x0, a complex λ a complex host array."""
+    def adjoint(J):
+        vals, vecs = _eig(eigsolver, J, nev)
+        i = int(np.argmin(np.abs(vals - np.conj(lam))))
+        if np.imag(lam) == 0:
+            return vals[i], _like(x0, np.asarray(vecs)[:, i])
+        return vals[i], _eigvec(J, vals, vecs, i)
     if hasattr(prob, "Jt"):
-        vals, vecs = _eig(eigsolver, prob.Jt(x0, p), nev)
+        val, vec = adjoint(prob.Jt(x0, p))
     else:
         prob.ctx.set_transpose(True)
         try:
-            vals, vecs = _eig(eigsolver, prob.J(x0, p), nev)
+            val, vec = adjoint(prob.J(x0, p))
         finally:
             prob.ctx.set_transpose(False)
-    i = int(np.argmin(np.abs(vals - np.conj(lam))))
-    if abs(vals[i].real) > 1e-2:
-        warnings.warn(f"The bifurcating eigenvalue is not that close to Re = 0. We found {vals[i].real} !≈ 0. "
+    if abs(val.real) > 1e-2:
+        warnings.warn(f"The bifurcating eigenvalue is not that close to Re = 0. We found {val.real} !≈ 0. "
                       "You can perhaps increase the argument `nev`.")
-    return _like(x0, np.asarray(vecs)[:, i])
+    return vec
 
 
 def _eigvals_at(br, bifpt):
@@ -172,6 +209,176 @@ def get_normal_form1d(it, br, ind_bif, nev=None, zeta=None, zeta_ad=None, bls=No
                          bptype=bptype)
 
 
+@dataclass
+class HopfNF:
+    """Hopf of src/NormalForms.jl (fields of the Hopf point): the point (x0, p), the frequency omega = Im λ, the eigenvector
+    zeta of J for λ and the adjoint vector zeta_ad with <zeta, zeta_ad> = 1 (complex host arrays), and HopfNormalForm in `nf`:
+    a, b of the reduced equation dA/dt = (iω + a dp) A + b A |A|^2, with Psi001, Psi110 (real host arrays) and Psi200 (complex);
+    all None for detailed = False.  type: SuperCritical / SubCritical / Singular by the sign of Re b, ? without a, b."""
+    type: str
+    x0: object
+    p: float
+    omega: float
+    zeta: object
+    zeta_ad: object
+    nf: dict
+
+
+def _jet(f, x0, p, *vs):
+    """the complex-multilinear extension of a real jet f(x0, p, v1, ..) (d2F / d3F) to complex host vectors, from real calls on
+    their real and imaginary parts (d2Fc, src/Problems.jl:171-178); calls on an imaginary part that is zero are skipped"""
+    parts = [(np.ascontiguousarray(np.real(v), dtype=np.float64), np.ascontiguousarray(np.imag(v), dtype=np.float64)) for v in vs]
+    re = im = 0.0
+    for pick in itertools.product((0, 1), repeat=len(vs)):
+        if any(k and not np.any(parts[j][1]) for j, k in enumerate(pick)):
+            continue
+        val = _host(f(x0, p, *[parts[j][k] for j, k in enumerate(pick)]))
+        n_im = sum(pick) % 4                                   # the factor i^n_im
+        if n_im == 0:
+            re = re + val
+        elif n_im == 1:
+            im = im + val
+        elif n_im == 2:
+            re = re - val
+        else:
+            im = im - val
+    return re + 1j * im
+
+
+def d2Fc(prob, x0, p, a, b):
+    """d2F(x0, p)[a, b] for complex host vectors a, b (four real bk_d2f calls at most)"""
+    return _jet(prob.d2F, x0, p, a, b)
+
+
+def d3Fc(prob, x0, p, a, b, c):
+    """d3F(x0, p)[a, b, c] for complex host vectors (eight real bk_d3f calls at most)"""
+    return _jet(prob.d3F, x0, p, a, b, c)
+
+
+def _complex_twin(prob):
+    """ComplexProblemB200 and ComplexGMRESB200 on a BK_COMPLEX context of the device problem's grid (codim2.py)"""
+    from .codim2 import ComplexProblemB200
+    from .core import Context, ComplexGMRESB200
+    ctx = prob.ctx
+    cctx = Context(ctx.kind, ctx.dims, ctx.lengths, krylov_m=ctx.krylov_m, params=ctx.params, complex=True)
+    return ComplexProblemB200(cctx, prob.params, prob.lens)
+
+
+def hopf_normal_form_at(prob, x0, p, omega, zeta, zeta_ad, ls, cprob=None, cls=None):
+    """__hopf_normal_form (src/NormalForms.jl:1009-1076) with autodiff = false: the parameter derivatives are central
+    differences with prob.delta.  Psi001 and Psi110 come from real solves ls(J, rhs) (the Newton linear solver), Psi200 from
+    (2iω - J) Psi200 = R20 solved by cls(cprob.J(x0, p), R20, a0 = 2iω, a1 = -1) on the complexified twin; for a device
+    problem both default to a BK_COMPLEX context of its grid and ComplexGMRESB200 with ls's settings.  zeta, zeta_ad: complex
+    host arrays.  Inner products are Julia's VI.inner(x, y) = Σ conj(x) y.  Returns a HopfNF."""
+    delta = prob.delta
+    zeta, zeta_ad = np.asarray(zeta, dtype=complex), np.asarray(zeta_ad, dtype=complex)
+    czeta = np.conj(zeta)
+    if cprob is None:
+        cprob = _complex_twin(prob)
+    if cls is None:
+        from .core import ComplexGMRESB200
+        cls = ComplexGMRESB200(reltol=ls.reltol, abstol=ls.abstol, restart=ls.restart, maxiter=ls.maxiter, Pl=ls.Pl, Pr=ls.Pr,
+                               orth=ls.orth, fused=ls.fused)
+    R2 = lambda a, b: d2Fc(prob, x0, p, a, b) / 2
+    R3 = lambda a, b, c: d3Fc(prob, x0, p, a, b, c) / 6
+
+    def solve(rhs, what):  # ls(L, rhs) with L re-made before the solve (a device context keeps one Jacobian)
+        psi, cv, its = ls(prob.J(x0, p), _like(x0, rhs))
+        if not cv:
+            warnings.warn(f"[Hopf {what}] Linear solver for J did not converge. it = {its}")
+        return _host(psi)
+
+    R01 = (_host(prob.F(x0, p + delta)) - _host(prob.F(x0, p - delta))) / (2 * delta)       # :1036-1037
+    Psi001 = solve(-R01, "Ψ001")                                                             # :1039
+    av = (_capply(prob.J(x0, p + delta), zeta) - _capply(prob.J(x0, p - delta), zeta)) / (2 * delta)  # :1046-1047
+    av = av + 2 * R2(zeta, Psi001)
+    a = complex(np.vdot(av, zeta_ad))
+    R20 = R2(zeta, zeta)                                                                     # :1053-1055
+    Psi200, cv, its = cls(cprob.J(x0, p), R20, a0=complex(0.0, 2 * omega), a1=-1.0)
+    if not cv:
+        warnings.warn(f"[Hopf Ψ200] Linear solver for J did not converge. it = {its}")
+    Psi200 = np.asarray(Psi200, dtype=complex)
+    R20 = 2 * R2(zeta, czeta)                                                                # :1058-1060
+    Psi110 = solve(-np.real(R20), "Ψ110")    # R2(ζ, conj ζ) is real: its imaginary part is rounding
+    bv = 2 * R2(zeta, Psi110) + 2 * R2(czeta, Psi200) + 3 * R3(zeta, zeta, czeta)          # :1063-1064
+    b = complex(np.vdot(bv, zeta_ad))
+    tp = "SuperCritical" if b.real < 0 else ("SubCritical" if b.real > 0 else "Singular")    # :1068-1074
+    return HopfNF(type=tp, x0=x0, p=p, omega=omega, zeta=zeta, zeta_ad=zeta_ad,
+                  nf=dict(a=a, b=b, Psi001=Psi001, Psi110=Psi110, Psi200=Psi200))
+
+
+def hopf_normal_form(it, br, ind_hopf, nev=None, zeta=None, zeta_ad=None, detailed=True, cprob=None, cls=None):
+    """hopf_normal_form(prob, br, ind_hopf; autodiff = false, detailed) (src/NormalForms.jl:1102-1204) for the branch `br`
+    computed by events.continuation over the iterator `it`.  λ is the saved eigenvalue ind_ev of the point and ω = Im λ.  zeta:
+    the eigenvector of J for λ -- given, or the one saved with the branch (ContinuationPar.save_eigenvectors), or recomputed
+    with newton_options.eigsolver; scaled by 1 / norm.  zeta_ad: the eigenvector of J' for the eigenvalue closest to conj(λ)
+    (given, or computed as get_normal_form1d does), normalised by ζ★ ./= dot(ζ, ζ★).  cprob / cls: see hopf_normal_form_at.
+    Returns a HopfNF; with detailed = False only the point, ω and ζ."""
+    prob, options = it.prob, it.contpar.newton_options
+    bifpt = br.specialpoint[ind_hopf]
+    if bifpt.type != "hopf":
+        raise ValueError("The provided index does not refer to a Hopf Point")
+    x0, p = bifpt.x, bifpt.param
+    entry = next(e for e in br.eig if e["step"] == bifpt.idx)
+    saved = np.asarray(entry["eigenvals"])
+    nev = len(saved) if nev is None else nev
+    k = bifpt.ind_ev - 1                                                                     # ind_ev is 1-based
+    # :1138-1139.  λ is the member of the crossing pair with Im λ > 0 -- the one the reference's DefaultEig puts at ind_ev (it
+    # lists a pair of equal real parts with the positive imaginary part second); the guess x0 + 2 Re(ζ A(t)) of the predictor
+    # runs forward in time only for ω > 0.  Eigensolvers that list the other member first (ShiftInvertB200) give the same λ.
+    lam = complex(saved[k])
+    lam = lam if lam.imag >= 0 else lam.conjugate()
+    omega = lam.imag
+    closest = lambda vals: int(np.argmin(np.abs(np.asarray(vals) - lam)))
+    if zeta is not None:
+        zeta = np.array(zeta, dtype=complex)
+    elif entry.get("eigenvecs") is not None:                                                 # :1150-1151
+        zeta = _eigvec(prob.J(x0, p), saved, entry["eigenvecs"], closest(saved))
+    else:                                                                                    # :1142-1148
+        vals, vecs = _eig(options.eigsolver, prob.J(x0, p), bifpt.ind_ev + 2)
+        if not _isapprox(vals[k], complex(saved[k])):
+            raise RuntimeError(f"We did not find the correct eigenvalue {saved[k]}. We found {vals}.\n"
+                               "If you use aBS, pass a higher `nev` (number of eigenvalues) to be computed.")
+        zeta = _eigvec(prob.J(x0, p), vals, vecs, closest(vals))
+    zeta = np.asarray(zeta, dtype=complex) / np.linalg.norm(zeta)                            # :1153
+    if not detailed:                                                                         # :1155-1168
+        nf = dict(a=None, b=None, Psi001=None, Psi110=None, Psi200=None)
+        return HopfNF(type="?", x0=x0, p=p, omega=omega, zeta=zeta, zeta_ad=np.zeros_like(zeta), nf=nf)
+    if zeta_ad is None:                                                                      # :1171-1173
+        zeta_ad = _adjoint_vector(prob, x0, p, lam, options.eigsolver, nev)
+    zeta_ad = np.array(zeta_ad, dtype=complex)
+    zeta_ad /= np.vdot(zeta, zeta_ad)                                                        # :1186: ζ★ ./= dot(ζ, ζ★)
+    if not _isapprox(np.vdot(zeta, zeta_ad), 1):
+        raise RuntimeError("Error of precision in normalization")
+    return hopf_normal_form_at(prob, x0, p, omega, zeta, zeta_ad, options.linsolver, cprob, cls)
+
+
+def _hopf_predictor(hp, ds, ampfactor):
+    """predictor(hp::Hopf, ds; ampfactor) (src/NormalForms.jl:1227-1281)"""
+    nf = hp.nf
+    x0 = _host(hp.x0)
+    if nf["a"] is not None and nf["b"] is not None:
+        a, b = nf["a"], nf["b"]
+        if abs(b.real) < 1e-10:
+            warnings.warn(f"The Lyapunov coefficient is nearly zero:\nb = {b}.\nThe Hopf predictor may be unreliable.")
+        dsfactor = 1.0 if a.real * b.real < 0 else -1.0
+        dsnew = abs(ds) * dsfactor
+        pnew = hp.p + dsnew
+        amp = ampfactor * math.sqrt(-dsnew * a.real / b.real)                               # a ds + b amp^2 = 0
+        omega = hp.omega + (a.imag - b.imag * a.real / b.real) * ds
+        Psi001, Psi110, Psi200 = nf["Psi001"], nf["Psi110"], nf["Psi200"]
+    else:
+        amp, omega, pnew, dsfactor = ampfactor, hp.omega, hp.p + ds, 1.0
+        Psi001, Psi110, Psi200 = np.zeros_like(x0), np.zeros_like(hp.zeta), np.zeros_like(hp.zeta)
+
+    def orbit(t):
+        A = amp * complex(math.cos(t), math.sin(t))                                          # amp cis(t)
+        return (x0 + 2 * np.real(hp.zeta * A) + ds * Psi001 + abs(A) ** 2 * np.real(Psi110)
+                + 2 * np.real(A ** 2 * Psi200))
+    return types.SimpleNamespace(orbit=orbit, Psi001=Psi001, amp=2 * amp, omega=omega, period=abs(2 * math.pi / omega), p=pnew,
+                                 dsfactor=dsfactor)
+
+
 def _comb(x, *terms):
     """x + sum(c v for (c, v) in terms), a new vector"""
     y = V.copy(x)
@@ -181,8 +388,11 @@ def _comb(x, *terms):
 
 
 def predictor(bp, ds, ampfactor=1.0):
-    """predictor(bp, ds; ampfactor) (src/NormalForms.jl:389-493): a point (x1, p) on the bifurcated branch near bp, as a
-    namespace with the reference's fields; None for a Fold."""
+    """predictor(bp, ds; ampfactor) (src/NormalForms.jl:389-493, :1227-1281): a point (x1, p) on the bifurcated branch near bp,
+    or for a Hopf point the guess of the bifurcated periodic orbits, as a namespace with the reference's fields; None for a
+    Fold."""
+    if isinstance(bp, HopfNF):
+        return _hopf_predictor(bp, ds, ampfactor)
     nf = bp.nf
     if bp.type == "Transcritical":                                                       # :389-435
         b11, b20, Psi01 = nf["b11"], nf["b20"], nf["Psi01"]

@@ -134,6 +134,9 @@ class ContinuationPar:
     nev: int = 3
     detect_bifurcation: int = 0
     tol_stability: float = 1e-10
+    # keep the eigenvectors of every step in the branch (events.continuation), as the Hopf normal form can use them; off by
+    # default, unlike the reference, because a device branch would keep nev state-sized host arrays per step
+    save_eigenvectors: bool = False
     # events.py (SURVEY 8f.2): fold detection by parameter monotony and bisection on the number of unstable eigenvalues
     detect_fold: bool = True
     n_inversion: int = 2

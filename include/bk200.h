@@ -206,6 +206,11 @@ int32_t bk_hessenberg_eig(const double* H, int32_t n, int32_t ldh, double* wr, d
 /* ---- P5: trapezoid periodic-orbit functional over the context's vector field
  *   (BK_POTRAP_CGL2D contexts; x = [x_1..x_M; T], src/periodicorbit/PeriodicOrbitTrapeze.jl:249-330) */
 int32_t bk_potrap_set_section(bk_ctx* ctx, const double* phi, const double* xpi); /* length N-1 each */
+/* the section from an orbit x (host or device, length N, the period is not read), at the context's current params:
+ * phi_i = scale * F(x_i) for every slice i, xpi = x[0 .. N-2], then phi_dot_xpi as bk_potrap_set_section computes it.
+ * scale = 1/M is updatesection! (PeriodicOrbitTrapeze.jl:665-679), scale = 1 the orbit form of re_make (:1056-1084).
+ * BK_ERR_ARG before any launch on a context of another kind or a null x. */
+int32_t bk_potrap_update_section(bk_ctx* ctx, const double* x, double scale);
 
 /* ---- the all-native PALC loop (SURVEY.md 8(b), optional entry): continuation(prob, PALC(...), opts; normC) of
  *   src/Continuation.jl:349-504, 506-601 for the context's problem -- two start-up Newton solves (src/Newton.jl:66-114), secant or

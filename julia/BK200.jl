@@ -156,6 +156,14 @@ function d3F(c::Context, u, params, dx1, dx2, dx3)
     out
 end
 
+"""updatesection!(trap, x, pars) (PeriodicOrbitTrapeze.jl:665-679) on a BK_POTRAP_CGL2D context: ϕ_i = scale F(x_i), xπ = x[1:end-1]
+(bk_potrap_update_section).  scale = 1/M for updatesection!, 1 for the orbit form of re_make (:1077-1080).  Not executed here."""
+function update_section!(c::Context, x, params, scale)
+    setparams!(c, params)
+    check(c, ccall((:bk_potrap_update_section, lib), Int32, (Ptr{Cvoid}, Ptr{Float64}, Float64), c.handle, ptr(x), scale))
+    true
+end
+
 # ---- AbstractIterativeLinearSolver (src/LinearSolver.jl:8-12,149-206) --------------------------------------------------
 Base.@kwdef mutable struct GMRESB200 <: BK.AbstractIterativeLinearSolver
     ctx::Context
