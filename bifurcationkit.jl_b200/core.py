@@ -20,6 +20,7 @@ Vectors may be NumPy arrays (host buffers: every call copies H2D/D2H inside the 
 or ``DeviceVec`` (device-resident, zero copies -- "option B").  Results have the container type of
 the right-hand side, as the reference requires (Newton does ``minus!!(x, u)``, src/Newton.jl:97).
 """
+import contextlib
 import ctypes as C
 
 import numpy as np
@@ -53,6 +54,11 @@ class Context:
         self.N = int(self.lib.bk_problem_size(h))
         self.N0 = int(self.lib.bk_state_size(h))
         self.complex = bool(complex)
+        # whether the kind has a J' kernel (has_jt of the library's kind table): bk_jac_set_transpose accepts it or refuses it.
+        # Asked once here, while the context's transpose is still off, so that no caller's setting is touched later.
+        self.has_adjoint = self.lib.bk_jac_set_transpose(h, 1) >= 0
+        if self.has_adjoint:
+            _chk(self, self.lib.bk_jac_set_transpose(h, 0))
         self.params = None
         if params is not None:
             self.set_params(params)
@@ -134,6 +140,14 @@ class Context:
         """J = jacobian(prob, u, params): snapshot of (u, current params) inside the context."""
         _chk(self, self.lib.bk_jac_set_state(self.handle, _l.ptr(u)))
         return Jacobian(self)
+
+    def jacobian_adjoint(self, u):
+        """J' = jacobian_adjoint(prob, u, params): the same snapshot as `jacobian`, as a handle that applies the transpose.
+        Raises for a kind without a J' kernel (has_adjoint)."""
+        if not self.has_adjoint:
+            raise _l.BK200Error("jacobian_adjoint: J' is not available for this problem kind")
+        _chk(self, self.lib.bk_jac_set_state(self.handle, _l.ptr(u)))
+        return TransposedJacobian(self)
 
     def cjacobian(self, u, transpose=False):
         """BK_COMPLEX contexts: J (or J') at the real state u, acting on complex vectors."""
@@ -259,6 +273,30 @@ class Jacobian:
         return self.ctx.jvp(dx)
 
 
+class TransposedJacobian(Jacobian):
+    """J' at the context's linearisation state (jacobian_adjoint, src/Problems.jl).  The solvers below select J' for the
+    duration of a call with this handle (`transpose`) and switch it off again; so does an application J'(dx)."""
+    transpose = True
+
+    def __call__(self, dx):
+        with _operator(self):
+            return self.ctx.jvp(dx)
+
+
+@contextlib.contextmanager
+def _operator(J):
+    """J or J' for the duration of one call, as the handle says (its `transpose`).  A handle without that attribute leaves the
+    context's setting as it is."""
+    if not hasattr(J, "transpose"):
+        yield
+        return
+    J.ctx.set_transpose(J.transpose)
+    try:
+        yield
+    finally:
+        J.ctx.set_transpose(False)
+
+
 def csplit(z):
     """complex array -> the split layout [re; im] of a BK_COMPLEX context"""
     z = np.asarray(z)
@@ -303,6 +341,10 @@ class GMRESB200:
                          _l.BK_ORTH_CGS2 if self.orth == "cgs2" else _l.BK_ORTH_CGS, self.fused)
 
     def __call__(self, J, rhs, rhs2=None, a0=0.0, a1=1.0):
+        with _operator(J):
+            return self._solve(J, rhs, rhs2, a0, a1)
+
+    def _solve(self, J, rhs, rhs2=None, a0=0.0, a1=1.0):
         ctx = J.ctx
         if rhs2 is not None:
             # src/LinearSolver.jl:15-19: ls(J, rhs1, rhs2) -> (x1, x2, flag1 & flag2, (it1, it2)): one ABI crossing (bk_gmres2)
@@ -331,7 +373,7 @@ class ComplexGMRESB200(GMRESB200):
         ctx.set_transpose(getattr(J, "transpose", False))
         ctx.set_shift_imag(a0.imag)
         try:
-            x, cv, it = GMRESB200.__call__(self, J, csplit(rhs), a0=a0.real, a1=a1)
+            x, cv, it = self._solve(J, csplit(rhs), a0=a0.real, a1=a1)
         finally:
             ctx.set_shift_imag(0.0)
         return cjoin(x), cv, it
@@ -358,6 +400,10 @@ class BorderingBLSB200:
         self.solver, self.tol, self.check_precision, self.k = solver, tol, check_precision, k
 
     def __call__(self, J, dR, dzu, dzp, R, n, xiu=1.0, xip=1.0, shift=None, dotscale=1.0):
+        with _operator(J):
+            return self._solve(J, dR, dzu, dzp, R, n, xiu, xip, shift, dotscale)
+
+    def _solve(self, J, dR, dzu, dzp, R, n, xiu, xip, shift, dotscale):
         ctx = J.ctx
         dX = ctx._like(R)
         o = self.solver.opts()
@@ -393,6 +439,10 @@ class MatrixFreeBLSB200:
         self.solver = solver
 
     def __call__(self, J, dR, dzu, dzp, R, n, xiu=1.0, xip=1.0, shift=None, dotscale=1.0):
+        with _operator(J):
+            return self._solve(J, dR, dzu, dzp, R, n, xiu, xip, shift, dotscale)
+
+    def _solve(self, J, dR, dzu, dzp, R, n, xiu, xip, shift, dotscale):
         ctx = J.ctx
         dX = ctx._like(R)
         o = self.solver.opts()
@@ -444,6 +494,10 @@ class ShiftInvertB200:
         self.sigma, self.ls, self.krylovdim, self.tol, self.maxrestart = sigma, ls, krylovdim, tol, maxrestart
 
     def __call__(self, J, nev, v0=None, want_vectors=False):
+        with _operator(J):   # the eigenpairs of J' for a TransposedJacobian handle
+            return self._solve(J, nev, v0, want_vectors)
+
+    def _solve(self, J, nev, v0, want_vectors):
         ctx = J.ctx
         kd = self.krylovdim or max(30, nev + 30)
         kd = min(kd, ctx.N)

@@ -78,7 +78,7 @@ const BkKindTraits* bk_kind_traits(int kind) {
                                        {2, 1, 0, true, true, true, false, true},       // BK_SH2D
                                        {3, 1, 0, true, true, true, false, true},       // BK_SH3D
                                        {2, 2, 0, false, true, true, false, true},      // BK_CGL2D
-                                       {3, 2, 1, false, false, false, false, false},   // BK_POTRAP_CGL2D
+                                       {3, 2, 1, false, true, false, false, false},    // BK_POTRAP_CGL2D
                                        {2, 1, 0, true, true, true, true, true}};       // BK_SH2D_PERIODIC
   static_assert(BK_CHAN == 1 && BK_POTRAP_CGL2D == 5 && BK_SH2D_PERIODIC == 6, "the table is indexed by kind");
   if (kind < BK_CHAN || kind > BK_SH2D_PERIODIC) return nullptr;

@@ -16,7 +16,8 @@
 //   examples/cGL2d.jl:209-213); for potrap contexts it is applied slice by slice (block Jacobi, cf.
 //   jacobian_block_diag, src/periodicorbit/PeriodicOrbitTrapeze.jl:619-643).
 // BK_PC_POTRAP_CIRC: block-circulant-in-time linearisation of the Trapeze functional at the trivial state, inverted
-//   exactly: DST-I in space, u1 +- i u2, DFT over the M-1 cyclic slices, scalar symbol.
+//   exactly: DST-I in space, u1 +- i u2, DFT over the M-1 cyclic slices, scalar symbol.  While J' is selected
+//   (bk_jac_set_transpose) it applies the exact transpose P'^-1, so that the J' solves are preconditioned with P'.
 #include <cmath>
 #include <cstdlib>
 #include <utility>
@@ -86,6 +87,67 @@ static __global__ void __launch_bounds__(128) k_potrap_time(double* __restrict__
     const double cr = lam + r;
     double2 sp = make_double2(omg.x - 0.5 * h * (opg.x * cr - opg.y * nu), omg.y - 0.5 * h * (opg.x * nu + opg.y * cr));
     double2 sm = make_double2(omg.x - 0.5 * h * (opg.x * cr + opg.y * nu), omg.y - 0.5 * h * (-opg.x * nu + opg.y * cr));
+    const double dp = 1.0 / (sp.x * sp.x + sp.y * sp.y), dm = 1.0 / (sm.x * sm.x + sm.y * sm.y);
+    yp[k] = make_double2((ap.x * sp.x + ap.y * sp.y) * dp * invK, (ap.y * sp.x - ap.x * sp.y) * dp * invK);
+    ym[k] = make_double2((am.x * sm.x + am.y * sm.y) * dm * invK, (am.y * sm.x - am.x * sm.y) * dm * invK);
+  }
+  for (int i = 0; i < K; ++i) {
+    double2 ap = make_double2(0, 0), am = make_double2(0, 0);
+    int idx = 0;
+    for (int k = 0; k < K; ++k) {
+      const double2 t = tw[idx];  // conj -> exp(+2 pi i k i / K)
+      ap.x += yp[k].x * t.x + yp[k].y * t.y;
+      ap.y += yp[k].y * t.x - yp[k].x * t.y;
+      am.x += ym[k].x * t.x + ym[k].y * t.y;
+      am.y += ym[k].y * t.x - ym[k].x * t.y;
+      idx += i;
+      if (idx >= K) idx -= K;
+    }
+    B[(long long)(2 * i) * n + g] = 0.5 * (ap.x + am.x);      // Re((yp + ym)/2)
+    B[(long long)(2 * i + 1) * n + g] = 0.5 * (ap.y - am.y);  // Re((yp - ym)/(2i)) = Im(yp - ym)/2
+  }
+}
+// k_potrap_time_tr: the same solve with the transposed block circulant (P'^-1 while J' is selected).  Its time blocks are
+// x_k - x_{k+1} (the shift the other way: g_k -> conj g_k) and its reaction block is [[a, nu], [-nu, a]] (nu -> -nu on w+-), so
+// its symbol is conj(s+-_k).  The closure slice M-1 is added to slice 0 first: the transpose of x_M = r_M + x_1.
+static __global__ void __launch_bounds__(128) k_potrap_time_tr(double* __restrict__ B, long long n, int nx, int K,
+                                                               const double* __restrict__ lamx, const double* __restrict__ lamy,
+                                                               double h, double r, double nu, const double2* __restrict__ tw) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n) return;
+  const double lam = lamx[g % nx] + lamy[g / nx];
+  double2 wp[BK_PO_KMAX], wm[BK_PO_KMAX];
+  for (int i = 0; i < K; ++i) {
+    double a = B[(long long)(2 * i) * n + g], b = B[(long long)(2 * i + 1) * n + g];
+    if (i == 0) {  // + the closure slice M-1 (field pair 2K, 2K+1, transformed with the rest)
+      a += B[(long long)(2 * K) * n + g];
+      b += B[(long long)(2 * K + 1) * n + g];
+    }
+    wp[i] = make_double2(a, b);
+    wm[i] = make_double2(a, -b);
+  }
+  double2 yp[BK_PO_KMAX], ym[BK_PO_KMAX];
+  const double invK = 1.0 / K;
+  for (int k = 0; k < K; ++k) {
+    double2 ap = make_double2(0, 0), am = make_double2(0, 0);
+    int idx = 0;
+    for (int i = 0; i < K; ++i) {
+      const double2 t = tw[idx];  // exp(-2 pi i k i / K)
+      ap.x += wp[i].x * t.x - wp[i].y * t.y;
+      ap.y += wp[i].x * t.y + wp[i].y * t.x;
+      am.x += wm[i].x * t.x - wm[i].y * t.y;
+      am.y += wm[i].x * t.y + wm[i].y * t.x;
+      idx += k;
+      if (idx >= K) idx -= K;
+    }
+    const double2 gk = tw[k];
+    // s = (1 - g) - h/2 (1 + g) (lam + r +- i nu), then conjugated
+    const double2 omg = make_double2(1.0 - gk.x, -gk.y), opg = make_double2(1.0 + gk.x, gk.y);
+    const double cr = lam + r;
+    double2 sp = make_double2(omg.x - 0.5 * h * (opg.x * cr - opg.y * nu), omg.y - 0.5 * h * (opg.x * nu + opg.y * cr));
+    double2 sm = make_double2(omg.x - 0.5 * h * (opg.x * cr + opg.y * nu), omg.y - 0.5 * h * (-opg.x * nu + opg.y * cr));
+    sp.y = -sp.y;  // the transposed symbols conj(s+-_k)
+    sm.y = -sm.y;
     const double dp = 1.0 / (sp.x * sp.x + sp.y * sp.y), dm = 1.0 / (sm.x * sm.x + sm.y * sm.y);
     yp[k] = make_double2((ap.x * sp.x + ap.y * sp.y) * dp * invK, (ap.y * sp.x - ap.x * sp.y) * dp * invK);
     ym[k] = make_double2((am.x * sm.x + am.y * sm.y) * dm * invK, (am.y * sm.x - am.x * sm.y) * dm * invK);
@@ -540,14 +602,18 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
     double* A = pc.work;
     double* Bf = pc.work2;
     // DST-I in space over all 2M slice components (mixed-radix FFT of the odd extension, bk_fft_gen.cuh), the circulant
-    // solve in time per spatial mode, DST-I back
+    // solve in time per spatial mode, DST-I back.  While J' is selected (bk_jac_set_transpose) this is P'^-1: the transposed
+    // time solve, then x_M = r_M and the period entry pass through (one copy: they are the last Ns + 1 entries).
     BK_TRY(transform_pass(c, 0, 0, in, A, nx, ny, nf, al));
     BK_TRY(transform_pass(c, 1, 0, A, Bf, nx, ny, nf, true));
-    BK_TRY(bk_launch_ordered(c, k_potrap_time, (unsigned)((nn + 127) / 128), 128, 0, Bf, nn, nx, M - 1, pc.lam[0], pc.lam[1],
-                             pc.po_T / M, pc.po_r, pc.po_nu, pc.tdft));
+    BK_TRY(bk_launch_ordered(c, c->transpose ? k_potrap_time_tr : k_potrap_time, (unsigned)((nn + 127) / 128), 128, 0, Bf, nn, nx,
+                             M - 1, pc.lam[0], pc.lam[1], pc.po_T / M, pc.po_r, pc.po_nu, pc.tdft));
     BK_TRY(transform_pass(c, 1, 1, Bf, A, nx, ny, nf, true));
     BK_TRY(transform_pass(c, 0, 1, A, out, nx, ny, nf, al));
-    BK_TRY(bk_launch_ordered(c, k_potrap_close, (unsigned)((Ns + 255) / 256), 256, 0, in, out, Ns, M));
+    if (c->transpose)
+      BK_CUDA(c, cudaMemcpyAsync(out + (M - 1) * Ns, in + (M - 1) * Ns, 8 * (size_t)(Ns + 1), cudaMemcpyDeviceToDevice, c->stream));
+    else
+      BK_TRY(bk_launch_ordered(c, k_potrap_close, (unsigned)((Ns + 255) / 256), 256, 0, in, out, Ns, M));
   } else if (pc.kind == BK_PC_CHAN_TRIDIAG) {
     BK_TRY(bk_launch_ordered(c, k_thomas, 1, 32, 0, pc.tri, in, out, (int)N));
   }

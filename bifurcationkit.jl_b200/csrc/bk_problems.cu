@@ -83,6 +83,15 @@ __device__ __forceinline__ double lap_dirichlet(const double* __restrict__ a, in
   double ym = j > 0 ? a[g - nx] : 0.0, yp = j < ny - 1 ? a[g + nx] : 0.0;
   return s * (cx * (xm - 2.0 * c + xp) + cy * (ym - 2.0 * c + yp));
 }
+// the same stencil on the sum a + b of two fields (one stencil evaluation for the two slices of a J' row)
+__device__ __forceinline__ double lap_dirichlet_sum(const double* __restrict__ a, const double* __restrict__ b, int i, int j,
+                                                    int nx, int ny, double cx, double cy, double s) {
+  const long long g = i + (long long)j * nx;
+  const double c = a[g] + b[g];
+  const double xm = i > 0 ? a[g - 1] + b[g - 1] : 0.0, xp = i < nx - 1 ? a[g + 1] + b[g + 1] : 0.0;
+  const double ym = j > 0 ? a[g - nx] + b[g - nx] : 0.0, yp = j < ny - 1 ? a[g + nx] + b[g + nx] : 0.0;
+  return s * (cx * (xm - 2.0 * c + xp) + cy * (ym - 2.0 * c + yp));
+}
 // Vector field / JVP at one grid point of one slice: base pointers to the slice's [u1;u2].
 template <int MODE, bool TR = false>
 __device__ __forceinline__ void cgl_point(const CglPar& p, const double* __restrict__ u, const double* __restrict__ v,
@@ -337,6 +346,61 @@ static __global__ void __launch_bounds__(256) k_potrap_phase(OpDesc op, const do
   out[n] = jvp_mode ? op.a0 * s * in[n] + op.a1 * ph : ph;
 }
 
+// J' of the Trapeze functional: the transpose of k_potrap_apply<0> with its phase row, in one pass.  With h/2 = T / (2M),
+// A_k = J_F(x_k), f_k = F(x_k) (fcache) and next(k) = k + 1, next(M - 2) = 0 (the inverse of the row map sl -> sp):
+//   (J'w)_k     = (w_k - w_next(k)) - h/2 A_k' (w_k + w_next(k)) + phi_k w_T   (k <= M - 2; slice 0 also - w_{M-1})
+//   (J'w)_{M-1} = w_{M-1} + phi_{M-1} w_T
+//   (J'w)_T     = -1/(2M) sum_{k <= M-2} <f_k, w_k + w_next(k)>
+// A_k' is the Dirichlet Laplacian (symmetric) plus the transposed 2 x 2 reaction block, so each point needs one stencil
+// evaluation, on w_k + w_next(k).  out = a0 s w + a1 s J'w (s = *in_scale_ptr); the period entry is the fixed-order grid
+// reduction of k_tail, written by the last CTA.
+static __global__ void __launch_bounds__(256, 3) k_potrap_apply_tr(OpDesc op, const double* __restrict__ in,
+                                                                const double* __restrict__ in_scale_ptr, double* __restrict__ out,
+                                                                double* __restrict__ partials, unsigned int* counter) {
+  const int nx = op.nx, ny = op.ny, M = op.nz;
+  const long long n = (long long)nx * ny, Ns = 2 * n, total = n * M;
+  const double s = in_scale_ptr ? __ldg(in_scale_ptr) : 1.0;
+  const CglPar p = cgl_par(op);
+  const double h2 = 0.5 * op.u[Ns * M] / M;
+  const double wT = s * in[Ns * M];
+  const double* wl = in + (long long)(M - 1) * Ns;
+  double acc[1] = {0.0};
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
+    const long long g = q % n;
+    const int sl = (int)(q / n);
+    const long long o = (long long)sl * Ns + g;
+    double r1 = op.phi[o] * wT, r2 = op.phi[o + n] * wT;
+    if (sl == M - 1) {
+      r1 += s * in[o];
+      r2 += s * in[o + n];
+    } else {
+      const int nk = sl < M - 2 ? sl + 1 : 0;
+      const double* wk = in + (long long)sl * Ns;
+      const double* wn = in + (long long)nk * Ns;
+      const double* uk = op.u + (long long)sl * Ns;
+      const double* fk = op.fcache + (long long)sl * Ns;
+      const int i = (int)(g % nx), j = (int)(g / nx);
+      const double d1 = wk[g] + wn[g], d2 = wk[g + n] + wn[g + n];
+      double a1, a2;
+      cgl_dnl<true>(p, uk[g], uk[g + n], s * d1, s * d2, a1, a2);
+      a1 += lap_dirichlet_sum(wk, wn, i, j, nx, ny, op.cx, op.cy, s);
+      a2 += lap_dirichlet_sum(wk + n, wn + n, i, j, nx, ny, op.cx, op.cy, s);
+      r1 += s * (wk[g] - wn[g]) - h2 * a1;
+      r2 += s * (wk[g + n] - wn[g + n]) - h2 * a2;
+      if (sl == 0) {
+        r1 -= s * wl[g];
+        r2 -= s * wl[g + n];
+      }
+      acc[0] = fma(fk[g], d1, acc[0]);
+      acc[0] = fma(fk[g + n], d2, acc[0]);
+    }
+    out[o] = op.a0 * s * in[o] + op.a1 * r1;
+    out[o + n] = op.a0 * s * in[o + n] + op.a1 * r2;
+  }
+  if (!bk_grid_reduce<1>(acc, partials, counter)) return;
+  out[Ns * M] = op.a0 * wT + op.a1 * (-0.5 / M) * s * acc[0];
+}
+
 // ------------------------------------------------------------------------------------------ host side
 static void fill_grid(bk_ctx* c, OpDesc& op) {
   op.kind = c->kind;
@@ -408,6 +472,9 @@ static int launch_kind(bk_ctx* c, const OpDesc& op, const double* in, const doub
     case BK_CGL2D:
       return bk_launch_ordered(c, k_cgl_apply<MODE>, bk_lin_grid(c, (long long)op.nx * op.ny), 256, 0, op, in, sp, out);
     case BK_POTRAP_CGL2D:
+      if (MODE == 0 && op.transpose)  // J': one kernel for the slices and the period entry
+        return bk_launch_ordered(c, k_potrap_apply_tr, bk_reduce_grid(c, (long long)op.nx * op.ny * op.nz), 256, 0, op, in, sp, out,
+                                 c->partials, c->counters + 9);
       BK_TRY(bk_launch_ordered(c, k_potrap_apply<MODE>, bk_lin_grid(c, (long long)op.nx * op.ny * op.nz), 256, 0, op, in, sp,
                                out));
       return bk_launch_ordered(c, k_potrap_phase, bk_reduce_grid(c, op.N - 1), 256, 0, op, in, sp, out, op.N - 1,

@@ -121,7 +121,7 @@ def locate_fold(rows, specialpoints, it, st):
     if cp.detect_fold and len(rows) > 2 and detect_fold(rows[-3]["param"], rows[-2]["param"], rows[-1]["param"]):
         specialpoints.append(SpecialPoint(type="fold", idx=len(rows) - 2, param=st.z_p, norm=it.normC(st.z_u), step=len(rows) - 2,
                                           status="guess", delta=(0, 0), ind_ev=0, interval=(rows[-2]["param"], rows[-2]["param"]),
-                                          x=V.copy(st.z_u), tau_p=st.tau_p))
+                                          x=V.copy(st.z_u), tau_p=st.tau_p, tau_u=V.copy(st.tau_u)))
         return True
     return False
 

@@ -98,8 +98,8 @@ def _eigvec(J, vals, vecs, k):
 
 def _adjoint_vector(prob, x0, p, lam, eigsolver, nev):
     """get_adjoint_basis(L★, conj(λ), eigsolver; nev) (src/NormalForms.jl:31-49): the eigenvector of J' whose eigenvalue is
-    closest to conj(λ).  J' is prob.Jt for host problems and J under bk_jac_set_transpose on the device.  A real λ gives a
-    real vector of the container of x0, a complex λ a complex host array."""
+    closest to conj(λ).  J' is prob.Jt where the problem has it (host problems, device kinds with a J' kernel), else J under
+    bk_jac_set_transpose.  A real λ gives a real vector of the container of x0, a complex λ a complex host array."""
     def adjoint(J):
         vals, vecs = _eig(eigsolver, J, nev)
         i = int(np.argmin(np.abs(vals - np.conj(lam))))

@@ -175,6 +175,19 @@ class BifurcationProblemB200:
         self._set(p)
         return self.ctx.jacobian(x)
 
+    @property
+    def Jt(self):
+        """jacobian_adjoint(prob, x, p) (src/Problems.jl:156) as prob.Jt(x, p): J' at (x, p), a handle with which the Krylov,
+        bordered and shift-invert solvers apply J' for the duration of a call.  Only the kinds with a J' kernel have it
+        (Context.has_adjoint), so that hasattr(prob, "Jt") is has_adjoint(prob)."""
+        if not self.ctx.has_adjoint:
+            raise AttributeError("Jt: J' is not available for this problem kind")
+        return self._jacobian_adjoint
+
+    def _jacobian_adjoint(self, x, p):
+        self._set(p)
+        return self.ctx.jacobian_adjoint(x)
+
     def d2F(self, x, p, dx1, dx2, out=None):
         """second differential of F in x (src/Problems.jl:165)"""
         self._set(p)

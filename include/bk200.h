@@ -140,7 +140,9 @@ int32_t bk_jvp(bk_ctx* ctx, const double* v, double* out, double a0, double a1);
 /* BK_COMPLEX contexts: imaginary part of the shift a0 of every later operator application (default 0) */
 int32_t bk_jac_set_shift_imag(bk_ctx* ctx, double a0_imag);
 /* apply J' instead of J from now on: apply_jacobian(prob, x, par, dx, true) / jacobian_adjoint (src/codim2/MinAugHopf.jl:79-81,
- * 152-155).  SH2d / SH3d / periodic SH2d are self-adjoint (no-op), cGL2d transposes its 2 x 2 reaction block; BK_CHAN / BK_POTRAP_CGL2D: error */
+ * 152-155).  SH2d / SH3d / periodic SH2d are self-adjoint (no-op), cGL2d transposes its 2 x 2 reaction block, BK_POTRAP_CGL2D
+ * applies J' of the Trapeze functional (one kernel, the period entry by a fixed-order reduction) and its BK_PC_POTRAP_CIRC
+ * preconditioner then applies the exact transpose P'^-1; BK_CHAN: error */
 int32_t bk_jac_set_transpose(bk_ctx* ctx, int32_t on);
 /* d2F(u; params)[dx1, dx2] and d3F(u; params)[dx1, dx2, dx3]: second / third differential of F in u at the
  * context's current params (bk_set_params, as bk_residual).  Host or device pointers, N0 doubles each.

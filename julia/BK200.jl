@@ -191,7 +191,8 @@ function (l::GMRESB200)(J::Jac, rhs; a₀ = VI.Zero(), a₁ = VI.One(), kwargs..
     return x, cv[] != 0, Int(it[])
 end
 # complex right-hand side / shift on a BK_COMPLEX context: the `shift = Complex(0, -ω)` solves of src/codim2/MinAugHopf.jl:17.
-# J.ctx must have been created with complex = true; jacobian_adjoint maps to transpose!(ctx, true).
+# J.ctx must have been created with complex = true; jacobian_adjoint maps to transpose!(ctx, true), which also selects J' of the
+# Trapeze functional on a BK_POTRAP_CGL2D context (and P'^-1 of its circulant preconditioner).  Not executed here.
 transpose!(c::Context, on::Bool) = check(c, ccall((:bk_jac_set_transpose, lib), Int32, (Ptr{Cvoid}, Int32), c.handle, on ? 1 : 0))
 function (l::GMRESB200)(J::Jac, rhs::AbstractVector{<:Complex}; a₀ = VI.Zero(), a₁ = VI.One(), kwargs...)
     c = J.ctx; s = ComplexF64(a₀ === VI.Zero() ? 0 : (a₀ === VI.One() ? 1 : a₀))
