@@ -178,6 +178,45 @@ class Context:
         _chk(self, self.lib.bk_d3f(self.handle, _l.ptr(u), _l.ptr(dx1), _l.ptr(dx2), _l.ptr(dx3), _l.ptr(out)))
         return out
 
+    def jet_moments(self, u, vecs, idx2=(), idx3=()):
+        """<v_i, d2F(u)[v_j, v_k]> for every row (i, j, k) of idx2, then <v_i, d3F(u)[v_j, v_k, v_l]> for every row (i, j, k, l)
+        of idx3, at the current params (bk_jet_moments): one host array of len(idx2) + len(idx3) values.  vecs: host or device
+        vectors.  Tuple lists longer than BK_JET_MOMENTS_MAX_TUPLES are split into several calls; with more than
+        BK_JET_MOMENTS_MAX_VEC vectors, the tuples are taken in order in groups that need at most that many distinct vectors, one
+        call per group (each vector is then read once per group that uses it)."""
+        idx2 = np.ascontiguousarray(np.reshape(idx2, (-1, 3)), dtype=np.int32)
+        idx3 = np.ascontiguousarray(np.reshape(idx3, (-1, 4)), dtype=np.int32)
+        n2, n3 = len(idx2), len(idx3)
+        cap = _l.BK_JET_MOMENTS_MAX_VEC
+        if len(vecs) > cap and all(0 <= int(i) < len(vecs) for i in np.concatenate([idx2.ravel(), idx3.ravel()])):
+            rows = [(0, r) for r in idx2] + [(1, r) for r in idx3]
+            out, t0 = np.zeros(n2 + n3), 0
+            while t0 < len(rows):
+                used, t1 = {}, t0
+                while t1 < len(rows):
+                    new = [int(i) for i in dict.fromkeys(rows[t1][1]) if int(i) not in used]
+                    if len(used) + len(new) > cap:
+                        break
+                    for i in new:
+                        used[i] = len(used)
+                    t1 += 1
+                g2 = [[used[int(i)] for i in r] for o, r in rows[t0:t1] if o == 0]
+                g3 = [[used[int(i)] for i in r] for o, r in rows[t0:t1] if o == 1]
+                out[t0:t1] = self.jet_moments(u, [vecs[i] for i in used], g2, g3)
+                t0 = t1
+            return out
+        out = np.zeros(n2 + n3)
+        pv = (C.c_void_p * len(vecs))(*[_l.ptr(v) for v in vecs])
+        ip = C.POINTER(C.c_int32)
+        step = _l.BK_JET_MOMENTS_MAX_TUPLES
+        for t0 in range(0, n2 + n3, step):
+            t1 = min(t0 + step, n2 + n3)
+            a2, a3 = idx2[min(t0, n2):min(t1, n2)], idx3[max(t0 - n2, 0):max(t1 - n2, 0)]
+            o = out[t0:t1]
+            _chk(self, self.lib.bk_jet_moments(self.handle, _l.ptr(u), len(vecs), pv, len(a2), a2.ctypes.data_as(ip), len(a3),
+                                               a3.ctypes.data_as(ip), o.ctypes.data_as(C.POINTER(C.c_double))))
+        return out
+
     def precond_setup(self, kind, a0=1.0, a1=1.0):
         _chk(self, self.lib.bk_precond_setup(self.handle, kind, a0, a1))
 

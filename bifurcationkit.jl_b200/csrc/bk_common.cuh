@@ -201,6 +201,11 @@ struct bk_ctx {
   double* host_pinned = nullptr; // pinned bounce buffer (ld doubles) for pageable host memory
   // generic temporaries for BLS/eigs
   std::vector<double*> tmp;
+  // bk_jet_moments, lazily allocated and grown: staged host vectors (N0 doubles each) and the tuples / results / partials
+  double* mom_stage = nullptr;
+  size_t mom_stage_cap = 0;  // bytes
+  void* mom_work = nullptr;
+  size_t mom_work_cap = 0;   // bytes
   // bk_vec_alloc pool: live allocations (ptr -> padded length) and the recycled free list
   std::unordered_map<double*, size_t> vec_live;
   std::vector<std::pair<size_t, double*>> vec_pool;

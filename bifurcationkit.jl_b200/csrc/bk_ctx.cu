@@ -195,6 +195,8 @@ extern "C" int32_t bk_ctx_destroy(bk_ctx* c) {
     if (b) cudaFree(b);
   for (double* b : c->tmp)
     if (b) cudaFree(b);
+  if (c->mom_stage) cudaFree(c->mom_stage);
+  if (c->mom_work) cudaFree(c->mom_work);
   if (c->h_pinned) cudaFreeHost(c->h_pinned);
   if (c->red_pinned) cudaFreeHost(c->red_pinned);
   if (c->coef_pinned) cudaFreeHost(c->coef_pinned);

@@ -240,6 +240,18 @@ __device__ __forceinline__ double chan_d3Nl(double x, double b) {
   const double h = 1.0 + b * x * x, x2 = x * x;
   return (-6.0 * b - 12.0 * b * x + 36.0 * b * b * x2 + 12.0 * b * b * x2 * x - 6.0 * b * b * b * x2 * x2) / (h * h * h * h);
 }
+// the per-point forms of the scalar kinds at point g, with ab = a[g] b[g] (c[g] is read for ORDER 3 only); chan: alpha = par[0],
+// beta = par[1]
+template <int ORDER>
+__device__ __forceinline__ double chan_jet(double alpha, double beta, double x, double ab, const double* c, long long g) {
+  if (ORDER == 2) return alpha * chan_d2Nl(x, beta) * ab;
+  return alpha * chan_d3Nl(x, beta) * ab * c[g];
+}
+// BK_SH2D, BK_SH3D, BK_SH2D_PERIODIC: F = -L1 u + l u + nu u^2 - u^3
+template <int ORDER>
+__device__ __forceinline__ double sh_jet(double nu, double u, double ab, const double* c, long long g) {
+  return ORDER == 2 ? (2.0 * nu - 6.0 * u) * ab : -6.0 * ab * c[g];
+}
 // cGL2d: NL(A) = (r + i nu) A - (c3 + i mu) |A|^2 A - c5 |A|^4 A (examples/cGL2d.jl:262-279).  With s = |A|^2 and
 // s_xy = 2 Re(x conj y), the forms are real-multilinear (s is not holomorphic):
 //   d2(s A)[a,b]     = s_ab A + s_A(a) b + s_A(b) a,                   s_A(x) = 2 Re(A conj x)
@@ -290,14 +302,91 @@ static __global__ void __launch_bounds__(256) k_jet(OpDesc op, const double* u, 
       const double x = u[g];
       const bool interior = g > 0 && g < n - 1;
       const double ab = a[g] * b[g];
-      double r;
-      if (ORDER == 2) r = op.par[0] * chan_d2Nl(x, op.par[1]) * ab;
-      else r = op.par[0] * chan_d3Nl(x, op.par[1]) * ab * c[g];
+      const double r = chan_jet<ORDER>(op.par[0], op.par[1], x, ab, c, g);
       out[g] = interior ? r : 0.0;
-    } else {  // BK_SH2D, BK_SH3D, BK_SH2D_PERIODIC: F = -L1 u + l u + nu u^2 - u^3
+    } else {  // the SH kinds
       const double ab = a[g] * b[g];
-      out[g] = ORDER == 2 ? (2.0 * op.par[1] - 6.0 * u[g]) * ab : -6.0 * ab * c[g];
+      out[g] = sh_jet<ORDER>(op.par[1], u[g], ab, c, g);
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------ jet moments
+// out[t] = <v_i, d2F(u)[v_j, v_k]> (tuple t < n2) or <v_i, d3F(u)[v_j, v_k, v_l]> (t >= n2) for a list of tuples over nvec
+// vectors, in one pass over the vectors: the per-point forms are those of k_jet, and the inner products are pointwise sums.
+// Each CTA stages a tile of BK_MOM_TP grid points of every vector (and of u) in shared memory, one row per (vector, field),
+// padded by one double so that the threads of a warp, each on its own tuple, read distinct rows from distinct banks.  Thread
+// t of the CTA owns the tuples t, t + 256, ..; it sums a tuple over the tile's points in order and adds the tile's sum to the
+// tuple's accumulator in shared memory.  The CTA's accumulators go to partials[blockIdx.x * ntup + t], which
+// k_jet_moments_fold sums over the CTAs in order: the summation order depends on the grid and the tuple list only.
+#define BK_MOM_TP 32
+struct MomVecs {
+  const double* v[BK_JET_MOMENTS_MAX_VEC + 1];  // the nvec vectors, then u
+};
+// KIND: BK_CHAN, BK_CGL2D, or BK_SH2D for the three SH kinds
+template <int KIND, int ORDER>
+__device__ __forceinline__ double moment_tile(const OpDesc& op, const double* __restrict__ s_v, int4 q, int urow, int np,
+                                              long long base, long long pts) {
+  constexpr int F = KIND == BK_CGL2D ? 2 : 1, LD = BK_MOM_TP + 1;
+  const double* vi = s_v + q.x * F * LD;
+  const double* va = s_v + q.y * F * LD;
+  const double* vb = s_v + q.z * F * LD;
+  const double* vc = s_v + (ORDER == 3 ? q.w : q.z) * F * LD;
+  const double* uu = s_v + urow * LD;
+  double s = 0.0;
+  for (int p = 0; p < np; ++p) {
+    if (KIND == BK_CGL2D) {
+      double o1, o2;
+      cgl_jet<ORDER>(cgl_par(op), make_double2(uu[p], uu[p + LD]), make_double2(va[p], va[p + LD]),
+                     make_double2(vb[p], vb[p + LD]), ORDER == 3 ? make_double2(vc[p], vc[p + LD]) : make_double2(0.0, 0.0),
+                     o1, o2);
+      s = fma(vi[p], o1, s);
+      s = fma(vi[p + LD], o2, s);
+    } else if (KIND == BK_CHAN) {
+      const long long g = base + p;
+      const double r = chan_jet<ORDER>(op.par[0], op.par[1], uu[p], va[p] * vb[p], vc, p);
+      s = fma(vi[p], g > 0 && g < pts - 1 ? r : 0.0, s);
+    } else {
+      s = fma(vi[p], sh_jet<ORDER>(op.par[1], uu[p], va[p] * vb[p], vc, p), s);
+    }
+  }
+  return s;
+}
+template <int KIND>
+static __global__ void __launch_bounds__(256) k_jet_moments(OpDesc op, MomVecs vs, int nvec, const int4* __restrict__ tup,
+                                                            int ntup, int n2, long long pts, double* __restrict__ partials) {
+  bk_pdl_sync();
+  constexpr int F = KIND == BK_CGL2D ? 2 : 1, LD = BK_MOM_TP + 1;
+  extern __shared__ double smem[];
+  const int rows = (nvec + 1) * F;
+  double* s_v = smem;                // rows x LD: row (vector, field), u last
+  double* s_acc = smem + rows * LD;  // ntup accumulators
+  for (int t = threadIdx.x; t < ntup; t += blockDim.x) s_acc[t] = 0.0;
+  const long long ntiles = (pts + BK_MOM_TP - 1) / BK_MOM_TP;
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const long long base = tile * BK_MOM_TP;
+    const int np = (int)(pts - base < BK_MOM_TP ? pts - base : BK_MOM_TP);
+    __syncthreads();  // the previous tile has been read
+    for (int e = threadIdx.x; e < rows * BK_MOM_TP; e += blockDim.x) {
+      const int r = e / BK_MOM_TP, p = e % BK_MOM_TP;
+      s_v[r * LD + p] = p < np ? vs.v[r / F][base + p + (r % F) * pts] : 0.0;
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < ntup; t += blockDim.x) {
+      const int4 q = tup[t];
+      s_acc[t] += t < n2 ? moment_tile<KIND, 2>(op, s_v, q, nvec * F, np, base, pts)
+                         : moment_tile<KIND, 3>(op, s_v, q, nvec * F, np, base, pts);
+    }
+  }
+  for (int t = threadIdx.x; t < ntup; t += blockDim.x) partials[(size_t)blockIdx.x * ntup + t] = s_acc[t];
+}
+// out[t] = the sum of the G partials of tuple t, in CTA order
+static __global__ void __launch_bounds__(256) k_jet_moments_fold(const double* __restrict__ partials, int ntup, int G,
+                                                                 double* __restrict__ out) {
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < ntup; t += gridDim.x * blockDim.x) {
+    double s = 0.0;
+    for (int b = 0; b < G; ++b) s += partials[(size_t)b * ntup + t];
+    out[t] = s;
   }
 }
 
@@ -603,6 +692,82 @@ extern "C" int32_t bk_d3f(bk_ctx* c, const double* u, const double* dx1, const d
   BkRange nvtx_range("bk_d3f");
   BK_CHECK(c, dx3 != nullptr, "null vector argument");
   return jet(c, u, dx1, dx2, dx3, out);
+}
+
+// grow a lazily allocated per-context buffer to at least `bytes` (its contents are not kept)
+static int grow(bk_ctx* c, void** buf, size_t* cap, size_t bytes) {
+  if (bytes <= *cap) return BK_OK;
+  if (*buf) {
+    BK_CUDA(c, cudaStreamSynchronize(c->stream));
+    BK_CUDA(c, cudaFree(*buf));
+    *buf = nullptr;
+    *cap = 0;
+  }
+  BK_CUDA(c, cudaMalloc(buf, bytes));
+  *cap = bytes;
+  return BK_OK;
+}
+
+extern "C" int32_t bk_jet_moments(bk_ctx* c, const double* u, int32_t nvec, const double* const* vecs, int32_t n2,
+                                  const int32_t* idx2, int32_t n3, const int32_t* idx3, double* out) {
+  BK_ENTER(c);
+  BkRange nvtx_range("bk_jet_moments");
+  const BkKindTraits* kt = bk_kind_traits(c->kind);
+  BK_CHECK(c, kt->has_jets, "d2F / d3F are not available for this problem kind");
+  BK_CHECK(c, !c->cplx, "d2F / d3F act on real states: not available in a BK_COMPLEX context");
+  BK_CHECK(c, nvec >= 1 && nvec <= BK_JET_MOMENTS_MAX_VEC, "bk_jet_moments: nvec out of range");
+  BK_CHECK(c, n2 >= 0 && n3 >= 0 && (long long)n2 + n3 <= BK_JET_MOMENTS_MAX_TUPLES, "bk_jet_moments: too many tuples");
+  BK_CHECK(c, u && vecs && out && (n2 == 0 || idx2) && (n3 == 0 || idx3), "null argument");
+  for (int i = 0; i < nvec; ++i) BK_CHECK(c, vecs[i] != nullptr, "null vector argument");
+  const int ntup = n2 + n3;
+  std::vector<int4> tup(ntup);
+  for (int t = 0; t < ntup; ++t) {
+    const int32_t* q = t < n2 ? idx2 + 3 * t : idx3 + 4 * (t - n2);
+    const int k = t < n2 ? 3 : 4;
+    for (int e = 0; e < k; ++e) BK_CHECK(c, q[e] >= 0 && q[e] < nvec, "bk_jet_moments: vector index out of range");
+    tup[t] = make_int4(q[0], q[1], q[2], k == 4 ? q[3] : 0);
+  }
+  if (ntup == 0) return BK_OK;
+  // host vectors (and u) are staged once, each into its own N0 row of the per-context buffer
+  const long long n = c->N0, pts = n / kt->fields;
+  MomVecs vs;
+  for (int i = 0; i <= nvec; ++i) {
+    const double* p = i < nvec ? vecs[i] : u;
+    if (bk_is_device_ptr(p)) {
+      vs.v[i] = p;
+      continue;
+    }
+    BK_TRY(grow(c, (void**)&c->mom_stage, &c->mom_stage_cap, 8 * (size_t)n * (nvec + 1)));
+    double* row = c->mom_stage + (size_t)n * i;
+    BK_CUDA(c, cudaMemcpyAsync(row, p, 8 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
+    c->stats.h2d_bytes += 8 * n;
+    vs.v[i] = row;
+  }
+  for (int i = nvec + 1; i <= BK_JET_MOMENTS_MAX_VEC; ++i) vs.v[i] = nullptr;
+  // work buffer: tuples | results | partials (G x ntup)
+  const int G = bk_reduce_grid(c, pts);
+  const size_t tup_bytes = 16 * (size_t)ntup, res_off = (tup_bytes + 255) / 256 * 256;
+  const size_t part_off = res_off + (8 * (size_t)ntup + 255) / 256 * 256;
+  BK_TRY(grow(c, &c->mom_work, &c->mom_work_cap, part_off + 8 * (size_t)ntup * G));
+  char* work = (char*)c->mom_work;
+  BK_CUDA(c, cudaMemcpyAsync(work, tup.data(), tup_bytes, cudaMemcpyHostToDevice, c->stream));
+  c->stats.h2d_bytes += tup_bytes;
+  const int4* dtup = (const int4*)work;
+  double* dres = (double*)(work + res_off);
+  double* dpart = (double*)(work + part_off);
+  const OpDesc op = bk_make_residual_op(c);
+  const size_t smem = 8 * ((size_t)(nvec + 1) * kt->fields * (BK_MOM_TP + 1) + ntup);
+  if (c->kind == BK_CGL2D)
+    BK_TRY(bk_launch(c, k_jet_moments<BK_CGL2D>, G, 256, smem, op, vs, (int)nvec, dtup, ntup, (int)n2, pts, dpart));
+  else if (c->kind == BK_CHAN)
+    BK_TRY(bk_launch(c, k_jet_moments<BK_CHAN>, G, 256, smem, op, vs, (int)nvec, dtup, ntup, (int)n2, pts, dpart));
+  else
+    BK_TRY(bk_launch(c, k_jet_moments<BK_SH2D>, G, 256, smem, op, vs, (int)nvec, dtup, ntup, (int)n2, pts, dpart));
+  BK_TRY(bk_launch_ordered(c, k_jet_moments_fold, (ntup + 255) / 256, 256, 0, (const double*)dpart, ntup, G, dres));
+  BK_CUDA(c, cudaMemcpyAsync(out, dres, 8 * (size_t)ntup, cudaMemcpyDeviceToHost, c->stream));
+  BK_CUDA(c, cudaStreamSynchronize(c->stream));
+  c->stats.d2h_bytes += 8 * ntup;
+  return BK_OK;
 }
 
 extern "C" int32_t bk_potrap_set_section(bk_ctx* c, const double* phi, const double* xpi) {

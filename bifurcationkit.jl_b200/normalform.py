@@ -13,11 +13,21 @@ Mirror of the reference:
   predictor (Hopf)       <->  predictor(hp::Hopf, ds)                       src/NormalForms.jl:1227-1281
   d2Fc / d3Fc            <->  d2Fc (src/Problems.jl:171-178): complex forms composed from real bk_d2f / bk_d3f calls
 
-The Hopf normal form keeps its complex vectors (ζ, ζ★, Ψ200) as host arrays: it is a handful of solves at one point.
-Branch switching from a Hopf point to periodic orbits is in periodic.py.
+  get_normal_formNd      <->  get_normal_formNd, autodiff = false           src/NormalForms.jl:656-896
+  (adjoint basis)        <->  get_adjoint_basis(L★, λs, eigsolver)          src/NormalForms.jl:1-24
+  biorthogonalise        <->  biorthogonalise(ζs, ζ★s)                      src/NormalForms.jl:51-91
+  NdBranchPointNF        <->  NdBranchPoint, its reduced form and bp(x, δp) src/NormalForms.jl:533-582
+  predictor_nd           <->  predictor(bp::NdBranchPoint, δp)              src/NormalForms.jl:916-985
+  multicontinuation      <->  multicontinuation(br, ind_bif, options_cont)  src/bifdiagram/BranchSwitching.jl:234-442
+  get_first_points_on_branch <-> get_first_points_on_branch                  src/bifdiagram/BranchSwitching.jl:298-352
 
-Not here: kernels of dimension > 1 (get_normal_formNd, multicontinuation), the generic BranchPoint predictor (_predictor,
-src/NormalForms.jl:496-535), usedeflation, bothside and bifurcationdiagram; higher codimension normal forms.
+The Hopf normal form keeps its complex vectors (ζ, ζ★, Ψ200) as host arrays: it is a handful of solves at one point.
+Branch switching from a Hopf point to periodic orbits is in periodic.py.  The N-dimensional normal form makes every inner
+product of a jet with ζ★ᵢ in one `bk_jet_moments` pass (prob.jet_moments); host problems get the same contractions from a jet
+call and a dot product per tuple (jet_moments_composed).
+
+Not here: the generic BranchPoint predictor (_predictor, src/NormalForms.jl:496-535), usedeflation = false, bothside and
+bifurcationdiagram; higher codimension normal forms.
 """
 import copy
 import itertools
@@ -96,24 +106,34 @@ def _eigvec(J, vals, vecs, k):
     return v + 1j * (lam.real * v - _host(_apply(J, np.ascontiguousarray(v)))) / lam.imag
 
 
-def _adjoint_vector(prob, x0, p, lam, eigsolver, nev):
-    """get_adjoint_basis(L★, conj(λ), eigsolver; nev) (src/NormalForms.jl:31-49): the eigenvector of J' whose eigenvalue is
-    closest to conj(λ).  J' is prob.Jt where the problem has it (host problems, device kinds with a J' kernel), else J under
-    bk_jac_set_transpose.  A real λ gives a real vector of the container of x0, a complex λ a complex host array."""
+def _adjoint_basis(prob, x0, p, lams, eigsolver, nev):
+    """get_adjoint_basis(L★, λs, eigsolver; nev) (src/NormalForms.jl:1-24): from one eigen-solve of J', for each λ of `lams` in
+    turn the eigenvector whose eigenvalue is closest to conj(λ), each eigenvalue used once.  J' is prob.Jt where the problem has
+    it (host problems, device kinds with a J' kernel), else J under bk_jac_set_transpose.  A real λ gives a real vector of the
+    container of x0, a complex λ a complex host array.  Returns (vectors, their eigenvalues)."""
     def adjoint(J):
         vals, vecs = _eig(eigsolver, J, nev)
-        i = int(np.argmin(np.abs(vals - np.conj(lam))))
-        if np.imag(lam) == 0:
-            return vals[i], _like(x0, np.asarray(vecs)[:, i])
-        return vals[i], _eigvec(J, vals, vecs, i)
+        free = np.array(vals, dtype=complex)
+        out, found = [], []
+        for lam in lams:
+            i = int(np.argmin(np.abs(free - np.conj(lam))))
+            free[i] = 1e9                                        # not used twice (:21)
+            found.append(vals[i])
+            out.append(_like(x0, np.asarray(vecs)[:, i]) if np.imag(lam) == 0 else _eigvec(J, vals, vecs, i))
+        return out, found
     if hasattr(prob, "Jt"):
-        val, vec = adjoint(prob.Jt(x0, p))
-    else:
-        prob.ctx.set_transpose(True)
-        try:
-            val, vec = adjoint(prob.J(x0, p))
-        finally:
-            prob.ctx.set_transpose(False)
+        return adjoint(prob.Jt(x0, p))
+    prob.ctx.set_transpose(True)
+    try:
+        return adjoint(prob.J(x0, p))
+    finally:
+        prob.ctx.set_transpose(False)
+
+
+def _adjoint_vector(prob, x0, p, lam, eigsolver, nev):
+    """get_adjoint_basis(L★, conj(λ), eigsolver; nev) (src/NormalForms.jl:31-49): the eigenvector of J' whose eigenvalue is
+    closest to conj(λ) (_adjoint_basis for one λ)."""
+    (vec,), (val,) = _adjoint_basis(prob, x0, p, [lam], eigsolver, nev)
     if abs(val.real) > 1e-2:
         warnings.warn(f"The bifurcating eigenvalue is not that close to Re = 0. We found {val.real} !≈ 0. "
                       "You can perhaps increase the argument `nev`.")
@@ -439,8 +459,8 @@ def continuation_from_bp(br, ind_bif, prob, alg, contpar, normC=V.norm2, ds=None
     if bifpt.type not in ("bp", "nd"):
         raise ValueError(f"You cannot branch from a :{bifpt.type} point using these arguments.")
     if abs(bifpt.delta[0]) > 1:
-        raise NotImplementedError(f"branch switching at a point with a {abs(bifpt.delta[0])}-dimensional kernel "
-                                  "(multicontinuation, src/bifdiagram/BranchSwitching.jl:234-330) is not implemented")
+        raise NotImplementedError(f"branch switching at a point with a {abs(bifpt.delta[0])}-dimensional kernel goes through "
+                                  "normalform.multicontinuation (src/bifdiagram/BranchSwitching.jl:234-442)")
     ds = contpar.ds if ds is None else ds
     nev = contpar.nev if nev is None else nev
     it = ContIterable(prob, alg, contpar, normC)
@@ -458,3 +478,362 @@ def continuation_from_bp(br, ind_bif, prob, alg, contpar, normC=V.norm2, ds=None
         prob2.params = list(prob.params)
         prob2.params[prob.lens] = bp.p
     return events.continuation(prob2, alg, cp, normC, verbose=verbose, callback=callback, u1=pred.x1, p1=pred.p), bp
+
+
+# ------------------------------------------------------------------------------------------------ kernels of dimension N > 1
+def jet_moments_composed(prob, x0, p, vecs, idx2=(), idx3=()):
+    """<v_i, d2F(x0, p)[v_j, v_k]> for the rows (i, j, k) of idx2, then <v_i, d3F(x0, p)[v_j, v_k, v_l]> for the rows of idx3: one
+    jet call and one dot product per tuple.  It serves problems that bring only d2F / d3F, and it is what the one-pass device
+    contraction (prob.jet_moments, bk_jet_moments) is checked against."""
+    idx2, idx3 = np.reshape(np.asarray(idx2, dtype=int), (-1, 3)), np.reshape(np.asarray(idx3, dtype=int), (-1, 4))
+    out = [V.dot(vecs[i], prob.d2F(x0, p, vecs[j], vecs[k])) for i, j, k in idx2]
+    out += [V.dot(vecs[i], prob.d3F(x0, p, vecs[j], vecs[k], vecs[l])) for i, j, k, l in idx3]
+    return np.array(out, dtype=float)
+
+
+def jet_moments(prob, x0, p, vecs, idx2=(), idx3=()):
+    """the contractions of jet_moments_composed, in one pass over the vectors where the problem has it (prob.jet_moments)"""
+    if hasattr(prob, "jet_moments"):
+        return prob.jet_moments(x0, p, vecs, idx2, idx3)
+    return jet_moments_composed(prob, x0, p, vecs, idx2, idx3)
+
+
+def _lincomb(coefs, vecs):
+    """sum_j coefs[j] vecs[j], a new vector of the container of vecs[0]"""
+    y = V.zeros_like(vecs[0])
+    for c, v in zip(coefs, vecs):
+        if c != 0:
+            V.axpby(y, float(c), v, 1.0)
+    return y
+
+
+def _gram(a, b):
+    return np.array([[V.dot(x, y) for y in b] for x in a])
+
+
+def biorthogonalise(zetas, zetas_ad):
+    """biorthogonalise(ζs, ζ★s) (src/NormalForms.jl:51-91): ζ★s <- Q' ζ★s with Q = pinv(G), G_ij = <ζ_i, ζ★_j>; when G is then
+    not the identity to 1e-5, the LU algorithm (G = P L U: ζs <- (P L)^-1 ζs, ζ★s <- U'^-1 ζ★s), which also changes ζs.
+    Raises as the reference does when G is singular or the result is not biorthogonal."""
+    import scipy.linalg as sla
+    assert len(zetas) == len(zetas_ad), "The Gram matrix is not square!"
+    G = _gram(zetas, zetas_ad)
+    if abs(np.linalg.det(G)) <= 1e-14:
+        raise RuntimeError(f"The Gram matrix is not invertible! det(G) = {np.linalg.det(G)}, G =\n{G}\n"
+                           "You can perhaps increase the argument `nev`.")
+    Q = np.linalg.pinv(G)
+    new_ad = [_lincomb(Q[:, i], zetas_ad) for i in range(len(zetas))]                  # (Q' ζ★s)_i = sum_j Q_ji ζ★_j
+    if np.max(np.abs(_gram(zetas, new_ad) - np.eye(len(zetas)))) >= 1e-5:
+        warnings.warn("Gram matrix not equal to identity. Switching to LU algorithm.\n This modifies the basis of right eigenvectors!")
+        Pm, Lm, Um = sla.lu(G)
+        M, Ui = np.linalg.inv(Pm @ Lm), np.linalg.inv(Um)
+        zetas = [_lincomb(M[i], zetas) for i in range(len(zetas))]
+        new_ad = [_lincomb(Ui[:, i], zetas_ad) for i in range(len(zetas))]
+    G = _gram(zetas, new_ad)
+    if not np.max(np.abs(G - np.eye(len(zetas)))) < 1e-5:
+        raise RuntimeError("Failure in bi-orthogonalisation of the right / left eigenvectors.\nThe left eigenvectors do not form "
+                           f"a basis.\nYou may want to increase `nev`, G =\n{G}")
+    return zetas, new_ad
+
+
+@dataclass
+class NdBranchPointNF:
+    """NdBranchPoint of src/NormalForms.jl:533-582 (fields of the point): (x0, p), the tangent (tau_u, tau_p), the kernel basis
+    zetas and the adjoint basis zetas_ad with <ζ_i, ζ★_j> = δ_ij, and in `nf` the coefficients a01 (N), a02 (N), b11 (N x N), b20
+    (N x N x N), b30 (N x N x N x N) of the reduced equation; type "N-d" or "NonQuadraticParameter" (:882)."""
+    x0: object
+    p: float
+    tau_u: object
+    tau_p: float
+    zetas: list
+    zetas_ad: list
+    nf: dict
+    type: str
+
+    def reduced_form(self, x, dp):
+        """bp(Val(:reducedForm), x, dp) (:541-574): a01 dp + dp b11 x + b20[x, x] / 2 + b30[x, x, x] / 6 (the a02 term carries the
+        reference's factor 0 dp)"""
+        nf, x = self.nf, np.asarray(x, dtype=float)
+        if len(x) != len(self.zetas):
+            raise ValueError(f"N = {len(self.zetas)} and length(x) = {len(x)} should match!")
+        return (dp * nf["a01"] + dp * nf["b11"] @ x + np.einsum("ijk,j,k->i", nf["b20"], x, x) / 2
+                + np.einsum("ijkl,j,k,l->i", nf["b30"], x, x, x) / 6)
+
+    def reduced_jacobian(self, x, dp):
+        """the derivative of reduced_form in x"""
+        nf, x = self.nf, np.asarray(x, dtype=float)
+        b20, b30 = nf["b20"], nf["b30"]
+        return (dp * nf["b11"] + (np.einsum("imk,k->im", b20, x) + np.einsum("ijm,j->im", b20, x)) / 2
+                + (np.einsum("imkl,k,l->im", b30, x, x) + np.einsum("ijml,j,l->im", b30, x, x)
+                   + np.einsum("ijkm,j,k->im", b30, x, x)) / 6)
+
+    def __call__(self, x, dp):
+        """bp(x, δp) (:576-582): x0 + sum_i x_i ζ_i"""
+        y = V.copy(self.x0)
+        for xi, z in zip(x, self.zetas):
+            V.axpby(y, float(xi), z, 1.0)
+        return y
+
+
+def get_normal_formNd(it, br, ind_bif, nev=None, zetas=None, zetas_ad=None, bls=None, tol_fold=1e-3):
+    """get_normal_formNd(prob, br, id_bif; autodiff = false) (src/NormalForms.jl:656-896) at the point br.specialpoint[ind_bif],
+    whose kernel has dimension N = |delta[0]| > 1, of the branch `br` computed by events.continuation over the iterator `it`.
+    zetas: a basis of the kernel; otherwise the eigenvectors ind_ev - N + 1 .. ind_ev, saved with the branch or recomputed with
+    newton_options.eigsolver; each is divided by its norm.  zetas_ad: the adjoint basis; otherwise ζs for a symmetric problem,
+    else the eigenvectors of J' closest to conj(λs).  Both are biorthogonalised.  bls: the solver of the singular systems,
+    through its solve_block with the borders (ζ★₁, ζ★₂; ζ₁, ζ₂) of the reference; MatrixFreeBLSB200 over the Newton linear
+    solver by default.  For N > 2 that two-border system is singular (its kernel is span(ζ₃ .. ζ_N)), so each solution is
+    projected to <ζ_i, ψ> = 0 for every i, the solution an N-border solve would give (DESIGN.md §2).  Every inner product of a
+    jet with ζ★ᵢ goes through one `jet_moments` call: one kernel pass over the 2N + 1 + N(N+1)/2 vectors up to N = 9, several
+    beyond (Context.jet_moments groups the tuples).  Returns an NdBranchPointNF."""
+    prob, options = it.prob, it.contpar.newton_options
+    bifpt = br.specialpoint[ind_bif]
+    N = abs(bifpt.delta[0])
+    if N < 2:
+        raise ValueError(f"get_normal_formNd needs a kernel of dimension > 1, here {N}: use get_normal_form1d.")
+    bls = bls or MatrixFreeBLSB200(options.linsolver)
+    x0, p, delta = bifpt.x, bifpt.param, prob.delta
+    entry = next(e for e in br.eig if e["step"] == bifpt.idx)
+    rightEv = np.asarray(entry["eigenvals"])
+    nev = max(2 * N, len(rightEv) if nev is None else nev)                               # :680-681
+    ind = list(range(bifpt.ind_ev - N, bifpt.ind_ev))                                    # indev-N+1:indev, 0-based
+    lams = rightEv[ind]
+    if zetas is None:                                                                    # :711-724
+        if entry.get("eigenvecs") is not None:
+            vecs = np.asarray(entry["eigenvecs"])
+        else:
+            vals, vecs = _eig(options.eigsolver, prob.J(x0, p), max(nev, len(rightEv)))
+            if np.max(np.abs(vals[: len(rightEv)] - rightEv)) > it.contpar.tol_stability:
+                warnings.warn(f"We did not find the correct eigenvalues. We found {vals[: len(rightEv)]} instead of {rightEv}.")
+        zetas = [_like(x0, np.asarray(vecs)[:, i]) for i in ind]
+    else:
+        zetas = [_like(x0, z) if isinstance(z, (list, np.ndarray)) else V.copy(z) for z in zetas]
+    for z in zetas:                                                                      # scaleζ = norm, :729
+        V.scale(z, 1.0 / V.norm2(z))
+    if zetas_ad is not None:                                                             # :737-747
+        zetas_ad = [_like(x0, z) if isinstance(z, (list, np.ndarray)) else V.copy(z) for z in zetas_ad]
+    elif getattr(prob, "symmetric", False):
+        zetas_ad = [V.copy(z) for z in zetas]
+    else:
+        zetas_ad, found = _adjoint_basis(prob, x0, p, lams, options.eigsolver, nev)   # it compares with conj(λ)
+        for val in found:
+            if abs(val.real) > 1e-2:
+                warnings.warn(f"Did not converge to the requested eigenvalues. We found {val.real} !≈ 0. This might not lead to "
+                              "precise normal form computation. You can perhaps increase the argument `nev`.")
+        zetas_ad = [z if not np.iscomplexobj(z) else _like(x0, z) for z in zetas_ad]    # real.(ζ★s), :748
+    zetas, zetas_ad = biorthogonalise(zetas, zetas_ad)                                   # :752
+
+    gram_inv = np.linalg.inv(_gram(zetas, zetas)) if N > 2 else None
+
+    def E(x):  # E_nd (:648-654): x - sum_i <x, ζ★_i> ζ_i, a new vector
+        return _lincomb([1.0] + [-V.dot(x, za) for za in zetas_ad], [x] + zetas)
+
+    def solve(rhs, what):  # solve_bls_block(bls, L, (ζ★₁, ζ★₂), (ζ₁, ζ₂), 0, rhs, 0) (:759-763), L re-made before each solve
+        psi, _, cv, its = bls.solve_block(prob.J(x0, p), tuple(zetas_ad[:2]), tuple(zetas[:2]), np.zeros((2, 2)), rhs, np.zeros(2))
+        if not cv:
+            warnings.warn(f"[Normal form Nd {what}] linear solver did not converge. it = {its}")
+        if gram_inv is not None:  # N > 2: the component in span(ζ₃ .. ζ_N) the two borders leave free, removed
+            c = gram_inv @ np.array([V.dot(z, psi) for z in zetas])
+            psi = _lincomb([1.0] + list(-c), [psi] + zetas)
+        return psi
+
+    def central(fp, fm):  # (fp - fm) / 2δ, in fp
+        return V.scale(V.axpby(fp, -1.0, fm, 1.0), 1.0 / (2 * delta))
+
+    dF = lambda q, v: _apply(prob.J(x0, q), v)
+    Fp, F0, Fm = prob.F(x0, p + delta), prob.F(x0, p), prob.F(x0, p - delta)            # :774-780
+    R02 = V.axpby(V.axpby(V.copy(Fp), -2.0, F0, 1.0), 1.0, Fm, 1.0)
+    V.scale(R02, 1.0 / delta**2)
+    R01 = central(Fp, Fm)
+    a01 = np.array([V.dot(R01, za) for za in zetas_ad])                                 # :782-784
+    # The reference re-solves the Ψ01 system inside its jj loop (:798) and the wst system of each ordered pair inside its b30
+    # loop (:844-857).  The device solver is deterministic, so one solve for Ψ01 gives the reference's numbers exactly, and so
+    # does one wst solve per unordered pair {k, l} where d2F is symmetric bit for bit: the SH kinds and chan, whose pointwise
+    # products commute.  For cGL2d (cgl_jet adds its terms in argument order) and host d2F the two orders agree to rounding.
+    Psi01 = solve(V.scale(E(R01), -1.0), "Ψ01")
+    R11 = [central(dF(p + delta, z), dF(p - delta, z)) for z in zetas]                   # :790-796
+    R11Psi = central(dF(p + delta, Psi01), dF(p - delta, Psi01))                         # :806-811 (the same for every jj)
+    a2v = V.axpby(R02, 2.0, R11Psi, 1.0)
+    pairs = [(k, l) for k in range(N) for l in range(k, N)]
+    w = {kl: solve(E(prob.d2F(x0, p, zetas[kl[0]], zetas[kl[1]])), "wst") for kl in pairs}
+    triples = [(j, k, l) for j in range(N) for k in range(N) for l in range(N) if j == k or j < k < l]   # :841
+    # one contraction pass: vectors ζ★ (0..N-1), ζ (N..2N-1), Ψ01 (2N), w_{kl} (2N+1..)
+    Z, ps = (lambda j: N + j), 2 * N
+    W = {kl: 2 * N + 1 + n for n, kl in enumerate(pairs)}
+    wid = lambda a, b: W[(min(a, b), max(a, b))]
+    idx2, idx3, at = [], [], {}
+    for i in range(N):
+        for j, k in pairs:                                                               # b20, :820-828
+            at["b20", i, j, k] = len(idx2); idx2.append((i, Z(j), Z(k)))
+        for j in range(N):                                                               # b11: R2(ζ_j, Ψ01), :800
+            at["b11", i, j] = len(idx2); idx2.append((i, Z(j), ps))
+        at["a02", i] = len(idx2); idx2.append((i, ps, ps))                               # a02: R2(Ψ01, Ψ01), :812
+        for j, k, l in triples:                                                          # b30, :842-857
+            at["b3w", i, j, k, l] = len(idx2)
+            idx2 += [(i, Z(j), wid(l, k)), (i, Z(k), wid(l, j)), (i, Z(l), wid(k, j))]
+            at["b3", i, j, k, l] = len(idx3); idx3.append((i, Z(j), Z(k), Z(l)))
+    vecs = list(zetas_ad) + list(zetas) + [Psi01] + [w[kl] for kl in pairs]
+    m = jet_moments(prob, x0, p, vecs, idx2, idx3)
+    m2, m3 = m[: len(idx2)], m[len(idx2):]
+
+    b11 = np.zeros((N, N)); a02 = np.zeros(N)
+    b20 = np.zeros((N, N, N)); b30 = np.zeros((N, N, N, N))
+    for i in range(N):
+        for j in range(N):
+            b11[i, j] = V.dot(R11[j], zetas_ad[i]) + m2[at["b11", i, j]]
+        a02[i] = V.dot(a2v, zetas_ad[i]) + m2[at["a02", i]]
+        for j, k in pairs:
+            b20[i, j, k] = b20[i, k, j] = m2[at["b20", i, j, k]]
+        for j, k, l in triples:
+            t = at["b3w", i, j, k, l]
+            c = m3[at["b3", i, j, k, l]] - m2[t] - m2[t + 1] - m2[t + 2]
+            for I in itertools.permutations((j, k, l)):
+                b30[(i,) + I] = c
+    nf = dict(a01=a01, a02=a02, b11=b11, b20=b20, b30=b30)
+    tp = "NonQuadraticParameter" if max(np.max(np.abs(a01)), np.max(np.abs(a02)), np.max(np.abs(b11))) < tol_fold else f"{N}-d"
+    return NdBranchPointNF(x0=x0, p=p, tau_u=bifpt.tau_u, tau_p=bifpt.tau_p, zetas=zetas, zetas_ad=zetas_ad, nf=nf, type=tp)
+
+
+class _Dense:
+    """a small dense Jacobian: apply(J, v) and its matrix"""
+
+    def __init__(self, A):
+        self.A = A
+
+    def __call__(self, v):
+        return self.A @ v
+
+
+def _dense_solve(J, rhs, rhs2=None, a0=0.0, a1=1.0):
+    """the linear solver of the reduced equation, in the one- and two-right-hand-side forms"""
+    A = a0 * np.eye(len(rhs)) + a1 * J.A
+    if rhs2 is None:
+        return np.linalg.solve(A, rhs), True, 1
+    x = np.linalg.solve(A, np.column_stack([rhs, rhs2]))
+    return np.ascontiguousarray(x[:, 0]), np.ascontiguousarray(x[:, 1]), True, (1, 1)
+
+
+class _ReducedProblem:
+    """the reduced equation perturb(bp.reduced_form(x, dp)) = 0 as a host problem for newton_deflated, with the analytic Jacobian
+    of the cubic (the reference differentiates it with ForwardDiff)"""
+
+    def __init__(self, bp, perturb):
+        self.bp, self.perturb = bp, perturb
+        self.u0, self.p0, self.delta = np.zeros(len(bp.zetas)), 0.0, 1e-8
+
+    def F(self, x, p, out=None):
+        r = np.asarray(self.perturb(self.bp.reduced_form(x, p)), dtype=float)
+        if out is not None:
+            out[...] = r
+            return out
+        return r
+
+    def J(self, x, p):
+        return _Dense(self.bp.reduced_jacobian(x, p))
+
+
+def _newton_deflated(prob, x0, p, defop, opts, normN):
+    """deflation.newton_deflated, with a diverging run (iterates beyond float range, where the reference's cbMaxNorm(1e100)
+    stops) or an iterate exactly on a deflated root (M(u) = 1 / 0, an infinite residual in the reference) returned as a failed
+    solve from the guess"""
+    from .deflation import newton_deflated
+    from .palc import NonLinearSolution
+    try:
+        return newton_deflated(prob, x0, p, defop, opts, normN)
+    except (ZeroDivisionError, OverflowError):
+        return NonLinearSolution(V.copy(x0), p, [math.inf], False, 0, 0)
+
+
+def predictor_nd(bp, dp, rng=None, ampfactor=1.0, nbfailures=50, maxiter=100, igs=None, amp_igs=1.0, normN=None,
+                 perturb=lambda r: r, tol=1e-12):
+    """predictor(bp::NdBranchPoint, δp) (src/NormalForms.jl:916-985): the zeros of the reduced equation at dp = -|δp| and +|δp|,
+    by deflated Newton (DeflationOperator(2, 0.1, [0]) per side, newton_deflated with NewtonPar(tol, maxiter)) from the vertices
+    of {-1, 0, 1}^N (scaled by amp_igs, or the guesses igs), then from random restarts until nbfailures of them fail.  rng: a
+    numpy.random.Generator (default_rng(0) by default), so that the result is reproducible.  perturb is applied to the reduced
+    residual, as the reference's.  The Jacobian is the analytic one of the cubic.  Returns (before, after): the roots found on
+    each side, the trivial one first, each multiplied by ampfactor."""
+    from .deflation import DeflationOperator
+    from .palc import NewtonPar
+    rng = np.random.default_rng(0) if rng is None else rng
+    n = len(bp.zetas)
+    normN = normN or (lambda v: float(np.max(np.abs(v))))
+    opts = NewtonPar(tol=tol, max_iterations=maxiter, linsolver=_dense_solve)
+    guesses = list(itertools.product((-1, 0, 1), repeat=n)) if igs is None else list(igs)
+
+    def roots(ds):
+        defop = DeflationOperator(2, 0.1, [np.zeros(n)])
+        prob = _ReducedProblem(bp, perturb)
+        u0 = rng.random(n) - 0.5
+        for ci in guesses:                                                               # :954-964
+            ci = np.asarray(ci, dtype=float)
+            if np.linalg.norm(ci) > 0:
+                u0 = ci * amp_igs
+                sol = _newton_deflated(prob, u0, ds, defop, opts, normN)
+                if sol.converged:
+                    defop.push(ampfactor * sol.u)
+        failures = 0
+        while failures < nbfailures:                                                     # :966-976
+            sol = _newton_deflated(prob, u0, ds, defop, opts, normN)
+            if sol.converged:
+                defop.push(ampfactor * sol.u)
+            else:
+                failures += 1
+            u0 = sol.u + 0.1 * (rng.random(n) - 0.5)
+        return defop.roots
+    return roots(-abs(dp)), roots(abs(dp))
+
+
+def get_first_points_on_branch(bp, solfromRE, prob, contpar, ds=None, max_iter_deflation=None, perturb_guess=lambda x: x,
+                               normN=V.norm2):
+    """get_first_points_on_branch(br, bpnf, solfromRE) (src/bifdiagram/BranchSwitching.jl:298-352): deflated Newton
+    (newton_deflated: DeflatedProblemCustomLS around the Newton linear solver) on the full problem at p + |ds| from bp(root) for
+    every root after the bifurcation point, then at p - |ds| for those before, each side with its own DeflationOperator(2, 1, []).
+    Returns a namespace (before, after: the converged states, bpm = p - |ds|, bpp = p + |ds|)."""
+    from .deflation import DeflationOperator
+    ds = abs(contpar.ds if ds is None else ds)
+    optn = contpar.newton_options
+    optnDf = replace(optn, max_iterations=min(50, 15 * optn.max_iterations) if max_iter_deflation is None else max_iter_deflation)
+    before, after = solfromRE
+
+    def side(roots, q):
+        defop = DeflationOperator(2, 1.0, [])
+        for xsol in roots:
+            sol = _newton_deflated(prob, perturb_guess(bp(xsol, ds)), q, defop, optnDf, normN)
+            if sol.converged:
+                defop.push(sol.u)
+        return defop.roots
+    after = side(after, bp.p + ds)
+    before = side(before, bp.p - ds)
+    return types.SimpleNamespace(before=before, after=after, bpm=bp.p - ds, bpp=bp.p + ds)
+
+
+def multicontinuation(br, ind_bif, prob, alg, contpar, normC=V.norm2, ds=None, ampfactor=1.0, nev=None, zetas=None, zetas_ad=None,
+                      bpnf=None, solfromRE=None, bls=None, tol_fold=1e-3, rng=None, max_iter_deflation=None,
+                      perturb_guess=lambda x: x, callback=None, verbose=False):
+    """multicontinuation(br, ind_bif, options_cont) (src/bifdiagram/BranchSwitching.jl:234-442): automatic branch switching at the
+    point br.specialpoint[ind_bif], whose kernel has dimension > 1, of a branch of `prob` computed by events.continuation.  The
+    normal form (get_normal_formNd with nev, zetas, zetas_ad, bls, tol_fold; or the precomputed `bpnf`), the roots of its reduced
+    equation at p ∓ |ds| (predictor_nd with ampfactor and rng; or `solfromRE` = (before, after)), their corrections on the full
+    problem (get_first_points_on_branch), then one events.continuation (alg, contpar, normC) from the two points (x0, p) and
+    (root, p ∓ |ds|) for every corrected root after the first, which is the trivial branch: contpar.ds = -|ds| before the point,
+    +|ds| after it (:432-437).  ds: contpar.ds by default.  `prob` and `contpar` are left as they are.  Returns a list of
+    (Branch, NdBranchPointNF)."""
+    it = ContIterable(prob, alg, contpar, normC)
+    bp = bpnf or get_normal_formNd(it, br, ind_bif, nev=contpar.nev if nev is None else nev, zetas=zetas, zetas_ad=zetas_ad,
+                                   bls=bls, tol_fold=tol_fold)
+    dp = abs(contpar.ds if ds is None else ds)
+    roots = solfromRE or predictor_nd(bp, dp, rng=rng, ampfactor=ampfactor)
+    first = get_first_points_on_branch(bp, roots, prob, contpar, dp, max_iter_deflation, perturb_guess, normN=normC)
+    prob2 = copy.copy(prob)                                                              # re_make(prob; params = par0)
+    prob2.u0, prob2.p0 = bp.x0, bp.p
+    if hasattr(prob2, "params"):
+        prob2.params = list(prob.params)
+        prob2.params[prob.lens] = bp.p
+    dscont = abs(contpar.ds)
+
+    def cont(u1, p1, sign):
+        cp = replace(contpar, ds=sign * dscont)
+        return events.continuation(prob2, alg, cp, normC, verbose=verbose, callback=callback, u1=u1, p1=p1), bp
+    out = [cont(u, first.bpm, -1.0) for u in first.before[1:]]
+    out += [cont(u, first.bpp, 1.0) for u in first.after[1:]]
+    return out

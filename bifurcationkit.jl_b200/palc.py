@@ -198,6 +198,12 @@ class BifurcationProblemB200:
         self._set(p)
         return self.ctx.d3f(x, dx1, dx2, dx3, out)
 
+    def jet_moments(self, x, p, vecs, idx2=(), idx3=()):
+        """<v_i, d2F(x, p)[v_j, v_k]> for the rows (i, j, k) of idx2, then <v_i, d3F(x, p)[v_j, v_k, v_l]> for the rows of idx3, in
+        one pass over the vectors (Context.jet_moments)"""
+        self._set(p)
+        return self.ctx.jet_moments(x, vecs, idx2, idx3)
+
     @property
     def symmetric(self):
         """is_symmetric(prob) (src/Problems.jl:126): J' = J for the Swift-Hohenberg kinds"""

@@ -154,6 +154,20 @@ int32_t bk_jac_set_transpose(bk_ctx* ctx, int32_t on);
  * src/Problems.jl:171-178). */
 int32_t bk_d2f(bk_ctx* ctx, const double* u, const double* dx1, const double* dx2, double* out);
 int32_t bk_d3f(bk_ctx* ctx, const double* u, const double* dx1, const double* dx2, const double* dx3, double* out);
+/* The contractions of the jets with vectors that the normal form of a branch point with an N-dimensional kernel needs
+ * (the inner products <ζ★_i, d2F[.,.]>, <ζ★_i, d3F[.,.,.]> of get_normal_formNd, src/NormalForms.jl:656-896), in one pass over
+ * the nvec vectors vecs[0 .. nvec-1] and u (host or device pointers, N0 doubles each), at the context's current params:
+ *   out[t]      = <v_i, d2F(u)[v_j, v_k]>        (i, j, k)    = idx2[3t .. 3t+2],  t < n2
+ *   out[n2 + t] = <v_i, d3F(u)[v_j, v_k, v_l]>   (i, j, k, l) = idx3[4t .. 4t+3],  t < n3
+ * <.,.> is the plain dot product over the N0 unknowns; the jets are those of bk_d2f / bk_d3f.  idx2, idx3 and out are host
+ * arrays; out holds n2 + n3 doubles.  Host vectors are staged once per call into a per-context buffer kept for later calls.
+ * The sums run in an order fixed by the grid and the tuple list: two calls on the same inputs, host or device, give the same
+ * bits.  BK_ERR_ARG before any launch: the refusals of bk_d2f, nvec outside [1, BK_JET_MOMENTS_MAX_VEC], n2 + n3 above
+ * BK_JET_MOMENTS_MAX_TUPLES (split longer lists into several calls), an index outside [0, nvec), a null pointer. */
+#define BK_JET_MOMENTS_MAX_VEC 64
+#define BK_JET_MOMENTS_MAX_TUPLES 8192
+int32_t bk_jet_moments(bk_ctx* ctx, const double* u, int32_t nvec, const double* const* vecs, int32_t n2, const int32_t* idx2,
+                       int32_t n3, const int32_t* idx3, double* out);
 
 /* ---- K6: preconditioner --------------------------------------------------------------------- */
 int32_t bk_precond_setup(bk_ctx* ctx, int32_t kind, double a0, double a1); /* SH_DCT, SH_FFT: (L1 + a0 I)^-1; CGL_DST: (a0 I + a1 Lap)^-1 */

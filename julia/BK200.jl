@@ -156,6 +156,30 @@ function d3F(c::Context, u, params, dx1, dx2, dx3)
     out
 end
 
+"""The contractions ⟨v_i, d2F(u)[v_j, v_k]⟩ for the rows (i, j, k) of idx2, then ⟨v_i, d3F(u)[v_j, v_k, v_l]⟩ for the rows of
+idx3 (1-based indices into vecs), that get_normal_formNd (src/NormalForms.jl:656-896) makes, in one pass over the vectors on the
+device (bk_jet_moments).  At most 64 vectors; longer tuple lists are split into calls of at most 8192 tuples."""
+function jet_moments(c::Context, u, params, vecs, idx2::AbstractMatrix{<:Integer}, idx3::AbstractMatrix{<:Integer})
+    setparams!(c, params)
+    pv = Ptr{Float64}[ptr(v) for v in vecs]
+    i2 = Int32.(permutedims(idx2 .- 1))   # row-major tuples, 0-based
+    i3 = Int32.(permutedims(idx3 .- 1))
+    n2, n3 = size(idx2, 1), size(idx3, 1)
+    out = zeros(n2 + n3)
+    t0 = 0
+    while t0 < n2 + n3
+        t1 = min(t0 + 8192, n2 + n3)
+        a2 = (min(t0, n2), min(t1, n2))
+        a3 = (max(t0 - n2, 0), max(t1 - n2, 0))
+        check(c, ccall((:bk_jet_moments, lib), Int32,
+                       (Ptr{Cvoid}, Ptr{Float64}, Int32, Ptr{Ptr{Float64}}, Int32, Ptr{Int32}, Int32, Ptr{Int32}, Ptr{Float64}),
+                       c.handle, ptr(u), length(pv), pv, a2[2] - a2[1], pointer(i2, 3 * a2[1] + 1), a3[2] - a3[1],
+                       pointer(i3, 4 * a3[1] + 1), pointer(out, t0 + 1)))
+        t0 = t1
+    end
+    out
+end
+
 """updatesection!(trap, x, pars) (PeriodicOrbitTrapeze.jl:665-679) on a BK_POTRAP_CGL2D context: ϕ_i = scale F(x_i), xπ = x[1:end-1]
 (bk_potrap_update_section).  scale = 1/M for updatesection!, 1 for the orbit form of re_make (:1077-1080).  Not executed here."""
 function update_section!(c::Context, x, params, scale)
