@@ -4,7 +4,8 @@ continuation.  The directory name carries a dot (bifurcationkit.jl_b200), so imp
 
 Contents: csrc/ (CUDA kernels + C ABI -> libbk200.so), lib.py (ctypes binding), core.py (mirror of
 the reference's AbstractLinearSolver / AbstractBorderedLinearSolver / AbstractEigenSolver surfaces),
-palc.py (host-side Newton / newton_palc / continuation loop driving the device kernels), periodic.py (periodic-orbit
+palc.py (host-side Newton / newton_palc / continuation loop driving the device kernels), defcont.py (deflated
+continuation), periodic.py (periodic-orbit
 branches with the Trapeze functional and branch switching to them from a Hopf point).
 """
 from . import lib
@@ -17,6 +18,7 @@ from . import segments
 from . import floquet
 from . import events
 from . import deflation
+from . import defcont
 from . import codim2
 from . import normalform
 from . import periodic

@@ -217,6 +217,30 @@ class Context:
                                                a3.ctypes.data_as(ip), o.ctypes.data_as(C.POINTER(C.c_double))))
         return out
 
+    def deflation_moments(self, u, roots, dirs=(), n=None):
+        """The deflation scalars over the first n entries (all N0 by default), in one pass over u, the directions and the roots
+        (bk_deflation_moments): (s, m, t, q) with s[i] = <u - r_i, u - r_i>, m[i] = max |u - r_i|, t[i, a] = <u - r_i, h_a> and
+        q[a, b] = <h_a, h_b> for at most two directions h_a.  Host or device vectors.  Lists longer than BK_DEFLATION_MAX_ROOTS
+        are split into several calls; a root's values do not depend on the split."""
+        nd, n = len(dirs), self.N0 if n is None else int(n)
+        W, cap = 2 + nd, _l.BK_DEFLATION_MAX_ROOTS
+        s, m, t = np.zeros(len(roots)), np.zeros(len(roots)), np.zeros((len(roots), nd))
+        q = np.zeros((nd, nd))
+        pd = (C.c_void_p * max(nd, 1))(*[_l.ptr(h) for h in dirs])
+        for r0 in range(0, max(len(roots), 1), cap):
+            rs = roots[r0:r0 + cap]
+            out = np.zeros(len(rs) * W + nd * (nd + 1) // 2)
+            pv = (C.c_void_p * max(len(rs), 1))(*[_l.ptr(r) for r in rs])
+            _chk(self, self.lib.bk_deflation_moments(self.handle, _l.ptr(u), len(rs), pv, nd, pd if nd else None, n,
+                                                     out.ctypes.data_as(C.POINTER(C.c_double))))
+            blk = out[:len(rs) * W].reshape(len(rs), W)
+            s[r0:r0 + len(rs)], m[r0:r0 + len(rs)], t[r0:r0 + len(rs)] = blk[:, 0], blk[:, 1], blk[:, 2:]
+            qv = out[len(rs) * W:]
+        if nd:
+            q[np.triu_indices(nd)] = qv
+            q[np.tril_indices(nd, -1)] = q.T[np.tril_indices(nd, -1)]
+        return s, m, t, q
+
     def precond_setup(self, kind, a0=1.0, a1=1.0):
         _chk(self, self.lib.bk_precond_setup(self.handle, kind, a0, a1))
 

@@ -206,6 +206,7 @@ struct bk_ctx {
   size_t mom_stage_cap = 0;  // bytes
   void* mom_work = nullptr;
   size_t mom_work_cap = 0;   // bytes
+  double* defl_pinned = nullptr;  // bk_deflation_moments: pinned landing buffer of the results (lazily allocated)
   // bk_vec_alloc pool: live allocations (ptr -> padded length) and the recycled free list
   std::unordered_map<double*, size_t> vec_live;
   std::vector<std::pair<size_t, double*>> vec_pool;

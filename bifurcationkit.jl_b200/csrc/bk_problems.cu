@@ -5,6 +5,8 @@
 //   P3 examples/SH3d.jl:16-53             P4 examples/cGL2d.jl:6-22,262-318
 //   P5 src/periodicorbit/PeriodicOrbitTrapeze.jl:209-330,362-386
 //   bordered map src/LinearBorderSolver.jl:299-335
+#include <cstring>
+
 #include "bk_common.cuh"
 #include "bk_stencil.cuh"
 #include "bk_krylov_tma.cuh"
@@ -390,6 +392,118 @@ static __global__ void __launch_bounds__(256) k_jet_moments_fold(const double* _
   }
 }
 
+// ------------------------------------------------------------------------------------------ deflation moments
+// Per root r_i: s_i = <d, d>, m_i = max |d|, t_{i,a} = <d, h_a> with d = u - r_i, and q_ab = <h_a, h_b>, in one pass (bk200.h).
+// A tile is 256 x BK_DEFL_PPT points, thread t owning points t, t + 256, ..; the CTAs of the grid (bk_reduce_grid of the tiles'
+// thread count) take the tiles in a grid-stride loop.  Per tile a thread keeps its points of u and of the directions in
+// registers and takes the roots in batches of BK_DEFL_RB: all the batch's loads are issued before the sums.  Each value is
+// folded over the warp (xor-shuffle tree) and added, in tile order, to that warp's own accumulator in shared memory, so the tile
+// loop has no barrier; after it, the 8 warps' accumulators are folded in warp order into partials[k * G + blockIdx.x], and
+// k_deflation_moments_fold folds those in CTA order.  A root's arithmetic is the same whichever batch slot it has, so its
+// outputs depend on n only.
+#define BK_DEFL_PPT 4
+#define BK_DEFL_RB 4
+struct DeflVecs {
+  const double* r[BK_DEFLATION_MAX_ROOTS];
+  const double* h[2];
+  const double* u;
+};
+// acc[k] += (or max=, for the m columns: k % W == 1 with W > 0) the warp total of v[k], for k < live (uniform over the warp)
+template <int K, int W>
+__device__ __forceinline__ void defl_warp_add(const double (&v)[K], int live, double* acc) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    if (k < live) {
+      const bool mx = W > 0 && k % W == 1;
+      const double t = mx ? bk_warp_max(v[k]) : bk_warp_sum(v[k]);
+      if (lane == 0) acc[k] = mx ? bk_nanmax(acc[k], t) : acc[k] + t;
+    }
+  }
+}
+template <int NDIR>
+static __global__ void __launch_bounds__(256) k_deflation_moments(DeflVecs vs, int nroots, long long n,
+                                                                  double* __restrict__ partials) {
+  bk_pdl_sync();
+  constexpr int W = 2 + NDIR, NQ = NDIR * (NDIR + 1) / 2, TP = 256 * BK_DEFL_PPT, LDA = BK_DEFLATION_MAX_ROOTS * W + 3;
+  __shared__ double s_acc[8 * LDA];  // one row of accumulators per warp
+  const int ncol = nroots * W + NQ;
+  for (int k = threadIdx.x; k < 8 * LDA; k += blockDim.x) s_acc[k] = 0.0;
+  __syncthreads();
+  double* acc = s_acc + (threadIdx.x >> 5) * LDA;
+  const long long ntiles = (n + TP - 1) / TP;
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    long long idx[BK_DEFL_PPT];
+    double u[BK_DEFL_PPT], h[2][BK_DEFL_PPT];
+#pragma unroll
+    for (int p = 0; p < BK_DEFL_PPT; ++p) {
+      idx[p] = tile * TP + threadIdx.x + 256 * p;
+      const bool in = idx[p] < n;
+      u[p] = in ? vs.u[idx[p]] : 0.0;
+#pragma unroll
+      for (int a = 0; a < 2; ++a) h[a][p] = in && a < NDIR ? vs.h[a][idx[p]] : 0.0;
+    }
+    if constexpr (NQ > 0) {
+      double q[3] = {0.0, 0.0, 0.0};
+#pragma unroll
+      for (int p = 0; p < BK_DEFL_PPT; ++p) {
+        q[0] = fma(h[0][p], h[0][p], q[0]);
+        q[1] = fma(h[0][p], h[1][p], q[1]);
+        q[2] = fma(h[1][p], h[1][p], q[2]);
+      }
+      defl_warp_add<3, 0>(q, NQ, acc + nroots * W);
+    }
+    for (int r0 = 0; r0 < nroots; r0 += BK_DEFL_RB) {
+      const int live = nroots - r0 < BK_DEFL_RB ? nroots - r0 : BK_DEFL_RB;
+      double x[BK_DEFL_RB][BK_DEFL_PPT];
+#pragma unroll
+      for (int j = 0; j < BK_DEFL_RB; ++j)
+#pragma unroll
+        for (int p = 0; p < BK_DEFL_PPT; ++p) x[j][p] = j < live && idx[p] < n ? vs.r[r0 + j][idx[p]] : u[p];
+      double v[BK_DEFL_RB * W];
+#pragma unroll
+      for (int j = 0; j < BK_DEFL_RB; ++j) {
+        double s = 0.0, m = 0.0, t[2] = {0.0, 0.0};
+#pragma unroll
+        for (int p = 0; p < BK_DEFL_PPT; ++p) {
+          const double d = u[p] - x[j][p];
+          s = fma(d, d, s);
+          m = bk_nanmax(m, fabs(d));
+#pragma unroll
+          for (int a = 0; a < NDIR; ++a) t[a] = fma(d, h[a][p], t[a]);
+        }
+        v[j * W] = s;
+        v[j * W + 1] = m;
+#pragma unroll
+        for (int a = 0; a < NDIR; ++a) v[j * W + 2 + a] = t[a];
+      }
+      defl_warp_add<BK_DEFL_RB * W, W>(v, live * W, acc + r0 * W);
+    }
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < ncol; k += blockDim.x) {
+    const bool mx = k < nroots * W && k % W == 1;
+    double t = 0.0;
+    for (int w = 0; w < 8; ++w) t = mx ? bk_nanmax(t, s_acc[w * LDA + k]) : t + s_acc[w * LDA + k];
+    partials[(size_t)k * gridDim.x + blockIdx.x] = t;
+  }
+}
+// out[k] = the fold of the G partials of column k in a fixed order: one warp per column, lane l taking the CTAs l, l + 32, ..
+// in order, then the xor-shuffle tree; max for the m columns (k < nmom, k % W == 1), sums otherwise
+static __global__ void __launch_bounds__(256) k_deflation_moments_fold(const double* __restrict__ partials, int ncol, int nmom,
+                                                                       int W, int G, double* __restrict__ out) {
+  const int k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (k >= ncol) return;  // uniform over the warp
+  const bool mx = k < nmom && k % W == 1;
+  double s = 0.0;
+  for (int b = lane; b < G; b += 32) {
+    const double x = partials[(size_t)k * G + b];
+    s = mx ? bk_nanmax(s, x) : s + x;
+  }
+  s = mx ? bk_warp_max(s) : bk_warp_sum(s);
+  if (lane == 0) out[k] = s;
+}
+
 // ------------------------------------------------------------------------------------------ tail reductions
 // Bordered map with NB = 1 or 2 borders (MatrixFreeBLSmap, src/LinearBorderSolver.jl:299-335; tuple form :338-389), one pass
 // after the operator has written out.u = Op(s x.u):   xp = s x.p,
@@ -767,6 +881,53 @@ extern "C" int32_t bk_jet_moments(bk_ctx* c, const double* u, int32_t nvec, cons
   BK_CUDA(c, cudaMemcpyAsync(out, dres, 8 * (size_t)ntup, cudaMemcpyDeviceToHost, c->stream));
   BK_CUDA(c, cudaStreamSynchronize(c->stream));
   c->stats.d2h_bytes += 8 * ntup;
+  return BK_OK;
+}
+
+extern "C" int32_t bk_deflation_moments(bk_ctx* c, const double* u, int32_t nroots, const double* const* roots, int32_t ndir,
+                                        const double* const* dirs, int64_t n, double* out) {
+  BK_ENTER(c);
+  BkRange nvtx_range("bk_deflation_moments");
+  BK_CHECK(c, !c->cplx, "bk_deflation_moments: not available in a BK_COMPLEX context");
+  BK_CHECK(c, nroots >= 1 && nroots <= BK_DEFLATION_MAX_ROOTS, "bk_deflation_moments: nroots out of range");
+  BK_CHECK(c, ndir >= 0 && ndir <= 2, "bk_deflation_moments: ndir out of range");
+  BK_CHECK(c, n >= 1 && n <= c->N0, "bk_deflation_moments: n out of range");
+  BK_CHECK(c, u && roots && out && (ndir == 0 || dirs), "null argument");
+  for (int i = 0; i < nroots; ++i) BK_CHECK(c, roots[i] != nullptr, "null root");
+  for (int a = 0; a < ndir; ++a) BK_CHECK(c, dirs[a] != nullptr, "null direction");
+  // host vectors are staged into rows of n doubles of the per-context buffer bk_jet_moments also uses
+  DeflVecs vs = {};
+  const int nvec = nroots + ndir + 1;
+  for (int i = 0; i < nvec; ++i) {
+    const double* p = i < nroots ? roots[i] : (i < nroots + ndir ? dirs[i - nroots] : u);
+    if (!bk_is_device_ptr(p)) {
+      BK_TRY(grow(c, (void**)&c->mom_stage, &c->mom_stage_cap, 8 * (size_t)n * nvec));
+      double* row = c->mom_stage + (size_t)n * i;
+      BK_CUDA(c, cudaMemcpyAsync(row, p, 8 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
+      c->stats.h2d_bytes += 8 * n;
+      p = row;
+    }
+    if (i < nroots) vs.r[i] = p;
+    else if (i < nroots + ndir) vs.h[i - nroots] = p;
+    else vs.u = p;
+  }
+  const int W = 2 + ndir, ncol = nroots * W + ndir * (ndir + 1) / 2;
+  const int G = bk_reduce_grid(c, (n + BK_DEFL_PPT - 1) / BK_DEFL_PPT);
+  const size_t part_off = (8 * (size_t)ncol + 255) / 256 * 256;
+  BK_TRY(grow(c, &c->mom_work, &c->mom_work_cap, part_off + 8 * (size_t)ncol * G));
+  double* dres = (double*)c->mom_work;
+  double* dpart = (double*)((char*)c->mom_work + part_off);
+  if (ndir == 0) BK_TRY(bk_launch(c, k_deflation_moments<0>, G, 256, 0, vs, (int)nroots, (long long)n, dpart));
+  else if (ndir == 1) BK_TRY(bk_launch(c, k_deflation_moments<1>, G, 256, 0, vs, (int)nroots, (long long)n, dpart));
+  else BK_TRY(bk_launch(c, k_deflation_moments<2>, G, 256, 0, vs, (int)nroots, (long long)n, dpart));
+  BK_TRY(bk_launch_ordered(c, k_deflation_moments_fold, (32 * ncol + 255) / 256, 256, 0, (const double*)dpart, ncol, nroots * W, W,
+                           G, dres));
+  if (!c->defl_pinned)
+    BK_CUDA(c, cudaMallocHost((void**)&c->defl_pinned, 8 * (size_t)(BK_DEFLATION_MAX_ROOTS * 4 + 3)));
+  BK_CUDA(c, cudaMemcpyAsync(c->defl_pinned, dres, 8 * (size_t)ncol, cudaMemcpyDeviceToHost, c->stream));
+  BK_CUDA(c, cudaStreamSynchronize(c->stream));
+  memcpy(out, c->defl_pinned, 8 * (size_t)ncol);
+  c->stats.d2h_bytes += 8 * ncol;
   return BK_OK;
 }
 

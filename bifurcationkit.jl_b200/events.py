@@ -201,6 +201,13 @@ class Branch:
     state: object = None
 
 
+def branch_row(prob, cp, st):
+    """get_state_summary (src/Continuation.jl:259-272): the row a branch keeps for the state st"""
+    stable, _, _ = is_stable(cp, st.eigvals)
+    return dict(param=st.z_p, x=prob.record(st.z_u), itnewton=st.itnewton, itlinear=st.itlinear, ds=st.ds, step=st.step,
+                n_unstable=st.n_unstable[0], n_imag=st.n_imag[0], stable=stable)
+
+
 def continuation(prob, alg, contpar, normC=V.norm2, verbose=False, callback=None, floquet=False, u1=None, p1=None):
     """continuation(prob, PALC(...), ContinuationPar(detect_bifurcation = 0..3)) with special points
     (src/Continuation.jl:349-400 start-up, :506-575 loop): the loop of palc.continuation with the detection before each
@@ -214,9 +221,7 @@ def continuation(prob, alg, contpar, normC=V.norm2, verbose=False, callback=None
     br = Branch(state=st)
 
     def save():
-        stable, _, _ = is_stable(cp, st.eigvals)
-        br.rows.append(dict(param=st.z_p, x=prob.record(st.z_u), itnewton=st.itnewton, itlinear=st.itlinear, ds=st.ds,
-                            step=st.step, n_unstable=st.n_unstable[0], n_imag=st.n_imag[0], stable=stable))
+        br.rows.append(branch_row(prob, cp, st))
         if st.eigvals is not None:
             br.eig.append(dict(eigenvals=np.array(st.eigvals), step=st.step))
             if cp.save_eigenvectors and st.eigvecs is not None:

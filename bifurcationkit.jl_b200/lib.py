@@ -18,13 +18,14 @@ BK_PC_NONE, BK_PC_SH_DCT, BK_PC_CHAN_TRIDIAG, BK_PC_CGL_DST, BK_PC_POTRAP_CIRC, 
 BK_SIDE_NONE, BK_SIDE_LEFT, BK_SIDE_RIGHT = 0, 1, 2
 BK_ORTH_CGS, BK_ORTH_CGS2 = 0, 1
 BK_JET_MOMENTS_MAX_VEC, BK_JET_MOMENTS_MAX_TUPLES = 64, 8192   # the caps of bk_jet_moments (include/bk200.h)
+BK_DEFLATION_MAX_ROOTS = 64   # the cap of bk_deflation_moments
 
 SYMBOLS = [
     "bk_ctx_create", "bk_ctx_destroy", "bk_last_error", "bk_problem_size", "bk_state_size", "bk_set_params", "bk_get_stats",
     "bk_set_timing", "bk_sync", "bk_stream",
     "bk_vec_alloc", "bk_vec_free", "bk_host_alloc", "bk_host_free", "bk_vec_upload", "bk_vec_download", "bk_vec_copy", "bk_vec_zero", "bk_vec_scale",
     "bk_vec_axpby", "bk_vec_dot", "bk_vec_norm2", "bk_vec_norminf", "bk_vec_diffdot",
-    "bk_residual", "bk_jac_set_state", "bk_jvp", "bk_jac_set_shift_imag", "bk_jac_set_transpose", "bk_d2f", "bk_d3f", "bk_jet_moments", "bk_precond_setup", "bk_precond_apply",
+    "bk_residual", "bk_jac_set_state", "bk_jvp", "bk_jac_set_shift_imag", "bk_jac_set_transpose", "bk_d2f", "bk_d3f", "bk_jet_moments", "bk_deflation_moments", "bk_precond_setup", "bk_precond_apply",
     "bk_gmres", "bk_gmres2", "bk_bls_bordering", "bk_bls_matrixfree", "bk_bls_map",
     "bk_bls_block_bordering", "bk_bls_block_matrixfree", "bk_bls_block_map",
     "bk_eigs_shift_invert", "bk_potrap_set_section", "bk_potrap_update_section", "bk_hessenberg_eig", "bk_palc_run",
@@ -120,6 +121,7 @@ def load():
         "bk_d2f": [C.c_void_p, vp, vp, vp, vp],
         "bk_d3f": [C.c_void_p, vp, vp, vp, vp, vp],
         "bk_jet_moments": [C.c_void_p, vp, i32, C.POINTER(vp), i32, C.POINTER(i32), i32, C.POINTER(i32), dp],
+        "bk_deflation_moments": [C.c_void_p, vp, i32, C.POINTER(vp), i32, C.POINTER(vp), i64, dp],
         "bk_precond_setup": [C.c_void_p, i32, dbl, dbl],
         "bk_precond_apply": [C.c_void_p, vp, vp],
         "bk_gmres": [C.c_void_p, vp, vp, dbl, dbl, C.POINTER(GmresOpts), C.POINTER(i32), C.POINTER(i32), dp],

@@ -733,15 +733,8 @@ class _ReducedProblem:
 
 
 def _newton_deflated(prob, x0, p, defop, opts, normN):
-    """deflation.newton_deflated, with a diverging run (iterates beyond float range, where the reference's cbMaxNorm(1e100)
-    stops) or an iterate exactly on a deflated root (M(u) = 1 / 0, an infinite residual in the reference) returned as a failed
-    solve from the guess"""
-    from .deflation import newton_deflated
-    from .palc import NonLinearSolution
-    try:
-        return newton_deflated(prob, x0, p, defop, opts, normN)
-    except (ZeroDivisionError, OverflowError):
-        return NonLinearSolution(V.copy(x0), p, [math.inf], False, 0, 0)
+    from .deflation import newton_deflated_or_fail
+    return newton_deflated_or_fail(prob, x0, p, defop, opts, normN)
 
 
 def predictor_nd(bp, dp, rng=None, ampfactor=1.0, nbfailures=50, maxiter=100, igs=None, amp_igs=1.0, normN=None,

@@ -221,14 +221,36 @@ class NonLinearSolution:
     itlineartot: int
 
 
-def newton(prob, x0, p, opts, normN=V.norm2):
-    """src/Newton.jl:66-114"""
+@dataclass
+class NewtonState:
+    """what a Newton callback sees (src/Newton.jl:87,108)"""
+    x: object
+    fx: object
+    residual: float
+    step: int
+    residuals: list
+
+
+class cbMaxNorm:
+    """cbMaxNorm(maxres) (src/Newton.jl:156-159): stop Newton, unconverged, once a residual reaches maxres"""
+
+    def __init__(self, maxres):
+        self.maxres = maxres
+
+    def __call__(self, state):
+        return state.residual < self.maxres
+
+
+def newton(prob, x0, p, opts, normN=V.norm2, callback=None):
+    """src/Newton.jl:66-114.  `callback(NewtonState)` is asked before the first step and after each one; False stops the
+    iteration and marks the result unconverged (:87,108,111).  None, the default, is the reference's cb_default."""
     x = V.copy(x0)
     fx = prob.F(x, p)
     res = normN(fx)
     residuals = [res]
     step = itlin = 0
-    while step < opts.max_iterations and res > opts.tol:
+    go = callback is None or callback(NewtonState(x, fx, res, step, residuals))
+    while step < opts.max_iterations and res > opts.tol and go:
         J = prob.J(x, p)
         u, cv, it = opts.linsolver(J, fx)
         itlin += int(np.sum(it))
@@ -237,7 +259,9 @@ def newton(prob, x0, p, opts, normN=V.norm2):
         res = normN(fx)
         residuals.append(res)
         step += 1
-    return NonLinearSolution(x, p, residuals, residuals[-1] < opts.tol, step, itlin)
+        go = callback is None or callback(NewtonState(x, fx, res, step, residuals))
+    ok = residuals[-1] < opts.tol and (callback is None or callback(NewtonState(x, fx, res, step, residuals)))
+    return NonLinearSolution(x, p, residuals, ok, step, itlin)
 
 
 def _dot_theta(u1, u2, p1, p2, theta):
@@ -371,8 +395,9 @@ class ContIterable:
     advances a state by one step; `correct`, `accept` and `advance` are the parts of that step a caller choosing its own step
     sizes (segments.continuation_speculative) runs itself."""
 
-    def __init__(self, prob, alg, contpar, normC=V.norm2):
+    def __init__(self, prob, alg, contpar, normC=V.norm2, callback_newton=None):
         self.prob, self.alg, self.contpar, self.normC = prob, alg, contpar, normC
+        self.callback_newton = callback_newton   # the Newton solves of the start-up (palc.newton's callback)
 
     def start(self, u1=None, p1=None):
         """start-up (src/Continuation.jl:349-405): z0 by Newton from prob.u0, z1 by Newton at p0 + ds / eta -- or the given
@@ -382,11 +407,11 @@ class ContIterable:
         p0 = prob.p0
         if u1 is None:
             assert cp.p_min <= p0 <= cp.p_max
-            sol0 = newton(prob, prob.u0, p0, cp.newton_options, self.normC)
+            sol0 = newton(prob, prob.u0, p0, cp.newton_options, self.normC, self.callback_newton)
             if not sol0.converged:
                 raise RuntimeError(f"Newton failed to converge for the initial guess: {sol0.residuals}")
             p1 = p0 + cp.ds / cp.eta
-            sol1 = newton(prob, sol0.u, p1, cp.newton_options, self.normC)
+            sol1 = newton(prob, sol0.u, p1, cp.newton_options, self.normC, self.callback_newton)
             if not sol1.converged:
                 raise RuntimeError("Newton failed to converge for the initial tangent")
             u0, u1 = sol0.u, sol1.u

@@ -168,6 +168,21 @@ int32_t bk_d3f(bk_ctx* ctx, const double* u, const double* dx1, const double* dx
 #define BK_JET_MOMENTS_MAX_TUPLES 8192
 int32_t bk_jet_moments(bk_ctx* ctx, const double* u, int32_t nvec, const double* const* vecs, int32_t n2, const int32_t* idx2,
                        int32_t n3, const int32_t* idx3, double* out);
+/* The scalars of a deflation operator and of its derivative along up to two directions (DeflationOperator, src/
+ * DeflationOperator.jl:122-167; the distance checks of deflated continuation, src/DeflatedContinuation.jl:281-284,334), in one
+ * pass over u, the directions and the roots (host or device pointers).  For each root r_i (i < nroots) over the first n entries:
+ *   s_i = <u - r_i, u - r_i>,  m_i = max |u - r_i|,  t_{i,a} = <u - r_i, h_a>   (a < ndir),
+ * and q_{ab} = <h_a, h_b> (a <= b < ndir).  out (host) holds, with W = 2 + ndir, s_i at out[W i], m_i at out[W i + 1], t_{i,a} at
+ * out[W i + 2 + a], then q_00 (ndir >= 1), q_01 and q_11 (ndir = 2) from out[W nroots]: nroots W + ndir (ndir + 1) / 2 doubles.
+ * The difference u - r_i is formed point by point (no expansion into <u,u> - 2<u,r> + <r,r>, which cancels near a root).  The
+ * sums run in an order fixed by n alone: host or device inputs give the same bits, and a root's outputs do not depend on the
+ * other roots of the call or on ndir, so a long list may be split into several calls.  m_i is NaN if an entry of u - r_i is.
+ * n < context length takes a prefix (the period of a periodic orbit left out of the distance, examples/cGL2d.jl:192).
+ * BK_ERR_ARG before any launch: nroots outside [1, BK_DEFLATION_MAX_ROOTS], ndir outside [0, 2], n outside [1, N0], a null
+ * pointer, a BK_COMPLEX context. */
+#define BK_DEFLATION_MAX_ROOTS 64
+int32_t bk_deflation_moments(bk_ctx* ctx, const double* u, int32_t nroots, const double* const* roots, int32_t ndir,
+                             const double* const* dirs, int64_t n, double* out);
 
 /* ---- K6: preconditioner --------------------------------------------------------------------- */
 int32_t bk_precond_setup(bk_ctx* ctx, int32_t kind, double a0, double a1); /* SH_DCT, SH_FFT: (L1 + a0 I)^-1; CGL_DST: (a0 I + a1 Lap)^-1 */

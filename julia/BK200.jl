@@ -180,6 +180,35 @@ function jet_moments(c::Context, u, params, vecs, idx2::AbstractMatrix{<:Integer
     out
 end
 
+"""The deflation scalars for up to 64 roots over the first n entries, in one pass (bk_deflation_moments): s[i] = ⟨u - rᵢ, u - rᵢ⟩,
+m[i] = max|u - rᵢ|, t[i, a] = ⟨u - rᵢ, hₐ⟩ and q[a, b] = ⟨hₐ, h_b⟩ for at most two directions — what DeflationOperator
+(src/DeflationOperator.jl:122-167) and the distance checks of DefCont (src/DeflatedContinuation.jl:281-284,334) need.  Longer
+root lists are split into calls of 64.  Not executed here."""
+function deflation_moments(c::Context, u, roots, dirs = (); n = length(u))
+    nd = length(dirs)
+    pd = Ptr{Float64}[ptr(h) for h in dirs]
+    s, m, t = zeros(length(roots)), zeros(length(roots)), zeros(length(roots), nd)
+    q = zeros(nd, nd)
+    for r0 in 1:64:length(roots)
+        rs = roots[r0:min(r0 + 63, end)]
+        pv = Ptr{Float64}[ptr(r) for r in rs]
+        out = zeros(length(rs) * (2 + nd) + nd * (nd + 1) ÷ 2)
+        check(c, ccall((:bk_deflation_moments, lib), Int32,
+                       (Ptr{Cvoid}, Ptr{Float64}, Int32, Ptr{Ptr{Float64}}, Int32, Ptr{Ptr{Float64}}, Int64, Ptr{Float64}),
+                       c.handle, ptr(u), length(pv), pv, nd, nd == 0 ? C_NULL : pd, n, out))
+        blk = permutedims(reshape(out[1:length(rs) * (2 + nd)], 2 + nd, length(rs)))
+        s[r0:r0 + length(rs) - 1] .= blk[:, 1]
+        m[r0:r0 + length(rs) - 1] .= blk[:, 2]
+        t[r0:r0 + length(rs) - 1, :] .= blk[:, 3:end]
+        k = length(rs) * (2 + nd)
+        for a in 1:nd, b in a:nd
+            k += 1
+            q[a, b] = q[b, a] = out[k]
+        end
+    end
+    s, m, t, q
+end
+
 """updatesection!(trap, x, pars) (PeriodicOrbitTrapeze.jl:665-679) on a BK_POTRAP_CGL2D context: ϕ_i = scale F(x_i), xπ = x[1:end-1]
 (bk_potrap_update_section).  scale = 1/M for updatesection!, 1 for the orbit form of re_make (:1077-1080).  Not executed here."""
 function update_section!(c::Context, x, params, scale)
