@@ -5,7 +5,9 @@ Mirror of src/codim2/MinAugFold.jl:
   FoldMinAug.residual      <->  (F::FoldMinimallyAugmentedFormulation)(x, p, params)            :15-39
   FoldMinAug.bordered_terms <-> _compute_bordered_vectors / _get_bordered_terms                   :55-104
   FoldMinAug.solve         <->  foldMALinearSolver, finite-difference branch (usehessian = false) :122-146
+  FoldMinAug.update        <->  update!(probma, iter, state), test_bt_cusp                        :276-309, 551-575
   newton_fold              <->  newton_fold(prob, foldpointguess, par, eigenvec, eigenvec_ad, options; bdlinsolver)  :201-222
+  MAProblem, MALinearSolver <-> FoldMAProblem, FoldLinearSolverMinAug                              :148-163
 Swift-Hohenberg is self-adjoint (is_symmetric = true, examples/SH3d.jl:123), so J' = J and no adjoint kernel is needed (for
 the Chan problem J' = J only up to the two boundary rows: the left null vector, hence sigma_x and sigma_p, are then approximate
 and Newton on the MA system degrades to a quasi-Newton iteration that still converges to the same fold).
@@ -14,7 +16,9 @@ Mirror of src/codim2/MinAugHopf.jl:
   HopfMinAug.residual       <->  (H::HopfMinimallyAugmentedFormulation)(x, p, omega, params)      :19-40
   HopfMinAug.bordered_terms <->  __compute_bordered_vectors / _get_bordered_terms                 :59-104
   HopfMinAug.solve          <->  _hopf_MA_linear_solver, finite-difference branch                 :122-188
+  HopfMinAug.update         <->  update!(probma, iter, state)                                     :323-367
   newton_hopf               <->  newton_hopf(prob, hopfpointguess, par, eigenvec, eigenvec_ad, options)  :258-283
+  MAProblem, MALinearSolver <->  HopfMAProblem, HopfLinearSolverMinAug                            :190-205
 The complex shifts (J - i omega, (J - i omega)^H = J' + i omega) are solved on a BK_COMPLEX context (include/bk200.h): split
 complex vectors, GMRES on the real-equivalent system, J' from bk_jac_set_transpose.  The complex bordered systems
 [A a; b^H 0] are eliminated by bordering on the host (one complex solve each, since their right-hand side is (0, 1));
@@ -47,9 +51,15 @@ class FoldSolution:
 class FoldMinAug:
     """[F(x, p); sigma(x, p)] with sigma from  [J a; b' 0] [v; sigma] = [0; 1]  (Govaerts 2000: a ~ left, b ~ right null vector)."""
 
+    # the MA state's BorderedVec.p <-> the scalar unknowns (p1,), and the residual's (sigma,) or a solve's (dp,) -> BorderedVec.p
+    unpack = staticmethod(lambda zp: (zp,))
+    pack = staticmethod(lambda sigma: sigma)
+    copy_rhs = False   # MALinearSolver hands solve() the right-hand side itself
+
     def __init__(self, prob, a, b, bls, symmetric=True, norm=V.norm2):
         assert symmetric or hasattr(prob, "Jt"), "non-symmetric problem: prob.Jt(x, p) (jacobian_adjoint) is required"
         self.prob, self.a, self.b, self.bls, self.symmetric, self.norm = prob, V.copy(a), V.copy(b), bls, symmetric, norm
+        self.problems = (prob,)      # the problems whose params[lens2] a curve sets
         self.zero = V.zeros_like(a)
         self.itlinear = 0
         self.BT, self.CP = 1.0, 1.0  # test functions of the Bogdanov-Takens / cusp events (MinAugFold.jl:421-423, 551-575)
@@ -122,27 +132,32 @@ class FoldMinAug:
         return self.BT
 
 
+def _newton_ma(ma, x0, q0, opts, resnorm):
+    """src/Newton.jl:66-114 on the MA system of `ma` in the state (x, q), q = (p,) or (p, omega): ma.residual(x, *q) -> (F, *s),
+    ma.solve(x, *q, F, *s) -> (dX, *dq, converged), resnorm(F, *s) -> the residual norm.  Returns (x, q, s, residuals, steps)."""
+    x, q = V.copy(x0), [float(v) for v in q0]
+    F, *s = ma.residual(x, *q)
+    residuals = [resnorm(F, *s)]
+    step = 0
+    while step < opts.max_iterations and residuals[-1] > opts.tol:
+        dX, *dq, _ = ma.solve(x, *q, F, *s)
+        V.axpby(x, -1.0, dX, 1.0)
+        q = [v - d for v, d in zip(q, dq)]
+        F, *s = ma.residual(x, *q)
+        residuals.append(resnorm(F, *s))
+        step += 1
+    return x, q, s, residuals, step
+
+
 def newton_fold(prob, x0, p0, eigenvec, eigenvec_ad, opts, bls, normN=V.norm2, symmetric=True):
     """Newton on the MA system from the guess (x0, p0) with guesses for the right / left null vectors
     (newton_fold, MinAugFold.jl:201-222 + src/Newton.jl:66-114 on the bordered state)."""
     ma = FoldMinAug(prob, eigenvec_ad, eigenvec, bls, symmetric=symmetric)
-    x, p = V.copy(x0), float(p0)
-    F, sigma = ma.residual(x, p)
-    res = math.hypot(normN(F), abs(sigma))
-    residuals = [res]
-    step = 0
-    while step < opts.max_iterations and res > opts.tol:
-        dX, dp, _ = ma.solve(x, p, F, sigma)
-        V.axpby(x, -1.0, dX, 1.0)
-        p -= dp
-        F, sigma = ma.residual(x, p)
-        res = math.hypot(normN(F), abs(sigma))
-        residuals.append(res)
-        step += 1
+    x, (p,), (sigma,), residuals, step = _newton_ma(ma, x0, (p0,), opts, lambda F, sigma: math.hypot(normN(F), abs(sigma)))
     return FoldSolution(x, p, residuals, residuals[-1] < opts.tol, step, ma.itlinear, sigma)
 
 
-# ------------------------------------------------------------------------------------------------ Fold curves in two parameters
+# ------------------------------------------------------------------------------------------------ Fold and Hopf curves in two parameters
 class BorderedVec:
     """BorderedArray(u, p) (src/BorderedArrays.jl:23-70, 86-217) with the method set of a DeviceVec, so that the PALC host
     loop (palc.py) runs on the state of a minimally augmented problem unchanged: (x, p1) for Folds, (x, [p1, omega]) for Hopf
@@ -195,50 +210,54 @@ class BorderedVec:
         return V.diffdot(self.u, x0.u, tau.u) + float(np.sum((self.p - x0.p) * tau.p))
 
 
-class _FoldMAJacobian:
-    """jacobian(FoldMAProblem{MinAug}, z, p2): a handle on (x, p1, p2); the bordered terms are computed once per handle and
-    shared by the right-hand sides BorderingBLS solves with it (the reference recomputes them per right-hand side)."""
+class _MAJacobian:
+    """jacobian(MAProblem, z, p2): a handle on (z, p2).  `terms` keeps what ma.solve may share between the right-hand sides
+    BorderingBLS solves with the handle (FoldMinAug: the bordered terms, which the reference recomputes per right-hand side)."""
 
     def __init__(self, pb, z, p2):
         self.pb, self.z, self.p2, self.terms = pb, z, p2, None
 
 
-class FoldLinearSolverMinAug:
-    """(foldl::FoldLinearSolverMinAug)(Jfold, rhs) -> (sol, converged, iters)   (MinAugFold.jl:148-163)"""
+class MALinearSolver:
+    """(foldl::FoldLinearSolverMinAug)(Jfold, rhs) / (hopfl::HopfLinearSolverMinAug)(Jhopf, rhs) -> (sol, converged, iters)
+    (MinAugFold.jl:148-163, MinAugHopf.jl:190-205): ma.solve on the unpacked state and right-hand side."""
 
     def __call__(self, Jma, rhs):
         pb, ma = Jma.pb, Jma.pb.ma
         pb._set2(Jma.p2)
         it0 = ma.itlinear
-        dX, dp, cv = ma.solve(Jma.z.u, Jma.z.p, rhs.u, rhs.p, cache=Jma)
-        return BorderedVec(dX, dp), cv, ma.itlinear - it0
+        rhsu = V.copy(rhs.u) if ma.copy_rhs else rhs.u
+        dX, *dq, cv = ma.solve(Jma.z.u, *ma.unpack(Jma.z.p), rhsu, *ma.unpack(rhs.p), cache=Jma)
+        return BorderedVec(dX, ma.pack(*dq)), cv, ma.itlinear - it0
 
 
-class FoldMAProblem:
-    """FoldMAProblem: the minimally augmented Fold system [F(x, p1, p2); sigma(x, p1, p2)] as a problem in the state
-    z = (x, p1) with continuation parameter p2 = params[lens2] (continuation_fold, MinAugFold.jl:366-452)."""
+class MAProblem:
+    """FoldMAProblem / HopfMAProblem: the minimally augmented system of `ma` ([F; sigma] for a FoldMinAug, [F; Re sigma; Im sigma]
+    for a HopfMinAug) as a problem in the state z = BorderedVec(x, p1) or BorderedVec(x, [p1, omega]) with continuation parameter
+    p2 = params[lens2] (continuation_fold, MinAugFold.jl:366-452; continuation_hopf, MinAugHopf.jl:425-522)."""
 
     def __init__(self, ma, lens2, z0, record=None):
         assert lens2 != ma.prob.lens, "Please choose 2 different parameters."
         self.ma, self.lens2, self.u0 = ma, lens2, z0
         self.p0 = float(ma.prob.params[lens2])
         self.delta = ma.prob.delta
-        self.record = record or (lambda z: z.p)   # record_from_solution of the Fold curve: (p1, p2) -- p2 is the row's param
+        self.record = record or (lambda z: ma.unpack(z.p)[0])   # record_from_solution: p1 -- p2 is the row's param
 
     def _set2(self, p2):
-        self.ma.prob.params[self.lens2] = p2
+        for prob in self.ma.problems:
+            prob.params[self.lens2] = p2
 
     def F(self, z, p2, out=None):
         self._set2(p2)
-        Fu, sigma = self.ma.residual(z.u, z.p)
+        Fu, *s = self.ma.residual(z.u, *self.ma.unpack(z.p))
         if out is None:
-            return BorderedVec(Fu, sigma)
+            return BorderedVec(Fu, self.ma.pack(*s))
         V.copyto(out.u, Fu)
-        out.p = sigma
+        out.p = self.ma.pack(*s)
         return out
 
     def J(self, z, p2):
-        return _FoldMAJacobian(self, z, p2)
+        return _MAJacobian(self, z, p2)
 
 
 class BorderingBLSHost:
@@ -295,6 +314,45 @@ def locate_event(it, _st, values_at, labels, indicator=None):
     return status, interval, (labels[min(changed[0], len(labels) - 1)] if changed else None)
 
 
+def _event(it, st, p2_prev, label, vals, values_at, labels, detect_event, indicator=None):
+    """An event indicator of a codim-2 curve changed between the accepted point at p2_prev and the state `st`, whose test-function
+    values are `vals` (label: the test function that changed).  detect_event = 1: a guess on the interval between the two points;
+    > 1: located by locate_event(it, st, values_at, labels, indicator), after which `st` holds the located state, params[lens2]
+    its p2 and `vals` its values_at.  Returns ((status, interval, label), or None where the bisection did not run; vals)."""
+    from . import events as E
+    if detect_event < 2:
+        return ("guess", tuple(E.getinterval(p2_prev, st.z_p)), label), vals
+    status, interval, lab = locate_event(it, st, values_at, labels, indicator)
+    it.prob._set2(st.z_p)
+    return (None if status == "none" else (status, tuple(interval), lab or label)), values_at(st)
+
+
+def _continue_ma(pb, contpar, alg, normC, point, callback):
+    """PALC on the MA problem `pb` in p2 = params[lens2] (MinAugFold.jl:446-457, MinAugHopf.jl:510-521): Newton linear solver
+    MALinearSolver, outer bordered solver BorderingBLS(MALinearSolver, check_precision = false), no bifurcation detection on the
+    MA system.  After every accepted point, with params[lens2] set to its p2: point(it, st), where False ends the curve, then the
+    user's callback(st).  The parameter lists the curve writes are left as they were.  Returns (rows, state)."""
+    from . import palc as P
+    mls = MALinearSolver()
+    no = contpar.newton_options
+    cp = P.ContinuationPar(**{**contpar.__dict__, "newton_options": P.NewtonPar(tol=no.tol, max_iterations=no.max_iterations, linsolver=mls),
+                              "detect_bifurcation": 0})
+    alg = alg or P.PALC()
+    alg = P.PALC(tangent=alg.tangent, theta=alg.theta, bls=BorderingBLSHost(mls))
+    it = P.ContIterable(pb, alg, cp, normC)
+
+    def cb(st):
+        pb._set2(st.z_p)
+        return point(it, st) is not False and (callback is None or callback(st))
+
+    saved = [prob.params[pb.lens2] for prob in pb.ma.problems]
+    try:
+        return P.continuation(pb, alg, cp, normC=normC, callback=cb, it=it)
+    finally:
+        for prob, p2 in zip(pb.ma.problems, saved):
+            prob.params[pb.lens2] = p2
+
+
 @dataclass
 class FoldCurve:
     rows: list      # palc rows: param = p2, x = record (default p1), itnewton, itlinear, ds, step
@@ -321,7 +379,7 @@ def continuation_fold(prob, x0, p1_0, lens2, eigenvec, eigenvec_ad, contpar, bls
                       update_minaug_every_step=1, record=None, callback=None, detect_event=0, eigsolver=None):
     """Codim-2 continuation of a Fold point in the parameters (p1 = params[prob.lens], p2 = params[lens2]):
     continuation_fold(prob, alg, foldpointguess, par, lens1, lens2, eigenvec, eigenvec_ad, options_cont; jacobian_ma = MinAug())
-    (MinAugFold.jl:366-452).  PALC on the minimally augmented system, Newton linear solver = FoldLinearSolverMinAug over the
+    (MinAugFold.jl:366-452).  PALC on the minimally augmented system, Newton linear solver = MALinearSolver over the
     bordered solver `bls` (bdlinsolver: MatrixFreeBLSB200 / BorderingBLSB200 on the device), outer bordered solver =
     BorderingBLS(that solver, check_precision = false), border vectors updated after every accepted step (update!), the
     Bogdanov-Takens and cusp test functions recorded along the curve.  detect_event = 1: a change of sign of a test function
@@ -329,32 +387,18 @@ def continuation_fold(prob, x0, p1_0, lens2, eigenvec, eigenvec_ad, contpar, bls
     bisection (locate_event) with contpar.n_inversion / max_bisection_steps / dsmin_bisection, and the curve goes on from the
     located state, as in the reference.  eigsolver (J, nev) -> (eigenvalues, ...): eigenvalues of J along the curve (FoldEig, :577-590;
     contpar.nev of them) for the Zero-Hopf event "zh" (DiscreteEvent(1, test_zh), :431; recorded at the point after the change)."""
-    from . import palc as P
-    ma = FoldMinAug(prob, eigenvec_ad, eigenvec, bls, symmetric=symmetric, norm=normC)
-    z0 = BorderedVec(V.copy(x0), p1_0)
-    pb = FoldMAProblem(ma, lens2, z0, record)
-    fls = FoldLinearSolverMinAug()
-    no = contpar.newton_options
-    cp = P.ContinuationPar(**{**contpar.__dict__, "newton_options": P.NewtonPar(tol=no.tol, max_iterations=no.max_iterations, linsolver=fls),
-                              "detect_bifurcation": 0})
-    alg = alg or P.PALC()
-    alg = P.PALC(tangent=alg.tangent, theta=alg.theta, bls=BorderingBLSHost(fls))
-    curve = FoldCurve([], [], [], [], [], ma, None, [])
     from . import events as E
-    it = P.ContIterable(pb, alg, cp, normC)
+    ma = FoldMinAug(prob, eigenvec_ad, eigenvec, bls, symmetric=symmetric, norm=normC)
+    pb = MAProblem(ma, lens2, BorderedVec(V.copy(x0), p1_0), record)
+    curve = FoldCurve([], [], [], [], [], ma, None, [])
     zh_hist = []
 
     def values_at(s):   # test_bt_cusp at a state, the border vectors untouched
         pb._set2(s.z_p)
         return (ma.update(s.z_u.u, s.z_u.p, keep_borders=True), s.tau_p)
 
-    def cb(st):
-        pb._set2(st.z_p)
-        if st.step % update_minaug_every_step == 0:
-            ma.update(st.z_u.u, st.z_u.p)
-        else:
-            ma.update(st.z_u.u, st.z_u.p, keep_borders=True)
-        vals = (ma.BT, st.tau_p)
+    def point(it, st):
+        vals = (ma.update(st.z_u.u, st.z_u.p, keep_borders=st.step % update_minaug_every_step != 0), st.tau_p)
         if eigsolver is not None:
             zh = test_zh(eigsolver(prob.J(st.z_u.u, st.z_u.p), contpar.nev)[0], contpar.tol_stability)
             if detect_event > 0 and zh_hist and st.step > 0 and zh != zh_hist[-1]:
@@ -365,25 +409,16 @@ def continuation_fold(prob, x0, p1_0, lens2, eigenvec, eigenvec_ad, contpar, bls
             prev = (curve.BT[-1], curve.CP[-1])
             flips = [k for k in range(2) if (prev[k] > 0) != (vals[k] > 0)]
             if flips:
-                status, interval, label = "guess", E.getinterval(curve.p2[-1], st.z_p), ("bt", "cusp")[flips[0]]
-                if detect_event > 1:
-                    status, interval, lab = locate_event(it, st, values_at, ("bt", "cusp"))
-                    label = lab or label
-                    pb._set2(st.z_p)
-                    vals = (ma.update(st.z_u.u, st.z_u.p, keep_borders=True), st.tau_p)
-                if status != "none":
-                    curve.specialpoint.append(Codim2Point(label, st.z_p, st.z_u.p, st.step, status, tuple(interval), V.copy(st.z_u.u)))
+                found, vals = _event(it, st, curve.p2[-1], ("bt", "cusp")[flips[0]], vals, values_at, ("bt", "cusp"), detect_event)
+                if found:
+                    status, interval, label = found
+                    curve.specialpoint.append(Codim2Point(label, st.z_p, st.z_u.p, st.step, status, interval, V.copy(st.z_u.u)))
         curve.p1.append(st.z_u.p)
         curve.p2.append(st.z_p)
         curve.BT.append(vals[0])
         curve.CP.append(vals[1])
-        return True if callback is None else callback(st)
 
-    p2_0 = prob.params[lens2]
-    try:
-        curve.rows, curve.state = P.continuation(pb, alg, cp, normC=normC, callback=cb, it=it)
-    finally:
-        prob.params[lens2] = p2_0  # the caller's parameter tuple is left as it was
+    curve.rows, curve.state = _continue_ma(pb, contpar, alg, normC, point, callback)
     return curve
 
 
@@ -431,8 +466,14 @@ class HopfMinAug:
     """[F(x, p); Re sigma; Im sigma](x, p, omega) with  [J - i omega, a; b^H, 0] [v; sigma] = [0; 1]
     (a ~ null vector of (J - i omega)^H, b ~ null vector of J - i omega)."""
 
+    # the MA state's BorderedVec.p <-> (p1, omega), and the residual's (Re sigma, Im sigma) or a solve's (dp, domega) -> BorderedVec.p
+    unpack = staticmethod(lambda zp: (float(zp[0]), float(zp[1])))
+    pack = staticmethod(lambda sr, si: np.array([sr, si]))
+    copy_rhs = True   # MALinearSolver hands solve() a copy of the right-hand side
+
     def __init__(self, prob, cprob, a, b, ls, cls, cbls=None):
         self.prob, self.cprob, self.ls, self.cls, self.cbls = prob, cprob, ls, cls, cbls
+        self.problems = (prob, cprob)   # the problems whose params[lens2] a curve sets
         self.a, self.b = np.array(a, dtype=complex), np.array(b, dtype=complex)
         self.itlinear = 0
 
@@ -466,8 +507,9 @@ class HopfMinAug:
         sigma_om = 1j * np.vdot(w, v)
         return v, w, dpF, sigma_p, sigma_om
 
-    def solve(self, x, p, om, duu, dup, duom):
-        """_hopf_MA_linear_solver: [J dpF 0; sigma_x sigma_p sigma_om] [dX; dp; dom] = [duu; dup; duom]"""
+    def solve(self, x, p, om, duu, dup, duom, cache=None):
+        """_hopf_MA_linear_solver: [J dpF 0; sigma_x sigma_p sigma_om] [dX; dp; dom] = [duu; dup; duom].  `cache` is not used:
+        the bordered terms are computed again for every right-hand side, as in the reference."""
         prob, cprob = self.prob, self.cprob
         eps = prob.delta
         v, w, dpF, sigma_p, sigma_om = self.bordered_terms(x, p, om)
@@ -487,74 +529,24 @@ class HopfMinAug:
         V.axpby(x1, -dp, x2, 1.0)
         return x1, float(dp), float(dom), cv
 
+    def update(self, x, p, om):
+        """update!(probma, iter, state) (MinAugHopf.jl:323-367): after an accepted step the border vectors follow the null
+        vectors, a <- w / ||w||inf, b <- v / ||v||inf."""
+        v, _ = self._border(self.cprob.J(x, p), complex(0.0, -om), self.a, self.b)
+        w, _ = self._border(self.cprob.J(x, p, transpose=True), complex(0.0, om), self.b, self.a)
+        self.a, self.b = w / float(np.max(np.abs(w))), v / float(np.max(np.abs(v)))
+
 
 def newton_hopf(prob, cprob, x0, p0, omega0, eigenvec, eigenvec_ad, opts, ls, cls, normN=V.norm2, cbls=None):
     """Newton on the Hopf MA system from (x0, p0, omega0) with guesses for the i omega eigenvector and its adjoint
     (newton_hopf, MinAugHopf.jl:258-283 + src/Newton.jl:66-114 on the state (x, [p, omega]))."""
     ma = HopfMinAug(prob, cprob, eigenvec_ad, eigenvec, ls, cls, cbls)
-    x, p, om = V.copy(x0), float(p0), float(omega0)
-    F, sr, si = ma.residual(x, p, om)
-    res = math.sqrt(normN(F) ** 2 + sr * sr + si * si)
-    residuals = [res]
-    step = 0
-    while step < opts.max_iterations and res > opts.tol:
-        dX, dp, dom, _ = ma.solve(x, p, om, F, sr, si)
-        V.axpby(x, -1.0, dX, 1.0)
-        p -= dp
-        om -= dom
-        F, sr, si = ma.residual(x, p, om)
-        res = math.sqrt(normN(F) ** 2 + sr * sr + si * si)
-        residuals.append(res)
-        step += 1
+    x, (p, om), _, residuals, step = _newton_ma(ma, x0, (p0, omega0), opts,
+                                               lambda F, sr, si: math.sqrt(normN(F) ** 2 + sr * sr + si * si))
     return HopfSolution(x, p, om, residuals, residuals[-1] < opts.tol, step, ma.itlinear)
 
 
 # ------------------------------------------------------------------------------------------------ Hopf curves in two parameters
-class _HopfMAJacobian:
-    def __init__(self, pb, z, p2):
-        self.pb, self.z, self.p2 = pb, z, p2
-
-
-class HopfLinearSolverMinAug:
-    """(hopfl::HopfLinearSolverMinAug)(Jhopf, rhs) -> (sol, converged, iters)   (MinAugHopf.jl:190-205)"""
-
-    def __call__(self, Jma, rhs):
-        pb, ma = Jma.pb, Jma.pb.ma
-        pb._set2(Jma.p2)
-        it0 = ma.itlinear
-        z = Jma.z
-        dX, dp, dom, cv = ma.solve(z.u, float(z.p[0]), float(z.p[1]), V.copy(rhs.u), float(rhs.p[0]), float(rhs.p[1]))
-        return BorderedVec(dX, [dp, dom]), cv, ma.itlinear - it0
-
-
-class HopfMAProblem:
-    """HopfMAProblem: [F(x, p1, p2); Re sigma; Im sigma] in the state z = (x, [p1, omega]) with continuation parameter
-    p2 = params[lens2] (continuation_hopf, MinAugHopf.jl:425-522)."""
-
-    def __init__(self, ma, lens2, z0, record=None):
-        assert lens2 != ma.prob.lens, "Please choose 2 different parameters."
-        self.ma, self.lens2, self.u0 = ma, lens2, z0
-        self.p0 = float(ma.prob.params[lens2])
-        self.delta = ma.prob.delta
-        self.record = record or (lambda z: float(z.p[0]))
-
-    def _set2(self, p2):
-        self.ma.prob.params[self.lens2] = p2
-        self.ma.cprob.params[self.lens2] = p2
-
-    def F(self, z, p2, out=None):
-        self._set2(p2)
-        Fu, sr, si = self.ma.residual(z.u, float(z.p[0]), float(z.p[1]))
-        if out is None:
-            return BorderedVec(Fu, [sr, si])
-        V.copyto(out.u, Fu)
-        out.p = np.array([sr, si])
-        return out
-
-    def J(self, z, p2):
-        return _HopfMAJacobian(self, z, p2)
-
-
 @dataclass
 class HopfCurve:
     rows: list
@@ -571,7 +563,7 @@ def continuation_hopf(prob, cprob, x0, p1_0, omega0, lens2, eigenvec, eigenvec_a
                       update_minaug_every_step=1, record=None, callback=None, cbls=None, detect_event=0, eigsolver=None):
     """Codim-2 continuation of a Hopf point in (p1 = params[prob.lens], p2 = params[lens2]): continuation_hopf(prob, alg,
     hopfpointguess, par, lens1, lens2, eigenvec, eigenvec_ad, options_cont; jacobian_ma = MinAug()) (MinAugHopf.jl:425-522).
-    PALC on the minimally augmented system in the state (x, [p1, omega]); Newton linear solver = HopfLinearSolverMinAug (one
+    PALC on the minimally augmented system in the state (x, [p1, omega]); Newton linear solver = MALinearSolver (one
     two-right-hand-side real solve + four complex shifted solves on the BK_COMPLEX twin `cprob`), outer bordered solver =
     BorderingBLS(that solver, check_precision = false); after every accepted step a <- w / ||w||, b <- v / ||v|| (update!,
     :323-367); the curve stops where omega -> 0 (Bogdanov-Takens, |omega| < 100 Newton tol).  With eigsolver (J, nev) -> (eigenvalues,
@@ -579,22 +571,11 @@ def continuation_hopf(prob, cprob, x0, p1_0, omega0, lens2, eigenvec, eigenvec_a
     src/events/BifurcationDetection.jl:57-70; tol_stability raised to 10 x the Newton tolerance so that the Hopf pair itself does not
     count): a change is a Zero-Hopf ("zh", one real eigenvalue) or Hopf-Hopf ("hh", a second pair) point, recorded (1) or located by
     the event bisection (2).  The Bautin test function (first Lyapunov coefficient) needs normal forms and is not evaluated."""
-    from . import palc as P
     ma = HopfMinAug(prob, cprob, eigenvec_ad, eigenvec, ls, cls, cbls)
-    z0 = BorderedVec(V.copy(x0), [p1_0, omega0])
-    pb = HopfMAProblem(ma, lens2, z0, record)
-    hls = HopfLinearSolverMinAug()
-    no = contpar.newton_options
-    cp = P.ContinuationPar(**{**contpar.__dict__, "newton_options": P.NewtonPar(tol=no.tol, max_iterations=no.max_iterations, linsolver=hls),
-                              "detect_bifurcation": 0})
-    alg = alg or P.PALC()
-    alg = P.PALC(tangent=alg.tangent, theta=alg.theta, bls=BorderingBLSHost(hls))
-    curve = HopfCurve([], [], [], [], ma, None)
-    curve.specialpoint = []
-    cnorm = lambda z: float(np.max(np.abs(z)))
-    from . import events as E
-    it = P.ContIterable(pb, alg, cp, normC)
-    tol_st = max(10 * no.tol, contpar.tol_stability)
+    pb = MAProblem(ma, lens2, BorderedVec(V.copy(x0), [p1_0, omega0]), record)
+    curve = HopfCurve([], [], [], [], ma, None, specialpoint=[])
+    tol = contpar.newton_options.tol
+    tol_st = max(10 * tol, contpar.tol_stability)
     nhist = []
 
     def unstable_at(s):   # (n_unstable, n_imag) of J at the Hopf point of state s (is_stable, src/Bifurcations.jl:5-18)
@@ -603,37 +584,26 @@ def continuation_hopf(prob, cprob, x0, p1_0, omega0, lens2, eigenvec, eigenvec_a
         un = ev.real > tol_st
         return (int(np.sum(un)), int(np.sum(un & (np.abs(ev.imag) > tol_st))))
 
-    def cb(st):
-        pb._set2(st.z_p)
-        x, p1, om = st.z_u.u, float(st.z_u.p[0]), float(st.z_u.p[1])
+    def point(it, st):
         if eigsolver is not None:
             nu = unstable_at(st)
             if detect_event > 0 and nhist and st.step > 0 and nu[0] != nhist[-1][0]:
-                prev, status, interval = nhist[-1], "guess", E.getinterval(curve.p2[-1], st.z_p)
-                if detect_event > 1:
-                    status, interval, _ = locate_event(it, st, lambda s: (unstable_at(s)[0],), ("hh",), indicator=lambda v: v[0])
-                    pb._set2(st.z_p)
-                    nu = unstable_at(st)
-                    x, p1, om = st.z_u.u, float(st.z_u.p[0]), float(st.z_u.p[1])
-                if status != "none":
+                prev = nhist[-1]
+                found, nu = _event(it, st, curve.p2[-1], None, nu, unstable_at, ("hh",), detect_event, indicator=lambda v: v[0])
+                if found:
                     dn, di = abs(nu[0] - prev[0]), abs(nu[1] - prev[1])
-                    curve.specialpoint.append(Codim2Point("zh" if dn == 1 else ("hh" if di == 2 else "nd"), st.z_p, p1, st.step, status, tuple(interval), V.copy(x)))
+                    curve.specialpoint.append(Codim2Point("zh" if dn == 1 else ("hh" if di == 2 else "nd"), st.z_p, ma.unpack(st.z_u.p)[0],
+                                                          st.step, found[0], found[1], V.copy(st.z_u.u)))
             nhist.append(nu)
+        p1, om = ma.unpack(st.z_u.p)
         if st.step % update_minaug_every_step == 0:
-            v, _ = ma._border(cprob.J(x, p1), complex(0.0, -om), ma.a, ma.b)
-            w, _ = ma._border(cprob.J(x, p1, transpose=True), complex(0.0, om), ma.b, ma.a)
-            ma.a, ma.b = w / cnorm(w), v / cnorm(v)
+            ma.update(st.z_u.u, p1, om)
         curve.p1.append(p1)
         curve.p2.append(st.z_p)
         curve.omega.append(om)
-        if abs(om) < 100 * no.tol:  # the frequency is null: not a Hopf point any more, the curve ends on a Bogdanov-Takens point
+        if abs(om) < 100 * tol:  # the frequency is null: not a Hopf point any more, the curve ends on a Bogdanov-Takens point
             curve.stopped_at_bt = True
             return False
-        return True if callback is None else callback(st)
 
-    p2_0, c2_0 = prob.params[lens2], cprob.params[lens2]
-    try:
-        curve.rows, curve.state = P.continuation(pb, alg, cp, normC=normC, callback=cb, it=it)
-    finally:
-        prob.params[lens2], cprob.params[lens2] = p2_0, c2_0
+    curve.rows, curve.state = _continue_ma(pb, contpar, alg, normC, point, callback)
     return curve
