@@ -14,13 +14,12 @@ The deflation operator is built with ``fused=True``: on device vectors M(u) and 
 come from one ``bk_deflation_moments`` pass, and so do the distances of a candidate to the known roots (the m_i / s_i of the
 kernel for ``normC`` = norminf / norm2).
 """
-import copy as _copy
 from dataclasses import dataclass, field, replace as _replace
 import math
 
 from .deflation import DeflationOperator, newton_deflated_or_fail
 from .events import Branch, branch_row, detect_bifurcation, get_bifurcation_type, getinterval
-from .palc import PALC, V, ContIterable
+from .palc import PALC, V, ContIterable, re_make
 
 
 def _perturb_solution(x, p, idb):
@@ -71,16 +70,6 @@ class DCResult:
     alg: DefCont
 
 
-def _re_make(prob, u0, p):
-    """re_make(prob; u0, params = set(par, lens, p))"""
-    new = _copy.copy(prob)
-    new.u0, new.p0 = u0, p
-    if getattr(prob, "params", None) is not None and getattr(prob, "lens", None) is not None:
-        new.params = list(prob.params)
-        new.params[prob.lens] = p
-    return new
-
-
 def distances(defop, u, others, normC):
     """[normC(u - r) for r in others]: from the m_i (norminf) or s_i (norm2) of one bk_deflation_moments pass where the operator
     runs fused at u, else by vector operations"""
@@ -125,7 +114,7 @@ def continuation(prob, alg, contpar, normC=V.norm2, callback_newton=None, save_s
     it = ContIterable(prob, alg.alg, cp, normC, callback_newton)
 
     # start-up (:157-166): every branch starts from iterate(contIt) with prob.u0 = roots[1]
-    it.prob = _re_make(prob, V.copy(defop.roots[0]), prob.p0)
+    it.prob = re_make(prob, V.copy(defop.roots[0]), prob.p0)
     states, branches = [], []
     for _ in defop.roots:
         dcs, br = _new_branch(it, sol_every)
@@ -159,7 +148,7 @@ def continuation(prob, alg, contpar, normC=V.norm2, callback_newton=None, save_s
     def new_solution(dcs, p, idb):
         """_DC_get_new_solution (:269-286)"""
         u0 = alg.perturb_solution(V.copy(dcs.state.z_u), p, idb)
-        pb = _re_make(it.prob, u0, p)
+        pb = re_make(it.prob, u0, p)
         sol = newton_deflated_or_fail(pb, u0, p, defop, _replace(opts, max_iterations=alg.max_iter_defop), normC, callback_newton)
         if sol.converged:
             sol.converged = normC(it.prob.F(sol.u, p)) < opts.tol     # the residual of the problem itself (:281)
@@ -200,7 +189,7 @@ def continuation(prob, alg, contpar, normC=V.norm2, callback_newton=None, save_s
                         if verbosity >= 1:
                             print(f"step {nstep} p={current:.6e}: new solution from branch {idb}", flush=True)
                         defop.roots.append(sol.u)
-                        itn = ContIterable(_re_make(it.prob, sol.u, current), alg.alg, cp, normC, callback_newton)
+                        itn = ContIterable(re_make(it.prob, sol.u, current), alg.alg, cp, normC, callback_newton)
                         new, br = _new_branch(itn, sol_every)
                         new.isactive = n_active + 1 < alg.max_branches
                         states.append(new)

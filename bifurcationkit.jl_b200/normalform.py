@@ -29,7 +29,6 @@ call and a dot product per tuple (jet_moments_composed).
 Not here: the generic BranchPoint predictor (_predictor, src/NormalForms.jl:496-535), usedeflation = false, bothside and
 bifurcationdiagram; higher codimension normal forms.
 """
-import copy
 import itertools
 from dataclasses import dataclass, replace
 import math
@@ -37,10 +36,12 @@ import types
 import warnings
 
 import numpy as np
+import scipy.linalg as sla
 
-from .codim2 import _apply
-from .core import DeviceVec, ShiftInvertB200, MatrixFreeBLSB200
-from .palc import V, ContIterable
+from .codim2 import _apply, ComplexProblemB200
+from .core import Context, DeviceVec, ComplexGMRESB200, ShiftInvertB200, MatrixFreeBLSB200
+from .deflation import DeflationOperator, newton_deflated_or_fail
+from .palc import V, ContIterable, NewtonPar, re_make
 from . import events
 
 
@@ -67,6 +68,11 @@ def _like(x, a):
     return x.ctx.to_device(a) if isinstance(x, DeviceVec) else a
 
 
+def _given(x, z):
+    """a vector given by the caller, as a new vector of the container of x: a list or host array through _like, else a copy"""
+    return _like(x, z) if isinstance(z, (list, np.ndarray)) else V.copy(z)
+
+
 def _eig(eigsolver, J, nev):
     """eigsolver(J, nev) with eigenvectors: (vals, vecs as columns)"""
     out = eigsolver(J, nev, want_vectors=True) if isinstance(eigsolver, ShiftInvertB200) else eigsolver(J, nev)
@@ -76,6 +82,23 @@ def _eig(eigsolver, J, nev):
 def _isapprox(a, b):
     """Julia's a ≈ b with the default rtol = sqrt(eps)"""
     return a == b or abs(a - b) <= math.sqrt(np.finfo(float).eps) * max(abs(a), abs(b))
+
+
+def _eig_entry(br, bifpt, nev):
+    """the br.eig entry saved at the special point bifpt, its eigenvalues as an array, and nev (their number when None)"""
+    entry = next(e for e in br.eig if e["step"] == bifpt.idx)
+    saved = np.asarray(entry["eigenvals"])
+    return entry, saved, len(saved) if nev is None else nev
+
+
+def _recomputed_eig(prob, x0, p, eigsolver, nev, k, expected):
+    """the eigenpairs of J at (x0, p) recomputed with eigsolver (nev of them); raises unless eigenvalue k ≈ expected, the one
+    saved with the branch"""
+    vals, vecs = _eig(eigsolver, prob.J(x0, p), nev)
+    if not _isapprox(vals[k], expected):
+        raise RuntimeError(f"We did not find the correct eigenvalue {expected}. We found {vals}.\n"
+                           "If you use aBS, pass a higher `nev` (number of eigenvalues) to be computed.")
+    return vals, vecs
 
 
 def _E(x, zeta, zeta_ad):
@@ -110,17 +133,23 @@ def _adjoint_basis(prob, x0, p, lams, eigsolver, nev):
     """get_adjoint_basis(L★, λs, eigsolver; nev) (src/NormalForms.jl:1-24): from one eigen-solve of J', for each λ of `lams` in
     turn the eigenvector whose eigenvalue is closest to conj(λ), each eigenvalue used once.  J' is prob.Jt where the problem has
     it (host problems, device kinds with a J' kernel), else J under bk_jac_set_transpose.  A real λ gives a real vector of the
-    container of x0, a complex λ a complex host array.  Returns (vectors, their eigenvalues)."""
+    container of x0, a complex λ a complex host array.  An eigenvalue found with |Re| > 1e-2 is warned of in the words of the
+    reference's method for one λ (:31-49) or for a list."""
     def adjoint(J):
         vals, vecs = _eig(eigsolver, J, nev)
         free = np.array(vals, dtype=complex)
-        out, found = [], []
+        out = []
         for lam in lams:
             i = int(np.argmin(np.abs(free - np.conj(lam))))
             free[i] = 1e9                                        # not used twice (:21)
-            found.append(vals[i])
+            if abs(vals[i].real) > 1e-2 and len(lams) == 1:
+                warnings.warn(f"The bifurcating eigenvalue is not that close to Re = 0. We found {vals[i].real} !≈ 0. "
+                              "You can perhaps increase the argument `nev`.")
+            elif abs(vals[i].real) > 1e-2:
+                warnings.warn(f"Did not converge to the requested eigenvalues. We found {vals[i].real} !≈ 0. This might not "
+                              "lead to precise normal form computation. You can perhaps increase the argument `nev`.")
             out.append(_like(x0, np.asarray(vecs)[:, i]) if np.imag(lam) == 0 else _eigvec(J, vals, vecs, i))
-        return out, found
+        return out
     if hasattr(prob, "Jt"):
         return adjoint(prob.Jt(x0, p))
     prob.ctx.set_transpose(True)
@@ -133,15 +162,32 @@ def _adjoint_basis(prob, x0, p, lams, eigsolver, nev):
 def _adjoint_vector(prob, x0, p, lam, eigsolver, nev):
     """get_adjoint_basis(L★, conj(λ), eigsolver; nev) (src/NormalForms.jl:31-49): the eigenvector of J' whose eigenvalue is
     closest to conj(λ) (_adjoint_basis for one λ)."""
-    (vec,), (val,) = _adjoint_basis(prob, x0, p, [lam], eigsolver, nev)
-    if abs(val.real) > 1e-2:
-        warnings.warn(f"The bifurcating eigenvalue is not that close to Re = 0. We found {val.real} !≈ 0. "
-                      "You can perhaps increase the argument `nev`.")
-    return vec
+    return _adjoint_basis(prob, x0, p, [lam], eigsolver, nev)[0]
 
 
-def _eigvals_at(br, bifpt):
-    return next(e["eigenvals"] for e in br.eig if e["step"] == bifpt.idx)
+def _adjoint_vectors(prob, x0, p, zetas, zetas_ad, lams, eigsolver, nev):
+    """ζ★s of a branch point (src/NormalForms.jl:260-272, :737-748): zetas_ad as given, in the container of x0; copies of ζs
+    for a symmetric problem; else the eigenvectors of J' for λs (_adjoint_basis), a complex one replaced by its real part"""
+    if zetas_ad is not None:
+        return [_given(x0, z) for z in zetas_ad]
+    if getattr(prob, "symmetric", False):
+        return [V.copy(z) for z in zetas]
+    return [z if not np.iscomplexobj(z) else _like(x0, z) for z in _adjoint_basis(prob, x0, p, lams, eigsolver, nev)]
+
+
+def _parameter_differences(prob, x0, p):
+    """R01 = ∂F/∂p and R02 = ∂²F/∂p² at (x0, p) by central differences with prob.delta (src/NormalForms.jl:293-297), from
+    F(p + δ), F(p), F(p - δ) in that order, and d_dp(v) = ∂(dF v)/∂p from J(p + δ) v and J(p - δ) v; each a new vector"""
+    delta = prob.delta
+
+    def central(fp, fm):  # (fp - fm) / 2δ, in fp
+        return V.scale(V.axpby(fp, -1.0, fm, 1.0), 1.0 / (2 * delta))
+
+    Fp, F0, Fm = prob.F(x0, p + delta), prob.F(x0, p), prob.F(x0, p - delta)
+    R02 = V.axpby(V.axpby(V.copy(Fp), -2.0, F0, 1.0), 1.0, Fm, 1.0)   # before central overwrites Fp
+    V.scale(R02, 1.0 / delta**2)
+    R01 = central(Fp, Fm)
+    return R01, R02, lambda v: central(_apply(prob.J(x0, p + delta), v), _apply(prob.J(x0, p - delta), v))
 
 
 def get_normal_form1d(it, br, ind_bif, nev=None, zeta=None, zeta_ad=None, bls=None, tol_fold=1e-3):
@@ -160,25 +206,18 @@ def get_normal_form1d(it, br, ind_bif, nev=None, zeta=None, zeta_ad=None, bls=No
         raise ValueError("We only provide normal form computation for simple bifurcation points e.g. when the kernel of the "
                          f"jacobian is 1d. Here, the dimension of the kernel is {abs(bifpt.delta[0])}.")
     bls = bls or MatrixFreeBLSB200(options.linsolver)
-    x0, p, delta = bifpt.x, bifpt.param, prob.delta                                      # :223-230
-    saved = np.asarray(_eigvals_at(br, bifpt))
-    nev = len(saved) if nev is None else nev
-    lam = float(np.real(saved[bifpt.ind_ev - 1]))                                        # :236 (ind_ev is 1-based)
+    x0, p = bifpt.x, bifpt.param                                                         # :223-230
+    _, saved, nev = _eig_entry(br, bifpt, nev)
+    k = bifpt.ind_ev - 1                                                                 # ind_ev is 1-based
+    lam = float(np.real(saved[k]))                                                       # :236
     if zeta is None:                                                                     # :243-256
-        nev_required = max(nev, bifpt.ind_ev + 2)
-        vals, vecs = _eig(options.eigsolver, prob.J(x0, p), nev_required)
-        if not _isapprox(vals[bifpt.ind_ev - 1], lam):
-            raise RuntimeError(f"We did not find the correct eigenvalue {lam}. We found {vals}")
-        zeta = _like(x0, np.asarray(vecs)[:, bifpt.ind_ev - 1])
+        _, vecs = _recomputed_eig(prob, x0, p, options.eigsolver, max(nev, bifpt.ind_ev + 2), k, lam)
+        zeta = _like(x0, np.asarray(vecs)[:, k])
     else:
-        zeta = _like(x0, zeta) if isinstance(zeta, (list, np.ndarray)) else V.copy(zeta)
+        zeta = _given(x0, zeta)
     V.scale(zeta, 1.0 / V.norm2(zeta))                                                   # scaleζ = norm, :257
-    if zeta_ad is not None:                                                              # :260-272
-        zeta_ad = _like(x0, zeta_ad) if isinstance(zeta_ad, (list, np.ndarray)) else V.copy(zeta_ad)
-    elif getattr(prob, "symmetric", False):
-        zeta_ad = V.copy(zeta)
-    else:
-        zeta_ad = _adjoint_vector(prob, x0, p, lam, options.eigsolver, nev)
+    (zeta_ad,) = _adjoint_vectors(prob, x0, p, [zeta], None if zeta_ad is None else [zeta_ad], [lam], options.eigsolver,
+                                  nev)                                                   # :260-272
     zz = V.dot(zeta, zeta_ad)
     if not abs(zz) > 1e-10:                                                              # :275-277
         raise RuntimeError(f"We got ζ⋅ζ★ = {zz}.\nThis dot product should not be zero.\n"
@@ -187,7 +226,6 @@ def get_normal_form1d(it, br, ind_bif, nev=None, zeta=None, zeta_ad=None, bls=No
 
     R2 = lambda a, b: prob.d2F(x0, p, a, b)
     R3 = lambda a, b, c: prob.d3F(x0, p, a, b, c)
-    dF = lambda q, v: _apply(prob.J(x0, q), v)
 
     def solve(rhs):  # bls(L, ζ★, ζ, 0, E(-rhs), 0): L is re-made before each solve (a device context keeps one Jacobian)
         r = V.scale(V.copy(rhs), -1.0)
@@ -196,18 +234,12 @@ def get_normal_form1d(it, br, ind_bif, nev=None, zeta=None, zeta_ad=None, bls=No
             warnings.warn(f"[Normal form] Linear solver for J did not converge. it = {its}")
         return psi
 
-    def central(fp, fm):  # (fp - fm) / 2δ, in fp
-        return V.scale(V.axpby(fp, -1.0, fm, 1.0), 1.0 / (2 * delta))
-
-    Fp, F0, Fm = prob.F(x0, p + delta), prob.F(x0, p), prob.F(x0, p - delta)            # :293-297
-    R02 = V.axpby(V.axpby(V.copy(Fp), -2.0, F0, 1.0), 1.0, Fm, 1.0)
-    V.scale(R02, 1.0 / delta**2)
-    R01 = central(Fp, Fm)
+    R01, R02, d_dp = _parameter_differences(prob, x0, p)                                 # :293-297
     a01 = V.dot(R01, zeta_ad)
     Psi01 = solve(R01)                                                                   # :303
-    R11 = central(dF(p + delta, zeta), dF(p - delta, zeta))                              # :310-312
+    R11 = d_dp(zeta)                                                                     # :310-312
     b11 = V.dot(V.axpby(R11, 1.0, R2(zeta, Psi01), 1.0), zeta_ad)
-    R11Psi = central(dF(p + delta, Psi01), dF(p - delta, Psi01))                         # :319-320
+    R11Psi = d_dp(Psi01)                                                                 # :319-320
     a2v = V.axpby(V.axpby(R02, 2.0, R11Psi, 1.0), 1.0, R2(Psi01, Psi01), 1.0)
     a02 = V.dot(a2v, zeta_ad)
     b2v = R2(zeta, zeta)                                                                 # :328
@@ -277,8 +309,6 @@ def d3Fc(prob, x0, p, a, b, c):
 
 def _complex_twin(prob):
     """ComplexProblemB200 and ComplexGMRESB200 on a BK_COMPLEX context of the device problem's grid (codim2.py)"""
-    from .codim2 import ComplexProblemB200
-    from .core import Context, ComplexGMRESB200
     ctx = prob.ctx
     cctx = Context(ctx.kind, ctx.dims, ctx.lengths, krylov_m=ctx.krylov_m, params=ctx.params, complex=True)
     return ComplexProblemB200(cctx, prob.params, prob.lens)
@@ -296,7 +326,6 @@ def hopf_normal_form_at(prob, x0, p, omega, zeta, zeta_ad, ls, cprob=None, cls=N
     if cprob is None:
         cprob = _complex_twin(prob)
     if cls is None:
-        from .core import ComplexGMRESB200
         cls = ComplexGMRESB200(reltol=ls.reltol, abstol=ls.abstol, restart=ls.restart, maxiter=ls.maxiter, Pl=ls.Pl, Pr=ls.Pr,
                                orth=ls.orth, fused=ls.fused)
     R2 = lambda a, b: d2Fc(prob, x0, p, a, b) / 2
@@ -339,9 +368,7 @@ def hopf_normal_form(it, br, ind_hopf, nev=None, zeta=None, zeta_ad=None, detail
     if bifpt.type != "hopf":
         raise ValueError("The provided index does not refer to a Hopf Point")
     x0, p = bifpt.x, bifpt.param
-    entry = next(e for e in br.eig if e["step"] == bifpt.idx)
-    saved = np.asarray(entry["eigenvals"])
-    nev = len(saved) if nev is None else nev
+    entry, saved, nev = _eig_entry(br, bifpt, nev)
     k = bifpt.ind_ev - 1                                                                     # ind_ev is 1-based
     # :1138-1139.  λ is the member of the crossing pair with Im λ > 0 -- the one the reference's DefaultEig puts at ind_ev (it
     # lists a pair of equal real parts with the positive imaginary part second); the guess x0 + 2 Re(ζ A(t)) of the predictor
@@ -355,10 +382,7 @@ def hopf_normal_form(it, br, ind_hopf, nev=None, zeta=None, zeta_ad=None, detail
     elif entry.get("eigenvecs") is not None:                                                 # :1150-1151
         zeta = _eigvec(prob.J(x0, p), saved, entry["eigenvecs"], closest(saved))
     else:                                                                                    # :1142-1148
-        vals, vecs = _eig(options.eigsolver, prob.J(x0, p), bifpt.ind_ev + 2)
-        if not _isapprox(vals[k], complex(saved[k])):
-            raise RuntimeError(f"We did not find the correct eigenvalue {saved[k]}. We found {vals}.\n"
-                               "If you use aBS, pass a higher `nev` (number of eigenvalues) to be computed.")
+        vals, vecs = _recomputed_eig(prob, x0, p, options.eigsolver, bifpt.ind_ev + 2, k, complex(saved[k]))
         zeta = _eigvec(prob.J(x0, p), vals, vecs, closest(vals))
     zeta = np.asarray(zeta, dtype=complex) / np.linalg.norm(zeta)                            # :1153
     if not detailed:                                                                         # :1155-1168
@@ -471,13 +495,15 @@ def continuation_from_bp(br, ind_bif, prob, alg, contpar, normC=V.norm2, ds=None
         pred = predictor(bp, ds, ampfactor)
     if pred is None:
         return None
-    cp = replace(contpar, ds=abs(contpar.ds) * float(np.sign(pred.p - bp.p)))            # :18-20
-    prob2 = copy.copy(prob)                                                              # re_make(prob; params = par0)
-    prob2.u0, prob2.p0 = bp.x0, bp.p
-    if hasattr(prob2, "params"):
-        prob2.params = list(prob.params)
-        prob2.params[prob.lens] = bp.p
-    return events.continuation(prob2, alg, cp, normC, verbose=verbose, callback=callback, u1=pred.x1, p1=pred.p), bp
+    sign = float(np.sign(pred.p - bp.p))                                                 # :18-20
+    return _continue_from(prob, bp, alg, contpar, normC, pred.x1, pred.p, sign, callback, verbose), bp
+
+
+def _continue_from(prob, bp, alg, contpar, normC, u1, p1, ds_sign, callback, verbose):
+    """events.continuation (alg, contpar with ds = |contpar.ds| ds_sign, normC, callback, verbose) of re_make(prob; u0 = bp.x0,
+    params = par0) from the two points (bp.x0, bp.p) and (u1, p1) (src/bifdiagram/BranchSwitching.jl:8-44)"""
+    cp = replace(contpar, ds=abs(contpar.ds) * ds_sign)
+    return events.continuation(re_make(prob, bp.x0, bp.p), alg, cp, normC, verbose=verbose, callback=callback, u1=u1, p1=p1)
 
 
 # ------------------------------------------------------------------------------------------------ kernels of dimension N > 1
@@ -515,7 +541,6 @@ def biorthogonalise(zetas, zetas_ad):
     """biorthogonalise(ζs, ζ★s) (src/NormalForms.jl:51-91): ζ★s <- Q' ζ★s with Q = pinv(G), G_ij = <ζ_i, ζ★_j>; when G is then
     not the identity to 1e-5, the LU algorithm (G = P L U: ζs <- (P L)^-1 ζs, ζ★s <- U'^-1 ζ★s), which also changes ζs.
     Raises as the reference does when G is singular or the result is not biorthogonal."""
-    import scipy.linalg as sla
     assert len(zetas) == len(zetas_ad), "The Gram matrix is not square!"
     G = _gram(zetas, zetas_ad)
     if abs(np.linalg.det(G)) <= 1e-14:
@@ -592,10 +617,9 @@ def get_normal_formNd(it, br, ind_bif, nev=None, zetas=None, zetas_ad=None, bls=
     if N < 2:
         raise ValueError(f"get_normal_formNd needs a kernel of dimension > 1, here {N}: use get_normal_form1d.")
     bls = bls or MatrixFreeBLSB200(options.linsolver)
-    x0, p, delta = bifpt.x, bifpt.param, prob.delta
-    entry = next(e for e in br.eig if e["step"] == bifpt.idx)
-    rightEv = np.asarray(entry["eigenvals"])
-    nev = max(2 * N, len(rightEv) if nev is None else nev)                               # :680-681
+    x0, p = bifpt.x, bifpt.param
+    entry, rightEv, nev = _eig_entry(br, bifpt, nev)
+    nev = max(2 * N, nev)                                                                # :680-681
     ind = list(range(bifpt.ind_ev - N, bifpt.ind_ev))                                    # indev-N+1:indev, 0-based
     lams = rightEv[ind]
     if zetas is None:                                                                    # :711-724
@@ -607,20 +631,10 @@ def get_normal_formNd(it, br, ind_bif, nev=None, zetas=None, zetas_ad=None, bls=
                 warnings.warn(f"We did not find the correct eigenvalues. We found {vals[: len(rightEv)]} instead of {rightEv}.")
         zetas = [_like(x0, np.asarray(vecs)[:, i]) for i in ind]
     else:
-        zetas = [_like(x0, z) if isinstance(z, (list, np.ndarray)) else V.copy(z) for z in zetas]
+        zetas = [_given(x0, z) for z in zetas]
     for z in zetas:                                                                      # scaleζ = norm, :729
         V.scale(z, 1.0 / V.norm2(z))
-    if zetas_ad is not None:                                                             # :737-747
-        zetas_ad = [_like(x0, z) if isinstance(z, (list, np.ndarray)) else V.copy(z) for z in zetas_ad]
-    elif getattr(prob, "symmetric", False):
-        zetas_ad = [V.copy(z) for z in zetas]
-    else:
-        zetas_ad, found = _adjoint_basis(prob, x0, p, lams, options.eigsolver, nev)   # it compares with conj(λ)
-        for val in found:
-            if abs(val.real) > 1e-2:
-                warnings.warn(f"Did not converge to the requested eigenvalues. We found {val.real} !≈ 0. This might not lead to "
-                              "precise normal form computation. You can perhaps increase the argument `nev`.")
-        zetas_ad = [z if not np.iscomplexobj(z) else _like(x0, z) for z in zetas_ad]    # real.(ζ★s), :748
+    zetas_ad = _adjoint_vectors(prob, x0, p, zetas, zetas_ad, lams, options.eigsolver, nev)   # :737-748
     zetas, zetas_ad = biorthogonalise(zetas, zetas_ad)                                   # :752
 
     gram_inv = np.linalg.inv(_gram(zetas, zetas)) if N > 2 else None
@@ -637,22 +651,15 @@ def get_normal_formNd(it, br, ind_bif, nev=None, zetas=None, zetas_ad=None, bls=
             psi = _lincomb([1.0] + list(-c), [psi] + zetas)
         return psi
 
-    def central(fp, fm):  # (fp - fm) / 2δ, in fp
-        return V.scale(V.axpby(fp, -1.0, fm, 1.0), 1.0 / (2 * delta))
-
-    dF = lambda q, v: _apply(prob.J(x0, q), v)
-    Fp, F0, Fm = prob.F(x0, p + delta), prob.F(x0, p), prob.F(x0, p - delta)            # :774-780
-    R02 = V.axpby(V.axpby(V.copy(Fp), -2.0, F0, 1.0), 1.0, Fm, 1.0)
-    V.scale(R02, 1.0 / delta**2)
-    R01 = central(Fp, Fm)
+    R01, R02, d_dp = _parameter_differences(prob, x0, p)                                 # :774-780
     a01 = np.array([V.dot(R01, za) for za in zetas_ad])                                 # :782-784
     # The reference re-solves the Ψ01 system inside its jj loop (:798) and the wst system of each ordered pair inside its b30
     # loop (:844-857).  The device solver is deterministic, so one solve for Ψ01 gives the reference's numbers exactly, and so
     # does one wst solve per unordered pair {k, l} where d2F is symmetric bit for bit: the SH kinds and chan, whose pointwise
     # products commute.  For cGL2d (cgl_jet adds its terms in argument order) and host d2F the two orders agree to rounding.
     Psi01 = solve(V.scale(E(R01), -1.0), "Ψ01")
-    R11 = [central(dF(p + delta, z), dF(p - delta, z)) for z in zetas]                   # :790-796
-    R11Psi = central(dF(p + delta, Psi01), dF(p - delta, Psi01))                         # :806-811 (the same for every jj)
+    R11 = [d_dp(z) for z in zetas]                                                       # :790-796
+    R11Psi = d_dp(Psi01)                                                                 # :806-811 (the same for every jj)
     a2v = V.axpby(R02, 2.0, R11Psi, 1.0)
     pairs = [(k, l) for k in range(N) for l in range(k, N)]
     w = {kl: solve(E(prob.d2F(x0, p, zetas[kl[0]], zetas[kl[1]])), "wst") for kl in pairs}
@@ -732,11 +739,6 @@ class _ReducedProblem:
         return _Dense(self.bp.reduced_jacobian(x, p))
 
 
-def _newton_deflated(prob, x0, p, defop, opts, normN):
-    from .deflation import newton_deflated_or_fail
-    return newton_deflated_or_fail(prob, x0, p, defop, opts, normN)
-
-
 def predictor_nd(bp, dp, rng=None, ampfactor=1.0, nbfailures=50, maxiter=100, igs=None, amp_igs=1.0, normN=None,
                  perturb=lambda r: r, tol=1e-12):
     """predictor(bp::NdBranchPoint, δp) (src/NormalForms.jl:916-985): the zeros of the reduced equation at dp = -|δp| and +|δp|,
@@ -745,8 +747,6 @@ def predictor_nd(bp, dp, rng=None, ampfactor=1.0, nbfailures=50, maxiter=100, ig
     numpy.random.Generator (default_rng(0) by default), so that the result is reproducible.  perturb is applied to the reduced
     residual, as the reference's.  The Jacobian is the analytic one of the cubic.  Returns (before, after): the roots found on
     each side, the trivial one first, each multiplied by ampfactor."""
-    from .deflation import DeflationOperator
-    from .palc import NewtonPar
     rng = np.random.default_rng(0) if rng is None else rng
     n = len(bp.zetas)
     normN = normN or (lambda v: float(np.max(np.abs(v))))
@@ -761,12 +761,12 @@ def predictor_nd(bp, dp, rng=None, ampfactor=1.0, nbfailures=50, maxiter=100, ig
             ci = np.asarray(ci, dtype=float)
             if np.linalg.norm(ci) > 0:
                 u0 = ci * amp_igs
-                sol = _newton_deflated(prob, u0, ds, defop, opts, normN)
+                sol = newton_deflated_or_fail(prob, u0, ds, defop, opts, normN)
                 if sol.converged:
                     defop.push(ampfactor * sol.u)
         failures = 0
         while failures < nbfailures:                                                     # :966-976
-            sol = _newton_deflated(prob, u0, ds, defop, opts, normN)
+            sol = newton_deflated_or_fail(prob, u0, ds, defop, opts, normN)
             if sol.converged:
                 defop.push(ampfactor * sol.u)
             else:
@@ -782,7 +782,6 @@ def get_first_points_on_branch(bp, solfromRE, prob, contpar, ds=None, max_iter_d
     (newton_deflated: DeflatedProblemCustomLS around the Newton linear solver) on the full problem at p + |ds| from bp(root) for
     every root after the bifurcation point, then at p - |ds| for those before, each side with its own DeflationOperator(2, 1, []).
     Returns a namespace (before, after: the converged states, bpm = p - |ds|, bpp = p + |ds|)."""
-    from .deflation import DeflationOperator
     ds = abs(contpar.ds if ds is None else ds)
     optn = contpar.newton_options
     optnDf = replace(optn, max_iterations=min(50, 15 * optn.max_iterations) if max_iter_deflation is None else max_iter_deflation)
@@ -791,7 +790,7 @@ def get_first_points_on_branch(bp, solfromRE, prob, contpar, ds=None, max_iter_d
     def side(roots, q):
         defop = DeflationOperator(2, 1.0, [])
         for xsol in roots:
-            sol = _newton_deflated(prob, perturb_guess(bp(xsol, ds)), q, defop, optnDf, normN)
+            sol = newton_deflated_or_fail(prob, perturb_guess(bp(xsol, ds)), q, defop, optnDf, normN)
             if sol.converged:
                 defop.push(sol.u)
         return defop.roots
@@ -817,16 +816,6 @@ def multicontinuation(br, ind_bif, prob, alg, contpar, normC=V.norm2, ds=None, a
     dp = abs(contpar.ds if ds is None else ds)
     roots = solfromRE or predictor_nd(bp, dp, rng=rng, ampfactor=ampfactor)
     first = get_first_points_on_branch(bp, roots, prob, contpar, dp, max_iter_deflation, perturb_guess, normN=normC)
-    prob2 = copy.copy(prob)                                                              # re_make(prob; params = par0)
-    prob2.u0, prob2.p0 = bp.x0, bp.p
-    if hasattr(prob2, "params"):
-        prob2.params = list(prob.params)
-        prob2.params[prob.lens] = bp.p
-    dscont = abs(contpar.ds)
-
-    def cont(u1, p1, sign):
-        cp = replace(contpar, ds=sign * dscont)
-        return events.continuation(prob2, alg, cp, normC, verbose=verbose, callback=callback, u1=u1, p1=p1), bp
-    out = [cont(u, first.bpm, -1.0) for u in first.before[1:]]
-    out += [cont(u, first.bpp, 1.0) for u in first.after[1:]]
+    out = [(_continue_from(prob, bp, alg, contpar, normC, u, first.bpm, -1.0, callback, verbose), bp) for u in first.before[1:]]
+    out += [(_continue_from(prob, bp, alg, contpar, normC, u, first.bpp, 1.0, callback, verbose), bp) for u in first.after[1:]]
     return out

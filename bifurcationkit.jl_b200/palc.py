@@ -9,6 +9,7 @@ The state vector is either a ``DeviceVec`` (device-resident, "option B") or a Nu
 buffers crossing the C ABI on every call, "option A"): the loop below is written against the small
 vector interface ``V`` and never touches elements.
 """
+import copy
 from dataclasses import dataclass, field
 import math
 
@@ -209,6 +210,17 @@ class BifurcationProblemB200:
         """is_symmetric(prob) (src/Problems.jl:126): J' = J for the Swift-Hohenberg kinds"""
         from . import lib as _l
         return (self.ctx.kind & ~_l.BK_COMPLEX) in (_l.BK_SH2D, _l.BK_SH3D, _l.BK_SH2D_PERIODIC)
+
+
+def re_make(prob, u0, p):
+    """re_make(prob; u0, params = set(par, lens, p)): a shallow copy of prob with (u0, p0) = (u0, p) and, where the problem has
+    params and a lens, a copy of params with the continuation parameter set to p; prob is left as it is"""
+    new = copy.copy(prob)
+    new.u0, new.p0 = u0, p
+    if getattr(prob, "params", None) is not None and getattr(prob, "lens", None) is not None:
+        new.params = list(prob.params)
+        new.params[prob.lens] = p
+    return new
 
 
 @dataclass
