@@ -6,7 +6,8 @@ Contents: csrc/ (CUDA kernels + C ABI -> libbk200.so), lib.py (ctypes binding), 
 the reference's AbstractLinearSolver / AbstractBorderedLinearSolver / AbstractEigenSolver surfaces),
 palc.py (host-side Newton / newton_palc / continuation loop driving the device kernels), defcont.py (deflated
 continuation), periodic.py (periodic-orbit
-branches with the Trapeze functional and branch switching to them from a Hopf point).
+branches with the Trapeze functional and branch switching to them from a Hopf point), bifdiagram.py (automatic bifurcation
+diagrams, sibling branches continued concurrently).
 """
 from . import lib
 from .lib import (BK200Error, BK_CHAN, BK_SH2D, BK_SH3D, BK_CGL2D, BK_POTRAP_CGL2D, BK_SH2D_PERIODIC, BK_COMPLEX, BK_PC_NONE,
@@ -22,3 +23,4 @@ from . import defcont
 from . import codim2
 from . import normalform
 from . import periodic
+from . import bifdiagram

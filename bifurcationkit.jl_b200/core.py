@@ -22,6 +22,7 @@ the right-hand side, as the reference requires (Newton does ``minus!!(x, u)``, s
 """
 import contextlib
 import ctypes as C
+import threading
 
 import numpy as np
 
@@ -36,10 +37,17 @@ def _chk(ctx, status):
 
 
 class Context:
-    """One per GPU: owns the CUDA stream, Krylov workspace and the problem description."""
+    """One per stream: owns the CUDA stream, Krylov workspace and the problem description.  Several contexts may share a
+    device, each used by one host thread at a time (bifdiagram.py runs sibling branches so, each on a `replicate`)."""
 
     def __init__(self, kind, dims, lengths=(1.0, 1.0, 1.0), krylov_m=100, device=0, params=None, complex=False):
         self.lib = _l.load()
+        # the vector pool, for a DeviceVec collected on another thread.  Reentrant: a cyclic collection may run, on the thread
+        # that holds the lock, between the Python steps around an allocation and finalise a DeviceVec of this context (the
+        # library call itself has returned by then, so the pool is never entered twice at once)
+        self._vec_lock = threading.RLock()
+        self._args = dict(kind=kind, dims=tuple(dims), lengths=tuple(lengths), krylov_m=krylov_m, device=device, complex=complex)
+        self.precond_calls = []             # the last precond_setup of each kind, (kind, a0, a1, params), in call order
         if complex:
             kind |= _l.BK_COMPLEX  # vectors [re; im] of length 2 N0, shifts a0 + i a0_imag (include/bk200.h)
         d = (C.c_int64 * 3)(*(list(dims) + [1, 1, 1])[:3])
@@ -63,10 +71,34 @@ class Context:
         if params is not None:
             self.set_params(params)
 
+    def replicate(self):
+        """A new context of the same kind, dims, lengths, krylov_m, device and params, with the preconditioner set-up of this one
+        replayed in the same order, each at the params it was made with (a set-up may read them, BK_PC_POTRAP_CIRC does): the
+        same problem on its own stream and workspace, whose results are the bits of this context's (every reduction order
+        depends on the grid only)."""
+        new = Context(params=self.params, **self._args)
+        for kind, a0, a1, params in self.precond_calls:
+            if params is not None:
+                new.set_params(params)
+            new.precond_setup(kind, a0, a1)
+        if self.params is not None:
+            new.set_params(self.params)
+        if "pin_host" in self.__dict__:
+            new.pin_host = self.pin_host
+        return new
+
+    def copy_from(self, v):
+        """A DeviceVec of this context holding the values of v, a DeviceVec of any context on the same device: one device-to-device
+        copy on this context's stream (bk_vec_copy takes any device pointer).  v's context must have finished writing v (sync)."""
+        out = DeviceVec(self, v.n)
+        _chk(self, self.lib.bk_vec_copy(self.handle, out.dptr, v.dptr, v.n))
+        return out
+
     def close(self):
         if getattr(self, "handle", None):
-            self.lib.bk_ctx_destroy(self.handle)
-            self.handle = None
+            with self._vec_lock:
+                h, self.handle = self.handle, None   # a DeviceVec finalised from here on frees nothing
+                self.lib.bk_ctx_destroy(h)
 
     def __del__(self):
         try:
@@ -243,6 +275,9 @@ class Context:
 
     def precond_setup(self, kind, a0=1.0, a1=1.0):
         _chk(self, self.lib.bk_precond_setup(self.handle, kind, a0, a1))
+        # a set-up replaces the previous one of its kind, so only the last of each kind is kept (continuation_fold_po re-sets
+        # the preconditioner at every accepted point)
+        self.precond_calls = [c for c in self.precond_calls if c[0] != kind] + [(kind, a0, a1, self.params)]
 
     def precond_apply(self, x, out=None):
         out = self._like(x) if out is None else out
@@ -264,13 +299,16 @@ class DeviceVec:
     def __init__(self, ctx, n):
         self.ctx, self.n = ctx, int(n)
         p = C.c_void_p()
-        _chk(ctx, ctx.lib.bk_vec_alloc(ctx.handle, self.n, C.byref(p)))
+        with ctx._vec_lock:
+            _chk(ctx, ctx.lib.bk_vec_alloc(ctx.handle, self.n, C.byref(p)))
         self.dptr = p.value
 
     def __del__(self):
         try:
-            if self.dptr and self.ctx.handle:
-                self.ctx.lib.bk_vec_free(self.ctx.handle, self.dptr)
+            if self.dptr:
+                with self.ctx._vec_lock:
+                    if self.ctx.handle:
+                        self.ctx.lib.bk_vec_free(self.ctx.handle, self.dptr)
         except Exception:
             pass
         self.dptr = None

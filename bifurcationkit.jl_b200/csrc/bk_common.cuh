@@ -346,8 +346,9 @@ static inline cudaError_t bk_launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
-  static int no_pdl = -1;  // BK_NO_PDL=1: plain stream order (diagnostics)
-  if (no_pdl < 0) no_pdl = getenv("BK_NO_PDL") ? 1 : 0;
+  // BK_NO_PDL=1: plain stream order (diagnostics); read once, by whichever thread launches first (a static local's
+  // initialisation is thread-safe, so contexts driven from several host threads do not race on it)
+  static const int no_pdl = getenv("BK_NO_PDL") ? 1 : 0;
   cfg.numAttrs = pdl && !no_pdl ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }

@@ -89,11 +89,10 @@ static Plan2 plan2(bk_ctx* c, long long units_of_256, size_t scratch_bytes_per_E
   }
   if (force_E) E = force_E;
   {
-    static int env_e = -1;
-    if (env_e < 0) {
+    static const int env_e = [] {  // read once; thread-safe initialisation
       const char* a = getenv("BK2_E");
-      env_e = a ? atoi(a) : 0;
-    }
+      return a ? atoi(a) : 0;
+    }();
     if (env_e >= 1 && env_e <= BK2_EMAX) E = env_e;  // tuning override
   }
   p.E = (int)E;

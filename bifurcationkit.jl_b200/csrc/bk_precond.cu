@@ -205,18 +205,16 @@ static int upload(bk_ctx* c, void** dst, const void* src, size_t bytes) {
 // GMRES loop, where more warps per SM hide the latencies that the neighbouring kernels' PDL overlap does not (an isolated
 // kernel can favour a larger E).  BK_FFT_LOGE overrides (2..5).
 static int fast_loge(long long n) {
-  static int e = -1;
-  if (e < 0) {
+  static const int e = [] {  // read once; thread-safe initialisation
     const char* a = getenv("BK_FFT_LOGE");
-    e = a ? atoi(a) : 0;
-    if (e < 2 || e > 5) e = 0;
-  }
+    const int v = a ? atoi(a) : 0;
+    return v < 2 || v > 5 ? 0 : v;
+  }();
   if (e) return e;
   return n >= 1024 ? 3 : 2;
 }
 static int fast_logn(long long n) {
-  static int off = -1;
-  if (off < 0) off = getenv("BK_FFT_NO_FAST") ? 1 : 0;  // diagnostics: force the general kernel everywhere
+  static const int off = getenv("BK_FFT_NO_FAST") ? 1 : 0;  // diagnostics: force the general kernel everywhere; read once
   if (off) return 0;
   for (int l = fast_loge(n) + 1; l <= 11; ++l)
     if (l >= 6 && n == (1LL << l)) return l;

@@ -26,8 +26,8 @@ Branch switching from a Hopf point to periodic orbits is in periodic.py.  The N-
 product of a jet with ζ★ᵢ in one `bk_jet_moments` pass (prob.jet_moments); host problems get the same contractions from a jet
 call and a dot product per tuple (jet_moments_composed).
 
-Not here: the generic BranchPoint predictor (_predictor, src/NormalForms.jl:496-535), usedeflation = false, bothside and
-bifurcationdiagram; higher codimension normal forms.
+Not here: the generic BranchPoint predictor (_predictor, src/NormalForms.jl:496-535), usedeflation = false and bothside;
+higher codimension normal forms.  bifurcationdiagram, which chains these calls, is bifdiagram.py.
 """
 import itertools
 from dataclasses import dataclass, replace

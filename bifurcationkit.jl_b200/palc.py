@@ -12,6 +12,7 @@ vector interface ``V`` and never touches elements.
 import copy
 from dataclasses import dataclass, field
 import math
+import threading
 
 import numpy as np
 
@@ -69,15 +70,18 @@ class V:
     def dot(x, y):
         return x.dot(y) if _obj(x) else float(np.dot(x, y))
 
-    _scratch = {}  # host path: one reusable buffer per vector length (an 8 MB temporary per call costs ~1 ms of page faults)
+    # host path: one reusable buffer per vector length and thread (an 8 MB temporary per call costs ~1 ms of page faults; a
+    # buffer shared between threads would mix the differences of two branches continued at once)
+    _scratch = threading.local()
 
     @staticmethod
     def diffdot(x, x0, tau):
         if _obj(x):
             return x.diffdot(x0, tau)
-        buf = V._scratch.get(len(x))
+        bufs = V._scratch.__dict__
+        buf = bufs.get(len(x))
         if buf is None:
-            buf = V._scratch[len(x)] = np.empty(len(x))
+            buf = bufs[len(x)] = np.empty(len(x))
         return float(np.dot(np.subtract(x, x0, out=buf), tau))
 
     @staticmethod
@@ -162,6 +166,16 @@ class BifurcationProblemB200:
         self.ctx, self.u0, self.params, self.lens, self.delta = ctx, u0, list(params), lens, delta
         self.p0 = float(params[lens])
         self.record = record or V.norm2  # record_from_solution default = norm(x) (src/Problems.jl:286)
+
+    def replicate(self, ctx=None):
+        """The same problem (u0, params, lens, record, delta) on ctx, by default a new self.ctx.replicate(); a device u0 is copied
+        onto ctx, which must then be able to read it (Context.copy_from).  Refused for subclasses, which may carry more state on
+        their context (periodic.TrapezeProblemB200: its section and update hook) than this copies."""
+        if type(self) is not BifurcationProblemB200:
+            raise NotImplementedError(f"replicate: {type(self).__name__} is not supported (only BifurcationProblemB200 itself)")
+        ctx = self.ctx.replicate() if ctx is None else ctx
+        u0 = ctx.copy_from(self.u0) if isinstance(self.u0, DeviceVec) else copy.copy(self.u0)
+        return BifurcationProblemB200(ctx, u0, self.params, self.lens, self.record, self.delta)
 
     def _set(self, p):
         q = list(self.params)
