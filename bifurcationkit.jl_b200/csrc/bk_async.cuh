@@ -33,6 +33,26 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned by
                "l"(src), "r"(bytes), "r"(bk2_smem(bar))
                : "memory");
 }
+// L2 eviction priorities for the cache-hint form of bulk_g2s: evict_first for data read once, evict_last for data the next
+// kernel reads again
+__device__ __forceinline__ unsigned long long l2_evict_first() {
+  unsigned long long p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ unsigned long long l2_evict_last() {
+  unsigned long long p;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* bar,
+                                         unsigned long long policy) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+          bk2_smem(dst)),
+      "l"(src), "r"(bytes), "r"(bk2_smem(bar)), "l"(policy)
+      : "memory");
+}
 // TMA bulk copy shared -> global (bulk async-group completion); the source must stay valid until bulk_store_wait_read()
 __device__ __forceinline__ void bulk_s2g(void* dst, const void* src, unsigned bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(bk2_smem(src)), "r"(bytes) : "memory");

@@ -158,6 +158,7 @@ struct BkEventTimer {
 struct bk_ctx {
   int device = 0;
   int nsm = BK_NSM_FALLBACK;
+  long long l2_bytes = 0;     // L2 cache size of the device (plan2: how many basis vectors a ring pass keeps in L2)
   cudaStream_t stream = nullptr;
   int kind = 0;
   long long dims[3] = {1, 1, 1};

@@ -123,6 +123,7 @@ extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dim
   cudaDeviceProp prop;
   BK_CUDA(c, cudaGetDeviceProperties(&prop, device));
   c->nsm = prop.multiProcessorCount;
+  c->l2_bytes = prop.l2CacheSize;
   if (const char* e = getenv("BK_NSM")) {  // diagnostics: size grids and reductions as for a device with BK_NSM SMs
     const int v = atoi(e);
     if (v >= 1 && v <= 1024) c->nsm = v;

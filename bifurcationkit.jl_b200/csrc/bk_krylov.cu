@@ -63,7 +63,7 @@ static __global__ void __launch_bounds__(BK_THREADS) k_lincomb(double* __restric
 // ------------------------------------------------------------------------------------------------ v2 (TMA ring) planning
 #define BK2_BLOCKS_PER_SM 4
 struct Plan2 {
-  int E, grid, NS, sred_off;
+  int E, grid, NS, sred_off, keep;
   size_t smem;
 };
 // per-CTA dynamic shared memory budget that still lets BK2_BLOCKS_PER_SM CTAs share one SM (228 KB, 1 KB reserved per CTA)
@@ -110,6 +110,9 @@ static Plan2 plan2(bk_ctx* c, long long units_of_256, size_t scratch_bytes_per_E
   lo = (lo + 127) / 128 * 128;
   p.sred_off = (int)(lo / sizeof(double));
   p.smem = lo + sred;
+  // basis vectors at the end of a ring pass that stay in L2 (evict_last) for the next pass, which starts with them: half of
+  // the L2; the other half holds w, the pass's output vector and the kernels in between (the preconditioner's transforms)
+  p.keep = (int)(c->l2_bytes / 2 / (units_of_256 * BK2_ROW * (long long)sizeof(double)));
   return p;
 }
 static size_t sh2_scratch_bytes(int E) { return sizeof(double) * (size_t)((BK2_ROW + 4) * (E + 4) + (BK2_ROW + 2) * (E + 2)); }
@@ -149,7 +152,7 @@ static int launch_fused(bk_ctx* c, const OpDesc& op, const double* in, const dou
   BK2_DISPATCH(p.E, {
     auto kern = op.bordered ? k2_fused<EE, true> : k2_fused<EE, false>;
     return bk_launch(c, kern, dim3(p.grid), dim3(BK2_THREADS), p.smem, op, in, sp, w, c->V, c->ld, j, c->scales, c->partials,
-                     c->counters + 0, hcol, c->gcoef, p.NS, p.sred_off);
+                     c->counters + 0, hcol, c->gcoef, p.keep, p.NS, p.sred_off);
   });
 }
 
@@ -161,7 +164,7 @@ int bk_launch_dots(bk_ctx* c, const double* basis, const double* scales, const d
   Plan2 p = plan2(c, (n + BK2_ROW - 1) / BK2_ROW, nullptr);
   BK_CHECK(c, p.grid <= c->gmax, "partial-sum workspace too small");
   BK2_DISPATCH(p.E, return bk_launch(c, k2_dots<EE>, dim3(p.grid), dim3(BK2_THREADS), p.smem, w, n, basis, c->ld, j, scales,
-                                     c->partials, c->counters + 1, hcol, gcoef, p.NS, p.sred_off));
+                                     c->partials, c->counters + 1, hcol, gcoef, p.keep, p.NS, p.sred_off));
 }
 static int launch_dots(bk_ctx* c, const double* w, long long n, int j, double* hcol) {
   return bk_launch_dots(c, c->V, c->scales, w, n, j, hcol, c->gcoef);
@@ -172,7 +175,7 @@ int bk_launch_update(bk_ctx* c, const double* basis, const double* gcoef, const 
   Plan2 p = plan2(c, (n + BK2_ROW - 1) / BK2_ROW, nullptr);
   BK_CHECK(c, p.grid <= c->gmax, "partial-sum workspace too small");
   BK2_DISPATCH(p.E, return bk_launch(c, k2_update<EE>, dim3(p.grid), dim3(BK2_THREADS), p.smem, w, n, basis, c->ld, j, gcoef, vout,
-                                     c->partials, c->counters + 2, h_out, scale_out, p.NS));
+                                     c->partials, c->counters + 2, h_out, scale_out, p.keep, p.NS));
 }
 static int launch_update(bk_ctx* c, const double* w, long long n, int j, double* vout, double* h_out, double* scale_out) {
   return bk_launch_update(c, c->V, c->gcoef, w, n, j, vout, h_out, scale_out);

@@ -48,9 +48,11 @@ __device__ __forceinline__ void ring_init(Ring* rg, int NS) {
 // REV: the basis is traversed from V_{j-1} down to V_0.  Pass 1 (dots) runs forward and pass 2 (update) backward, so each
 // pass starts with the vectors the previous pass touched last, which may still be in the L2 (50 MB on an H100: the last few
 // 8 MB basis vectors at 1024^2); with both passes forward the LRU order evicts exactly what is needed next.
+// keep: the last `keep` vectors of the pass are read with L2 evict_last, all others with evict_first, so that the vectors the
+// next pass starts with survive the rest of this pass and the kernels in between (plan2 sizes keep from the L2).
 template <int E, int MODE, bool REV = false>
-__device__ __forceinline__ void stream_basis(const Tile2& tl, const double* __restrict__ V, long long ld, int j, double* ring,
-                                             int NS, Ring* rg, double (&val)[E], double* sred,
+__device__ __forceinline__ void stream_basis(const Tile2& tl, const double* __restrict__ V, long long ld, int j, int keep,
+                                             double* ring, int NS, Ring* rg, double (&val)[E], double* sred,
                                              const double* __restrict__ gcoef) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8) {
@@ -60,17 +62,20 @@ __device__ __forceinline__ void stream_basis(const Tile2& tl, const double* __re
       const unsigned last_b = (unsigned)(((tl.last_len + 1) & ~1) * 8);
       const bool contiguous = (tl.rs == BK2_ROW) && (tl.len == BK2_ROW);
       const unsigned total = row_b * (unsigned)(tl.rows - 1) + last_b;
+      const unsigned long long pol_first = l2_evict_first(), pol_last = l2_evict_last();
       for (int i = 0; i < j; ++i) {
         const int s = i % NS, round = i / NS;
         if (round > 0) mbar_wait(&rg->empty[s], (unsigned)((round - 1) & 1));
         mbar_arrive_expect_tx(&rg->full[s], total);
         const double* src = V + (long long)(REV ? j - 1 - i : i) * ld + tl.base;
         double* dst = ring + (size_t)s * (E * BK2_ROW);
+        const unsigned long long pol = i >= j - keep ? pol_last : pol_first;
         if (contiguous) {
-          bulk_g2s(dst, src, total, &rg->full[s]);
+          bulk_g2s(dst, src, total, &rg->full[s], pol);
         } else {
-          for (int r = 0; r < tl.rows - 1; ++r) bulk_g2s(dst + r * BK2_ROW, src + (long long)r * tl.rs, row_b, &rg->full[s]);
-          bulk_g2s(dst + (tl.rows - 1) * BK2_ROW, src + (long long)(tl.rows - 1) * tl.rs, last_b, &rg->full[s]);
+          for (int r = 0; r < tl.rows - 1; ++r)
+            bulk_g2s(dst + r * BK2_ROW, src + (long long)r * tl.rs, row_b, &rg->full[s], pol);
+          bulk_g2s(dst + (tl.rows - 1) * BK2_ROW, src + (long long)(tl.rows - 1) * tl.rs, last_b, &rg->full[s], pol);
         }
       }
     }
@@ -227,6 +232,19 @@ __device__ __forceinline__ void sh2_tile_eval(const OpDesc& op, const double* __
   double* qs = scratch + S::V_ELEMS;
   const int nx = op.nx, ny = op.ny;
   const int len = min(BK2_ROW, nx - x0);
+  const int t = threadIdx.x;
+  const double l = op.par[0], nu = op.par[1];
+  const int gx = x0 + t;
+  const bool colok = t < BK2_ROW && gx < nx;
+  const int rows = min(E, ny - y0);
+  // Epilogue in sub-passes so that each issues E independent global loads before the first use (the first version mixed the
+  // loads of u, a, b with the arithmetic row by row and stalled on each of them).  The u rows do not depend on the tile, so
+  // their loads are issued before the tile wait and arrive while the tile and the q pass are in progress.
+  double g[E];
+  if (!RESID) {
+#pragma unroll
+    for (int e = 0; e < E; ++e) g[e] = (colok && e < rows) ? __ldg(op.u + gx + (long long)(y0 + e) * nx) : 0.0;
+  }
   if (threadIdx.x < 4 * S::VY) {
     const int jj = threadIdx.x >> 2, h = threadIdx.x & 3;
     const int i = h < 2 ? h : len + h;  // 0, 1, len + 2, len + 3
@@ -247,18 +265,6 @@ __device__ __forceinline__ void sh2_tile_eval(const OpDesc& op, const double* __
     qs[q] = c0 + op.cx * (p[-1] - 2.0 * c0 + p[1]) + op.cy * (p[-S::VX] - 2.0 * c0 + p[S::VX]);
   }
   __syncthreads();
-  const int t = threadIdx.x;
-  const double l = op.par[0], nu = op.par[1];
-  const int gx = x0 + t;
-  const bool colok = t < BK2_ROW && gx < nx;
-  const int rows = min(E, ny - y0);
-  // Epilogue in sub-passes so that each issues E independent global loads before the first use (the first version mixed the
-  // loads of u, a, b with the arithmetic row by row and stalled on each of them).
-  double g[E];
-  if (!RESID) {
-#pragma unroll
-    for (int e = 0; e < E; ++e) g[e] = (colok && e < rows) ? __ldg(op.u + gx + (long long)(y0 + e) * nx) : 0.0;
-  }
 #pragma unroll
   for (int e = 0; e < E; ++e) {
     double r = 0.0;
@@ -297,7 +303,7 @@ static __global__ void __launch_bounds__(BK2_THREADS, 4) k2_fused(OpDesc op, con
                                                                   long long ld, int j, const double* __restrict__ scales,
                                                                   double* __restrict__ partials, unsigned int* counter,
                                                                   double* __restrict__ hcol, double* __restrict__ gcoef,
-                                                                  int NS, int sred_off) {
+                                                                  int keep, int NS, int sred_off) {
   extern __shared__ __align__(128) double smem2[];
   __shared__ Ring rg;
   __shared__ __align__(8) unsigned long long tbar;
@@ -321,7 +327,8 @@ static __global__ void __launch_bounds__(BK2_THREADS, 4) k2_fused(OpDesc op, con
   const double s = in_scale_ptr ? __ldg(in_scale_ptr) : 1.0;
   if (threadIdx.x == BK2_CONS) {
     sh2_tile_issue<E>(op, in, x0, y0, smem2, &tbar);
-    // pull what the stencil epilogue and the first ring rounds will read into L2 while the tile is in flight
+    // pull what the stencil epilogue will read into L2 while the tile is in flight.  No basis tiles: the first ones are still
+    // in L2 from k2_update (evict_last), and prefetching more of them only competes with the prologue for HBM
     const unsigned row_b = (unsigned)(((tl.len + 1) & ~1) * 8);
     for (int r = 0; r < tl.rows; ++r) {
       const long long o = tl.base + (long long)r * tl.rs;
@@ -331,21 +338,19 @@ static __global__ void __launch_bounds__(BK2_THREADS, 4) k2_fused(OpDesc op, con
         bulk_prefetch_l2(op.bb + o, row_b);
       }
     }
-    const int npf = j < 2 * NS ? j : 2 * NS;
-    for (int i = 0; i < npf; ++i)
-      for (int r = 0; r < tl.rows; ++r) bulk_prefetch_l2(V + (long long)i * ld + tl.base + (long long)r * tl.rs, row_b);
   }
   const double xp = BORDERED ? s * __ldg(in + op.N) : 0.0;
   double bsum = 0.0;
   sh2_tile_eval<E, BORDERED>(op, in, s, x0, y0, smem2, &tbar, val, xp, &bsum);
+  fence_proxy_async_smem();  // generic-proxy accesses to the scratch are ordered before the TMA writes that reuse it
+  __syncthreads();           // scratch is dead, barriers are initialised: the ring takes over the shared memory
+  stream_basis<E, 0>(tl, V, ld, j, keep, ring, NS, &rg, val, sred, nullptr);
+  // w is stored after the basis stream (val is unchanged by it), so that it is still in L2 when k2_update reads it
   if (threadIdx.x < tl.len) {
 #pragma unroll
     for (int e = 0; e < E; ++e)
       if (e < tl.rows) w[tl.base + (long long)e * tl.rs + threadIdx.x] = val[e];
   }
-  fence_proxy_async_smem();  // generic-proxy accesses to the scratch are ordered before the TMA writes that reuse it
-  __syncthreads();           // scratch is dead, barriers are initialised: the ring takes over the shared memory
-  stream_basis<E, 0>(tl, V, ld, j, ring, NS, &rg, val, sred, nullptr);
   if (BORDERED) {
     __shared__ double s_wp;
     bsum = bk_warp_sum(bsum);  // bsum already carries the input scale (v = s * in)
@@ -417,8 +422,8 @@ static __global__ void __launch_bounds__(BK2_THREADS, 4) k2_dots(const double* _
                                                                  const double* __restrict__ V, long long ld, int j,
                                                                  const double* __restrict__ scales,
                                                                  double* __restrict__ partials, unsigned int* counter,
-                                                                 double* __restrict__ hcol, double* __restrict__ gcoef, int NS,
-                                                                 int sred_off) {
+                                                                 double* __restrict__ hcol, double* __restrict__ gcoef, int keep,
+                                                                 int NS, int sred_off) {
   extern __shared__ __align__(128) double smem2[];
   __shared__ Ring rg;
   __shared__ int s_flag;
@@ -434,7 +439,7 @@ static __global__ void __launch_bounds__(BK2_THREADS, 4) k2_dots(const double* _
     val[e] = (threadIdx.x < BK2_ROW && e < tl.rows && (int)threadIdx.x < lim) ? w[tl.base + e * BK2_ROW + threadIdx.x] : 0.0;
   }
   __syncthreads();
-  stream_basis<E, 0>(tl, V, ld, j, ring, NS, &rg, val, sred, nullptr);
+  stream_basis<E, 0>(tl, V, ld, j, keep, ring, NS, &rg, val, sred, nullptr);
   __syncthreads();
   dots_finish(j, sred, scales, partials, counter, hcol, gcoef, &s_flag);
 }
@@ -445,7 +450,7 @@ static __global__ void __launch_bounds__(BK2_THREADS, 4) k2_update(const double*
                                                                    const double* __restrict__ gcoef, double* vout,
                                                                    double* __restrict__ partials, unsigned int* counter,
                                                                    double* __restrict__ h_out, double* __restrict__ scale_out,
-                                                                   int NS) {
+                                                                   int keep, int NS) {
   extern __shared__ __align__(128) double smem2[];
   __shared__ Ring rg;
   __shared__ double s_w[9];
@@ -462,7 +467,7 @@ static __global__ void __launch_bounds__(BK2_THREADS, 4) k2_update(const double*
     val[e] = (t < BK2_ROW && e < tl.rows && t < lim) ? w[tl.base + e * BK2_ROW + t] : 0.0;
   }
   __syncthreads();
-  stream_basis<E, 1, true>(tl, V, ld, j, ring, NS, &rg, val, nullptr, gcoef);
+  stream_basis<E, 1, true>(tl, V, ld, j, keep, ring, NS, &rg, val, nullptr, gcoef);
   double acc = 0.0;
   if (t < BK2_ROW) {
 #pragma unroll

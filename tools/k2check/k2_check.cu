@@ -73,7 +73,7 @@ static void run(long long n, int j, int NS, int reps, int pdl) {
   if (pdl) setenv("BK_NO_PDL", "1", 0);
   for (int rep = 0; rep < reps; ++rep) {
     CK(cudaMemset(out, 0, 8 * ld)); CK(cudaMemset(bad, 0, 4 * (size_t)G)); CK(cudaMemset(first, 0x7f, 8 * (size_t)G));
-    CK(bk_launch_pdl(k2_update<E>, dim3(G), dim3(BK2_THREADS), smem, 0, true, (const double*)w, n, (const double*)V, ld, j, (const double*)g, out, partials, counter, hout, hout + 1, NS));
+    CK(bk_launch_pdl(k2_update<E>, dim3(G), dim3(BK2_THREADS), smem, 0, true, (const double*)w, n, (const double*)V, ld, j, (const double*)g, out, partials, counter, hout, hout + 1, 0, NS));
     CK(cudaDeviceSynchronize());
     k_cmp<<<2048, 256>>>(out, ref, n, tile, bad, first);
     CK(cudaDeviceSynchronize());
@@ -86,7 +86,7 @@ static void run(long long n, int j, int NS, int reps, int pdl) {
     for (int t = 0; t < G && shown < 12; ++t) if (hb[t]) { printf(" [cta %d n=%u first=%lld]", t, hb[t], hf[t]); ++shown; }
     printf("\n");
     // dots: compare per-CTA partials with per-tile reference
-    CK(bk_launch_pdl(k2_dots<E>, dim3(G), dim3(BK2_THREADS), smem, 0, true, (const double*)w, n, (const double*)V, ld, j, (const double*)scales, partials, counter + 1, hcol, gcoef, NS, (int)(ring / 8)));
+    CK(bk_launch_pdl(k2_dots<E>, dim3(G), dim3(BK2_THREADS), smem, 0, true, (const double*)w, n, (const double*)V, ld, j, (const double*)scales, partials, counter + 1, hcol, gcoef, 0, NS, (int)(ring / 8)));
     CK(cudaDeviceSynchronize());
     std::vector<double> hp((size_t)j * G), hr((size_t)G * j);
     CK(cudaMemcpy(hp.data(), partials, 8 * (size_t)j * G, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(hr.data(), refd, 8 * (size_t)G * j, cudaMemcpyDeviceToHost));
@@ -103,12 +103,12 @@ static void run(long long n, int j, int NS, int reps, int pdl) {
     const int T = 20;
     cudaEventRecord(e0);
     for (int r = 0; r < T; ++r)
-      bk_launch_pdl(k2_update<E>, dim3(G), dim3(BK2_THREADS), smem, 0, true, (const double*)w, n, (const double*)V, ld, j, (const double*)g, out, partials, counter, hout, hout + 1, NS);
+      bk_launch_pdl(k2_update<E>, dim3(G), dim3(BK2_THREADS), smem, 0, true, (const double*)w, n, (const double*)V, ld, j, (const double*)g, out, partials, counter, hout, hout + 1, 0, NS);
     cudaEventRecord(e1); CK(cudaDeviceSynchronize());
     float mu = 0; cudaEventElapsedTime(&mu, e0, e1);
     cudaEventRecord(e0);
     for (int r = 0; r < T; ++r)
-      bk_launch_pdl(k2_dots<E>, dim3(G), dim3(BK2_THREADS), smem, 0, true, (const double*)w, n, (const double*)V, ld, j, (const double*)scales, partials, counter + 1, hcol, gcoef, NS, (int)(ring / 8));
+      bk_launch_pdl(k2_dots<E>, dim3(G), dim3(BK2_THREADS), smem, 0, true, (const double*)w, n, (const double*)V, ld, j, (const double*)scales, partials, counter + 1, hcol, gcoef, 0, NS, (int)(ring / 8));
     cudaEventRecord(e1); CK(cudaDeviceSynchronize());
     float md = 0; cudaEventElapsedTime(&md, e0, e1);
     const double bu = 8.0 * n * (j + 2), bd = 8.0 * n * (j + 1);
