@@ -294,6 +294,9 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
                                         double* vals_im, double* vecs, int32_t* nconv, int32_t* nops) {
   BK_ENTER(c);
   BkRange nvtx_range("bk_eigs_shift_invert");
+  // the operator of a complex context is the real-equivalent form of ((-sigma + i a0_imag) I + J): neither symmetric for the
+  // thick restart nor mapped back by lambda = sigma + 1/theta, and every eigenvalue of J would come out twice
+  BK_CHECK(c, !c->cplx, "bk_eigs_shift_invert: not available in a BK_COMPLEX context");
   BK_CHECK(c, c->have_state, "bk_jac_set_state must be called first");
   BK_CHECK(c, inner != nullptr && vals_re && vals_im, "null argument");
   const long long n = c->N;
@@ -353,18 +356,12 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
     int kstart = 0;
     for (int rs = 0; rs < maxrestart && !converged; ++rs) {
       BK_TRY(arnoldi_expand(c, ws, op, inner, x, n, m, kstart, H, &keff, &total_ops));
-      // symmetrised projected matrix (exactly symmetric in exact arithmetic)
+      // symmetrised projected matrix (exactly symmetric in exact arithmetic), mirrored from the upper triangle of H.  After a
+      // restart the retained Ritz values sit on the diagonal of columns 0..kstart-1, and the arrow <Q_q, Op q_kstart> that couples
+      // them to the residual direction is column kstart's Gram-Schmidt coefficients, so the lower triangle is never needed.
       std::vector<double> A((size_t)keff * keff);
       for (int jj = 0; jj < keff; ++jj)
-        for (int i = 0; i < keff; ++i) {
-          double hij = (i <= jj + 1 || jj < kstart) ? H[i + (size_t)jj * (m + 1)] : 0.0;
-          double hji = (jj <= i + 1 || i < kstart) ? H[jj + (size_t)i * (m + 1)] : 0.0;
-          // below-diagonal entries of Arnoldi columns other than the sub-diagonal are zero; the arrow row of a
-          // restarted factorisation is stored in row kstart of the retained columns
-          A[i + (size_t)jj * keff] = (i == jj) ? hij : ((i < jj) ? hij : hji);
-        }
-      for (int jj = 0; jj < keff; ++jj)
-        for (int i = jj + 1; i < keff; ++i) A[i + (size_t)jj * keff] = A[jj + (size_t)i * keff];
+        for (int i = 0; i < keff; ++i) A[i + (size_t)jj * keff] = H[std::min(i, jj) + (size_t)std::max(i, jj) * (m + 1)];
       jacobi_eig(A, keff, wsym, Ssym);
       order.resize(keff);
       for (int i = 0; i < keff; ++i) order[i] = i;
@@ -393,16 +390,8 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
         }
         BK_TRY(bk_dev_copy(c, c->Q2 + (size_t)pkeep * c->ld, c->Q + (size_t)keff * c->ld, n));  // residual direction q_{m+1}
         BK_CUDA(c, cudaMemcpyAsync(c->Q, c->Q2, 8 * (size_t)c->ld * (pkeep + 1), cudaMemcpyDeviceToDevice, c->stream));
-        std::vector<double> bnew(pkeep), thnew(pkeep);
-        for (int q = 0; q < pkeep; ++q) {
-          thnew[q] = wsym[order[q]];
-          bnew[q] = hlast * Ssym[(keff - 1) + (size_t)order[q] * keff];
-        }
         std::fill(H.begin(), H.end(), 0.0);
-        for (int q = 0; q < pkeep; ++q) {
-          H[q + (size_t)q * (m + 1)] = thnew[q];
-          H[pkeep + (size_t)q * (m + 1)] = bnew[q];
-        }
+        for (int q = 0; q < pkeep; ++q) H[q + (size_t)q * (m + 1)] = wsym[order[q]];
         kstart = pkeep;
       }
     }
@@ -413,6 +402,17 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
     BK_TRY(arnoldi_expand(c, ws, op, inner, x, n, m, 0, H, &keff, &total_ops));
     // Ritz values / vectors of H(keff x keff)
     BK_CHECK(c, hess_eigvals(H, keff, m + 1, ev), "QR iteration on the Hessenberg matrix did not converge");
+    // the complex QR returns the members of a conjugate pair with moduli that differ in the last bits: make them exact
+    // conjugates, so that the tie rule below, and not rounding, decides which member an nev cutting the pair keeps
+    for (int i = 0; i < keff; ++i) {
+      if (!(ev[i].imag() > 0)) continue;
+      int jb = -1;
+      for (int j = 0; j < keff; ++j)
+        if (ev[j].imag() < 0 && (jb < 0 || std::abs(ev[j] - std::conj(ev[i])) < std::abs(ev[jb] - std::conj(ev[i])))) jb = j;
+      if (jb < 0) continue;
+      const double d = std::abs(ev[jb] - std::conj(ev[i]));
+      if (d <= 1e-8 * std::abs(ev[i]) && d < ev[i].imag()) ev[jb] = std::conj(ev[i]);
+    }
     std::sort(ev.begin(), ev.end(), [](const cplx& a, const cplx& b) {
       double da = std::abs(a), db = std::abs(b);
       if (da != db) return da > db;

@@ -225,7 +225,8 @@ int32_t bk_bls_block_map(bk_ctx* ctx, int32_t m, const double* const* a, const d
 
 /* ---- S10: shift-invert Arnoldi (src/EigSolver.jl:246-266; inner solver = bk_gmres with a0=-sigma)
  *   vals sorted by decreasing real part; vecs (N x nev, column-major, real Schur/Ritz vectors; complex pairs
- *   as (re, im) consecutive columns) may be NULL. */
+ *   as (re, im) consecutive columns) may be NULL.  BK_COMPLEX contexts: BK_ERR_ARG before any launch (J is real: take its
+ *   eigenpairs on a real context of the same grid). */
 int32_t bk_eigs_shift_invert(bk_ctx* ctx, double sigma, int32_t nev, int32_t krylovdim, double tol, int32_t maxrestart,
                              const bk_gmres_opts* inner, const double* v0, double* vals_re, double* vals_im, double* vecs,
                              int32_t* nconv, int32_t* nops);
