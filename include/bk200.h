@@ -20,6 +20,9 @@
  *   - One context per GPU; a context is not thread-safe; calls are synchronous with respect to
  *     host-visible outputs.
  *   - Layout: Julia column-major, x fastest: u[i + j*Nx (+ k*Nx*Ny)], 0-based here.
+ *   - GMRES reduces ||v||^2 unscaled: a right-hand side (or preconditioned residual) of norm below ~1e-160 underflows to
+ *     beta0 = 0 and the solve returns x = 0 as converged after 0 iterations; one above ~1e154 overflows.  Scale such
+ *     systems before the call.
  */
 #ifndef BK200_H
 #define BK200_H
@@ -77,7 +80,10 @@ typedef struct bk_gmres_opts {
   int32_t restart; /* 200  */
   int32_t maxiter; /* 100  */
   int32_t pc_side; /* BK_SIDE_*: which of Pl / Pr holds the context's preconditioner */
-  int32_t orth;    /* BK_ORTH_CGS (single classical Gram-Schmidt pass) or BK_ORTH_CGS2 */
+  int32_t orth;    /* BK_ORTH_CGS (single classical Gram-Schmidt pass) or BK_ORTH_CGS2.  A single-pass CGS cycle that ends
+                      converged with >= 40 columns or reltol < 1e-9 is re-checked against the true residual (accepted when
+                      <= 4 tol, else the solve continues with CGS2 and counts a cgs_fallback), unless that cycle also
+                      reached maxiter: then `converged` rests on the Givens estimate alone */
   int32_t fused;   /* 0: separate kernels; nonzero: JVP fused into the Arnoldi dot kernel where a fused kernel exists, i.e. real
                       SH2d with an even nx, at most one border (the bordered map), preconditioner not on the left.
                       BK_SH2D_PERIODIC with BK_PC_SH_FFT on either side: operator and preconditioner in ONE transform per
