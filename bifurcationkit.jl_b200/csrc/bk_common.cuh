@@ -81,20 +81,26 @@ struct PerPw {
 };
 #define PW_D 1
 
+// The transform of one dimension of the spectral preconditioners (bk_precond.cu line_setup / line_free)
+struct Line {
+  int n = 0;
+  int type = 0;               // 0: DCT-II (Neumann), 1: DST-I (Dirichlet)
+  double* lam = nullptr;      // 1-D eigenvalues of the Laplacian factor (natural order)
+  // register-resident power-of-two kernels (bk_fft_fast.cuh): log2(n) or 0, and their tables
+  int fast = 0;
+  double2* ftw = nullptr;     // per-pass contiguous FFT twiddles
+  double2* fom = nullptr;     // w_k = exp(-i pi k / 2n), register-major
+  double2* flam2 = nullptr;   // (lambda[k], lambda[n-k]), register-major
+  // general lengths (bk_fft_gen.cuh): the plan points at gwl / gph
+  bkg::Plan plan = {};
+  double2* gwl = nullptr;
+  double2* gph = nullptr;
+};
+
 struct Precond {
   int kind = BK_PC_NONE;
   double a0 = 0, a1 = 0;
-  double* lam[3] = {nullptr, nullptr, nullptr};     // 1-D eigenvalues of the Laplacian factors (natural order)
-  int ttype[3] = {0, 0, 0};                         // 0: DCT-II (Neumann), 1: DST-I (Dirichlet)
-  // register-resident power-of-two kernels (bk_fft_fast.cuh): log2(n) or 0, and their tables
-  int fast[3] = {0, 0, 0};
-  double2* ftw[3] = {nullptr, nullptr, nullptr};    // per-pass contiguous FFT twiddles
-  double2* fom[3] = {nullptr, nullptr, nullptr};    // w_k = exp(-i pi k / 2n), register-major
-  double2* flam2[3] = {nullptr, nullptr, nullptr};  // (lambda[k], lambda[n-k]), register-major
-  // general lengths (bk_fft_gen.cuh)
-  bkg::Plan gplan[3] = {};
-  double2* gwl[3] = {nullptr, nullptr, nullptr};
-  double2* gph[3] = {nullptr, nullptr, nullptr};
+  Line line[3];
   double* work = nullptr;                           // scratch vector (N)
   double* work2 = nullptr;
   // chan tridiagonal LU factors
@@ -289,6 +295,7 @@ int bk_launch_apply(bk_ctx* c, const OpDesc& op, const double* in_dev, const dou
 int bk_potrap_refresh_cache(bk_ctx* c);
 
 int bk_precond_apply_dev(bk_ctx* c, const double* in_dev, double* out_dev, long long n);
+void line_free(Line& ln);
 
 // BK_SH2D_PERIODIC (bk_precond.cu): transform tables and work buffers at bk_ctx_create, then the three-kernel spectral pipeline
 // x r2c -> y (forward, symbol, inverse) -> x c2r for the residual, the JVP and the one-transform preconditioned operator

@@ -184,11 +184,7 @@ extern "C" int32_t bk_ctx_destroy(bk_ctx* c) {
                     c->red_out, c->phi, c->xpi, c->fcache, c->pc.work, c->pc.work2, c->pc.tri, c->Q, c->Q2, c->eig_dev};
   for (double* b : bufs)
     if (b) cudaFree(b);
-  for (int d = 0; d < 3; ++d) {
-    void* tabs[] = {c->pc.lam[d], c->pc.ftw[d], c->pc.fom[d], c->pc.flam2[d], c->pc.gwl[d], c->pc.gph[d]};
-    for (void* t : tabs)
-      if (t) cudaFree(t);
-  }
+  for (Line& ln : c->pc.line) line_free(ln);
   if (c->pc.tdft) cudaFree(c->pc.tdft);
   if (c->counters) cudaFree(c->counters);
   for (auto& kv : c->vec_live) cudaFree(kv.first);

@@ -20,7 +20,6 @@
 //   (bk_jac_set_transpose) it applies the exact transpose P'^-1, so that the J' solves are preconditioned with P'.
 #include <cmath>
 #include <cstdlib>
-#include <utility>
 #include <vector>
 #include "bk_common.cuh"
 
@@ -54,7 +53,11 @@ static __global__ void __launch_bounds__(256) k_helmholtz_symbol_div(double* __r
 // spatial mode: w+- = u1 +- i u2 over the K = M-1 cyclic slices, DFT in time, divide by
 //   s+-_k = (1 - g_k) - h/2 (1 + g_k)(lambda + r +- i nu),   g_k = exp(-2 pi i k/K),
 // inverse DFT, back to (u1, u2).  In place.
+// TR: the same solve with the transposed block circulant (P'^-1 while J' is selected).  Its time blocks are x_k - x_{k+1} (the
+// shift the other way: g_k -> conj g_k) and its reaction block is [[a, nu], [-nu, a]] (nu -> -nu on w+-), so its symbol is
+// conj(s+-_k).  The closure slice M-1 is added to slice 0 first: the transpose of x_M = r_M + x_1.
 #define BK_PO_KMAX 64
+template <bool TR>
 static __global__ void __launch_bounds__(128) k_potrap_time(double* __restrict__ B, long long n, int nx, int K,
                                                             const double* __restrict__ lamx, const double* __restrict__ lamy,
                                                             double h, double r, double nu, const double2* __restrict__ tw) {
@@ -63,7 +66,13 @@ static __global__ void __launch_bounds__(128) k_potrap_time(double* __restrict__
   const double lam = lamx[g % nx] + lamy[g / nx];
   double2 wp[BK_PO_KMAX], wm[BK_PO_KMAX];
   for (int i = 0; i < K; ++i) {
-    const double a = B[(long long)(2 * i) * n + g], b = B[(long long)(2 * i + 1) * n + g];
+    double a = B[(long long)(2 * i) * n + g], b = B[(long long)(2 * i + 1) * n + g];
+    if constexpr (TR) {
+      if (i == 0) {  // + the closure slice M-1 (field pair 2K, 2K+1, transformed with the rest)
+        a += B[(long long)(2 * K) * n + g];
+        b += B[(long long)(2 * K + 1) * n + g];
+      }
+    }
     wp[i] = make_double2(a, b);
     wm[i] = make_double2(a, -b);
   }
@@ -87,67 +96,10 @@ static __global__ void __launch_bounds__(128) k_potrap_time(double* __restrict__
     const double cr = lam + r;
     double2 sp = make_double2(omg.x - 0.5 * h * (opg.x * cr - opg.y * nu), omg.y - 0.5 * h * (opg.x * nu + opg.y * cr));
     double2 sm = make_double2(omg.x - 0.5 * h * (opg.x * cr + opg.y * nu), omg.y - 0.5 * h * (-opg.x * nu + opg.y * cr));
-    const double dp = 1.0 / (sp.x * sp.x + sp.y * sp.y), dm = 1.0 / (sm.x * sm.x + sm.y * sm.y);
-    yp[k] = make_double2((ap.x * sp.x + ap.y * sp.y) * dp * invK, (ap.y * sp.x - ap.x * sp.y) * dp * invK);
-    ym[k] = make_double2((am.x * sm.x + am.y * sm.y) * dm * invK, (am.y * sm.x - am.x * sm.y) * dm * invK);
-  }
-  for (int i = 0; i < K; ++i) {
-    double2 ap = make_double2(0, 0), am = make_double2(0, 0);
-    int idx = 0;
-    for (int k = 0; k < K; ++k) {
-      const double2 t = tw[idx];  // conj -> exp(+2 pi i k i / K)
-      ap.x += yp[k].x * t.x + yp[k].y * t.y;
-      ap.y += yp[k].y * t.x - yp[k].x * t.y;
-      am.x += ym[k].x * t.x + ym[k].y * t.y;
-      am.y += ym[k].y * t.x - ym[k].x * t.y;
-      idx += i;
-      if (idx >= K) idx -= K;
+    if constexpr (TR) {  // the transposed symbols conj(s+-_k)
+      sp.y = -sp.y;
+      sm.y = -sm.y;
     }
-    B[(long long)(2 * i) * n + g] = 0.5 * (ap.x + am.x);      // Re((yp + ym)/2)
-    B[(long long)(2 * i + 1) * n + g] = 0.5 * (ap.y - am.y);  // Re((yp - ym)/(2i)) = Im(yp - ym)/2
-  }
-}
-// k_potrap_time_tr: the same solve with the transposed block circulant (P'^-1 while J' is selected).  Its time blocks are
-// x_k - x_{k+1} (the shift the other way: g_k -> conj g_k) and its reaction block is [[a, nu], [-nu, a]] (nu -> -nu on w+-), so
-// its symbol is conj(s+-_k).  The closure slice M-1 is added to slice 0 first: the transpose of x_M = r_M + x_1.
-static __global__ void __launch_bounds__(128) k_potrap_time_tr(double* __restrict__ B, long long n, int nx, int K,
-                                                               const double* __restrict__ lamx, const double* __restrict__ lamy,
-                                                               double h, double r, double nu, const double2* __restrict__ tw) {
-  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= n) return;
-  const double lam = lamx[g % nx] + lamy[g / nx];
-  double2 wp[BK_PO_KMAX], wm[BK_PO_KMAX];
-  for (int i = 0; i < K; ++i) {
-    double a = B[(long long)(2 * i) * n + g], b = B[(long long)(2 * i + 1) * n + g];
-    if (i == 0) {  // + the closure slice M-1 (field pair 2K, 2K+1, transformed with the rest)
-      a += B[(long long)(2 * K) * n + g];
-      b += B[(long long)(2 * K + 1) * n + g];
-    }
-    wp[i] = make_double2(a, b);
-    wm[i] = make_double2(a, -b);
-  }
-  double2 yp[BK_PO_KMAX], ym[BK_PO_KMAX];
-  const double invK = 1.0 / K;
-  for (int k = 0; k < K; ++k) {
-    double2 ap = make_double2(0, 0), am = make_double2(0, 0);
-    int idx = 0;
-    for (int i = 0; i < K; ++i) {
-      const double2 t = tw[idx];  // exp(-2 pi i k i / K)
-      ap.x += wp[i].x * t.x - wp[i].y * t.y;
-      ap.y += wp[i].x * t.y + wp[i].y * t.x;
-      am.x += wm[i].x * t.x - wm[i].y * t.y;
-      am.y += wm[i].x * t.y + wm[i].y * t.x;
-      idx += k;
-      if (idx >= K) idx -= K;
-    }
-    const double2 gk = tw[k];
-    // s = (1 - g) - h/2 (1 + g) (lam + r +- i nu), then conjugated
-    const double2 omg = make_double2(1.0 - gk.x, -gk.y), opg = make_double2(1.0 + gk.x, gk.y);
-    const double cr = lam + r;
-    double2 sp = make_double2(omg.x - 0.5 * h * (opg.x * cr - opg.y * nu), omg.y - 0.5 * h * (opg.x * nu + opg.y * cr));
-    double2 sm = make_double2(omg.x - 0.5 * h * (opg.x * cr + opg.y * nu), omg.y - 0.5 * h * (-opg.x * nu + opg.y * cr));
-    sp.y = -sp.y;  // the transposed symbols conj(s+-_k)
-    sm.y = -sm.y;
     const double dp = 1.0 / (sp.x * sp.x + sp.y * sp.y), dm = 1.0 / (sm.x * sm.x + sm.y * sm.y);
     yp[k] = make_double2((ap.x * sp.x + ap.y * sp.y) * dp * invK, (ap.y * sp.x - ap.x * sp.y) * dp * invK);
     ym[k] = make_double2((am.x * sm.x + am.y * sm.y) * dm * invK, (am.y * sm.x - am.x * sm.y) * dm * invK);
@@ -237,39 +189,30 @@ static int fast_logn(long long n) {
     default: BKF_DISPATCH_N(5, LOGN, __VA_ARGS__) break;                               \
   }
 
-template <class FC>
-static int fast_setup(bk_ctx* c, int d, const double* lam_host) {
-  std::vector<double> tw, om, lam2;
-  bkf::build_tables<FC>(tw, om, lam2, lam_host);
-  Precond& pc = c->pc;
-  if (tw.empty()) tw.assign(2, 0.0);
-  BK_TRY(upload(c, (void**)&pc.ftw[d], tw.data(), 8 * tw.size()));
-  BK_TRY(upload(c, (void**)&pc.fom[d], om.data(), 8 * om.size()));
-  BK_TRY(upload(c, (void**)&pc.flam2[d], lam2.data(), 8 * lam2.size()));
-  return BK_OK;
-}
-
 // strided: mode 0 forward (2 C), 1 inverse (n x), 2 fused forward + symbol + inverse, 3 periodic fused y pass;
 // contiguous: mode 0 forward, 1 inverse, 2 periodic r2c, 3 periodic c2r (prologue / epilogue pw)
-template <class FC>
-static int fast_launch(bk_ctx* c, int d, bool strided, int mode, const double* in, double* out, const bkf::Geom& g,
+static int fast_launch(bk_ctx* c, const Line& ln, bool strided, int mode, const double* in, double* out, const bkf::Geom& g,
                        const bkf::Symbol* sy, const PerPw* pw = nullptr) {
-  Precond& pc = c->pc;
-  bkf::Tables tb{pc.ftw[d], pc.fom[d], pc.flam2[d]};
+  bkf::Tables tb{ln.ftw, ln.fom, ln.flam2};
   bkf::Symbol s0{};
   if (sy) s0 = *sy;
   PerPw p0{};
   if (pw) p0 = *pw;
-  if (strided) {
-    static decltype(&bkf::k_strided<FC, 0>) const kern[4] = {bkf::k_strided<FC, 0>, bkf::k_strided<FC, 1>, bkf::k_strided<FC, 2>,
-                                                             bkf::k_strided<FC, 3>};
-    const dim3 grid((g.nb + 2 * FC::PP - 1) / (2 * FC::PP), g.nouter);
-    return bk_launch(c, kern[mode], grid, dim3(FC::THREADS), mode >= 2 ? FC::SMEM_FUSED : FC::SMEM, in, out, g, tb, s0);
-  }
-  static decltype(&bkf::k_contig<FC, 0>) const kern[4] = {bkf::k_contig<FC, 0>, bkf::k_contig<FC, 1>, bkf::k_contig<FC, 2>,
-                                                          bkf::k_contig<FC, 3>};
-  const dim3 grid((unsigned)((g.nb + 2 * FC::PP - 1) / (2 * FC::PP)));
-  return bk_launch(c, kern[mode], grid, dim3(FC::THREADS), FC::SMEM, in, out, g, tb, p0);
+  int st;
+  BKF_DISPATCH(ln.fast, {
+    if (strided) {
+      static decltype(&bkf::k_strided<FC, 0>) const kern[4] = {bkf::k_strided<FC, 0>, bkf::k_strided<FC, 1>, bkf::k_strided<FC, 2>,
+                                                               bkf::k_strided<FC, 3>};
+      const dim3 grid((g.nb + 2 * FC::PP - 1) / (2 * FC::PP), g.nouter);
+      st = bk_launch(c, kern[mode], grid, dim3(FC::THREADS), mode >= 2 ? FC::SMEM_FUSED : FC::SMEM, in, out, g, tb, s0);
+    } else {
+      static decltype(&bkf::k_contig<FC, 0>) const kern[4] = {bkf::k_contig<FC, 0>, bkf::k_contig<FC, 1>, bkf::k_contig<FC, 2>,
+                                                              bkf::k_contig<FC, 3>};
+      const dim3 grid((unsigned)((g.nb + 2 * FC::PP - 1) / (2 * FC::PP)));
+      st = bk_launch(c, kern[mode], grid, dim3(FC::THREADS), FC::SMEM, in, out, g, tb, p0);
+    }
+  });
+  return st;
 }
 
 // ---- general path ----------------------------------------------------------------------------------------------------------
@@ -296,12 +239,11 @@ static int gen_ppg(int L) {
   return p;
 }
 
-// type 0: DCT-II (Neumann), 1: DST-I (Dirichlet)
-static int gen_setup(bk_ctx* c, int d, int n, int type) {
-  Precond& pc = c->pc;
-  bkg::Plan& pl = pc.gplan[d];
+static int gen_setup(bk_ctx* c, Line& ln) {
+  bkg::Plan& pl = ln.plan;
+  const int n = ln.n;
   pl.n = n;
-  pl.L = type == 0 ? 2 * n : 2 * n + 2;
+  pl.L = ln.type == 0 ? 2 * n : 2 * n + 2;
   BK_CHECK(c, 32LL * pl.L <= BKG_SMEM_MAX, "line too long for the general transform kernel (n <= 3199)");
   factorize(pl.L, pl);
   const long double PI = 3.14159265358979323846264338327950288L;
@@ -314,17 +256,17 @@ static int gen_setup(bk_ctx* c, int d, int n, int type) {
     ph[2 * k] = (double)cosl(-PI * k / (2.0L * n));
     ph[2 * k + 1] = (double)sinl(-PI * k / (2.0L * n));
   }
-  BK_TRY(upload(c, (void**)&pc.gwl[d], wl.data(), 8 * wl.size()));
-  BK_TRY(upload(c, (void**)&pc.gph[d], ph.data(), 8 * ph.size()));
-  pl.wl = pc.gwl[d];
-  pl.ph = pc.gph[d];
+  BK_TRY(upload(c, (void**)&ln.gwl, wl.data(), 8 * wl.size()));
+  BK_TRY(upload(c, (void**)&ln.gph, ph.data(), 8 * ph.size()));
+  pl.wl = ln.gwl;
+  pl.ph = ln.gph;
   pl.dst_scale = 0.5 * sqrt(2.0 / (n + 1.0));
   return BK_OK;
 }
 
 // mode 0 DCT forward (2 C), 1 DCT inverse (n x), 2 DST-I (orthonormal)
-static int gen_launch(bk_ctx* c, int d, bool strided, int mode, const double* in, double* out, const bkf::Geom& g) {
-  const bkg::Plan& pl = c->pc.gplan[d];
+static int gen_launch(bk_ctx* c, const Line& ln, bool strided, int mode, const double* in, double* out, const bkf::Geom& g) {
+  const bkg::Plan& pl = ln.plan;
   const int ppg = gen_ppg(pl.L);
   const size_t sm = 32 * (size_t)pl.L * ppg;
   const long long npairs = ((long long)g.nb + 1) / 2;
@@ -334,21 +276,48 @@ static int gen_launch(bk_ctx* c, int d, bool strided, int mode, const double* in
   return bk_launch(c, kern[strided][mode], grid, dim3(BKG_THREADS), sm, in, out, g, pl, ppg);
 }
 
-// transform tables for dimension d of length n. type 0: DCT-II (Neumann), 1: DST-I (Dirichlet)
-static int setup_dim(bk_ctx* c, int d, long long n, double inv_h2, int type, bool even_nx) {
-  Precond& pc = c->pc;
+// The transform of one dimension: its eigenvalues lam (n = lam.size()) and the tables of the kernels that may run it.  The
+// fast kernels take DCT-II lines of a power-of-two length whose grid rows hold an even number of values (16-byte accesses);
+// with `general` the line also gets the general plan, which unaligned vectors fall back to.  Without it (the periodic
+// pipeline, which has no general kernel) the line is a power of two and always runs on the fast kernels.
+static int line_setup(bk_ctx* c, Line& ln, int type, const std::vector<double>& lam, bool general) {
+  const long long n = (long long)lam.size();
+  ln.n = (int)n;
+  ln.type = type;
+  BK_TRY(upload(c, (void**)&ln.lam, lam.data(), 8 * n));
+  if (general) {
+    ln.fast = (type == 0 && c->dims[0] % 2 == 0) ? fast_logn(n) : 0;
+  } else {
+    ln.fast = 0;
+    while ((1LL << ln.fast) < n) ++ln.fast;
+  }
+  if (ln.fast) {
+    std::vector<double> tw, om, lam2;
+    BKF_DISPATCH(ln.fast, bkf::build_tables<FC>(tw, om, lam2, lam.data()));
+    if (tw.empty()) tw.assign(2, 0.0);
+    BK_TRY(upload(c, (void**)&ln.ftw, tw.data(), 8 * tw.size()));
+    BK_TRY(upload(c, (void**)&ln.fom, om.data(), 8 * om.size()));
+    BK_TRY(upload(c, (void**)&ln.flam2, lam2.data(), 8 * lam2.size()));
+  }
+  return general ? gen_setup(c, ln) : BK_OK;
+}
+
+void line_free(Line& ln) {
+  void* tabs[] = {ln.lam, ln.ftw, ln.fom, ln.flam2, ln.gwl, ln.gph};
+  for (void* t : tabs)
+    if (t) cudaFree(t);
+}
+
+// dimension d of a grid Laplacian. type 0: DCT-II (Neumann), 1: DST-I (Dirichlet)
+static int setup_dim(bk_ctx* c, int d, int type) {
+  const long long n = c->dims[d];
+  const double inv_h2 = bk_inv_h2(c, d);
   std::vector<double> lam(n);
   const long double PI = 3.14159265358979323846264338327950288L;
   for (long long k = 0; k < n; ++k)
     lam[k] = (type == 0) ? (double)((2.0L * cosl(PI * k / n) - 2.0L)) * inv_h2
                          : (double)(-(2.0L - 2.0L * cosl(PI * (k + 1) / (n + 1)))) * inv_h2;
-  BK_TRY(upload(c, (void**)&pc.lam[d], lam.data(), 8 * n));
-  pc.ttype[d] = type;
-  pc.fast[d] = (type == 0 && even_nx) ? fast_logn(n) : 0;  // 16-byte accesses need an even row length
-  if (pc.fast[d]) {
-    BKF_DISPATCH(pc.fast[d], BK_TRY(fast_setup<FC>(c, d, lam.data())));
-  }
-  return gen_setup(c, d, (int)n, type);  // always available: unaligned vectors fall back to it
+  return line_setup(c, c->pc.line[d], type, lam, true);
 }
 
 // ---- BK_SH2D_PERIODIC: real 2-D FFT pipeline -------------------------------------------------------------------------------
@@ -361,33 +330,30 @@ int bk_periodic_setup(bk_ctx* c) {
   const long double PI = 3.14159265358979323846264338327950288L;
   for (int d = 0; d < 2; ++d) {
     const long long n = c->dims[d];
-    int logn = 0;
-    while ((1LL << logn) < n) ++logn;
     std::vector<double> lam(n);
     for (long long k = 0; k < n; ++k) {
       const long double ks = (long double)(k <= n / 2 ? k : k - n), w = PI * ks / (long double)c->lengths[d];
       lam[k] = (double)(-w * w);
     }
-    BK_TRY(upload(c, (void**)&pc.lam[d], lam.data(), 8 * n));
-    pc.fast[d] = logn;
-    BKF_DISPATCH(logn, BK_TRY(fast_setup<FC>(c, d, lam.data())));
+    BK_TRY(line_setup(c, pc.line[d], 0, lam, false));
   }
   if (!pc.work) BK_CUDA(c, cudaMalloc(&pc.work, 8 * (size_t)c->ld));
   if (!pc.work2) BK_CUDA(c, cudaMalloc(&pc.work2, 8 * (size_t)c->ld));
   return BK_OK;
 }
 
-// out = epilogue(F^-1 sigma F prologue(in)), sigma = gain / (Nx Ny) * (neg ? -L1 : 1 / (L1 + shift)); 3 kernels, 64N bytes at most
+// out = epilogue(F^-1 sigma F prologue(in)), sigma = gain / (Nx Ny) * (neg ? -L1 : 1 / (L1 + shift)); 3 kernels, 64N bytes at most.
+// The y pass also copies the border entries of `tail` (border_tail).
 static int periodic_pipeline(bk_ctx* c, const double* in, double* out, const PerPw& pw, bool neg, double gain, double shift,
-                             const double* tail_src = nullptr, double* tail_dst = nullptr, int tail_n = 0) {
+                             const bkf::Symbol& tail = {}) {
   Precond& pc = c->pc;
   const int nx = (int)c->dims[0], ny = (int)c->dims[1];
   const bkf::Geom gx{1, nx, ny, 1}, gy{nx, (long long)nx * ny, nx, 1};
-  const bkf::Symbol sy{pc.lam[0], nullptr, shift, gain / ((double)nx * (double)ny), tail_src, tail_dst, tail_n, neg ? 1 : 0};
-  BKF_DISPATCH(pc.fast[0], BK_TRY(fast_launch<FC>(c, 0, false, 2, in, pc.work, gx, nullptr, &pw)));
-  BKF_DISPATCH(pc.fast[1], BK_TRY(fast_launch<FC>(c, 1, true, 3, pc.work, pc.work2, gy, &sy)));
-  BKF_DISPATCH(pc.fast[0], BK_TRY(fast_launch<FC>(c, 0, false, 3, pc.work2, out, gx, nullptr, &pw)));
-  return BK_OK;
+  const bkf::Symbol sy{pc.line[0].lam, nullptr, shift, gain / ((double)nx * (double)ny), tail.tail_src, tail.tail_dst, tail.tail_n,
+                       neg ? 1 : 0};
+  BK_TRY(fast_launch(c, pc.line[0], false, 2, in, pc.work, gx, nullptr, &pw));
+  BK_TRY(fast_launch(c, pc.line[1], true, 3, pc.work, pc.work2, gy, &sy));
+  return fast_launch(c, pc.line[0], false, 3, pc.work2, out, gx, nullptr, &pw);
 }
 
 int bk_periodic_residual(bk_ctx* c, const OpDesc& op, const double* u, double* out) {
@@ -414,23 +380,22 @@ extern "C" int32_t bk_precond_setup(bk_ctx* c, int32_t kind, double a0, double a
   }
   if (!pc.work) BK_CUDA(c, cudaMalloc(&pc.work, 8 * (size_t)c->ld));
   if (!pc.work2) BK_CUDA(c, cudaMalloc(&pc.work2, 8 * (size_t)c->ld));
-  const bool even_nx = (c->dims[0] % 2) == 0;
   if (kind == BK_PC_SH_DCT) {
     BK_CHECK(c, c->kind == BK_SH2D || c->kind == BK_SH3D, "BK_PC_SH_DCT needs a Swift-Hohenberg context");
-    for (int d = 0; d < bk_kind_traits(c->kind)->ndims; ++d) BK_TRY(setup_dim(c, d, c->dims[d], bk_inv_h2(c, d), 0, even_nx));
+    for (int d = 0; d < bk_kind_traits(c->kind)->ndims; ++d) BK_TRY(setup_dim(c, d, 0));
   } else if (kind == BK_PC_SH_FFT) {
     BK_CHECK(c, c->kind == BK_SH2D_PERIODIC, "BK_PC_SH_FFT needs a BK_SH2D_PERIODIC context");
     BK_CHECK(c, a0 > 0, "BK_PC_SH_FFT: a0 must be > 0 (the symbol of L1 vanishes at |k| = 1)");
     // tables and work buffers are the context's own (bk_periodic_setup)
   } else if (kind == BK_PC_CGL_DST) {
     BK_CHECK(c, c->kind == BK_CGL2D || c->kind == BK_POTRAP_CGL2D, "BK_PC_CGL_DST needs a cGL context");
-    for (int d = 0; d < 2; ++d) BK_TRY(setup_dim(c, d, c->dims[d], bk_inv_h2(c, d), 1, even_nx));
+    for (int d = 0; d < 2; ++d) BK_TRY(setup_dim(c, d, 1));
   } else if (kind == BK_PC_POTRAP_CIRC) {
     BK_CHECK(c, c->kind == BK_POTRAP_CGL2D, "BK_PC_POTRAP_CIRC needs a Trapeze (potrap) context");
     const int K = (int)c->dims[2] - 1;
     BK_CHECK(c, K >= 1 && K <= BK_PO_KMAX, "BK_PC_POTRAP_CIRC supports 2 <= M <= 65 time slices");
     BK_CHECK(c, a0 > 0, "BK_PC_POTRAP_CIRC: a0 must be the period T > 0");
-    for (int d = 0; d < 2; ++d) BK_TRY(setup_dim(c, d, c->dims[d], bk_inv_h2(c, d), 1, even_nx));
+    for (int d = 0; d < 2; ++d) BK_TRY(setup_dim(c, d, 1));
     std::vector<double2> tw(K);
     const long double PI = 3.14159265358979323846264338327950288L;
     for (int j = 0; j < K; ++j) tw[j] = make_double2((double)cosl(-2.0L * PI * j / K), (double)sinl(-2.0L * PI * j / K));
@@ -469,12 +434,12 @@ extern "C" int32_t bk_precond_setup(bk_ctx* c, int32_t kind, double a0, double a
   return BK_OK;
 }
 
-// one 1-D transform pass along dimension d over fields of nx * ny * nz values.
-// mode 0: forward, 1: inverse; fused != NULL (fast path, last dimension): forward + symbol + inverse in one kernel.
+// one 1-D transform pass of line ln along dimension d over fields of nx * ny * nz values.
+// mode 0: forward, 1: inverse; fused != NULL (fast path): forward + symbol + inverse in one kernel.  The fast kernels run when the
+// line has them and in / out are 16-byte aligned, the general kernel otherwise.
 // Conventions: DCT forward returns 2 C, DCT inverse returns n x (the caller's symbol carries 1 / prod(2 n_d)); DST-I is orthonormal.
-static int transform_pass(bk_ctx* c, int d, int mode, const double* in, double* out, int nx, int ny, int nz, bool aligned,
-                          const bkf::Symbol* fused = nullptr) {
-  Precond& pc = c->pc;
+static int transform_pass(bk_ctx* c, const Line& ln, int d, int mode, const double* in, double* out, int nx, int ny, int nz,
+                          bool aligned, const bkf::Symbol* fused = nullptr) {
   bkf::Geom g;
   bool strided = d != 0;
   if (d == 0) {
@@ -493,16 +458,49 @@ static int transform_pass(bk_ctx* c, int d, int mode, const double* in, double* 
     g.os = nx;
     g.nouter = ny;
   }
-  if (pc.fast[d] && aligned) {
-    BKF_DISPATCH(pc.fast[d], BK_TRY(fast_launch<FC>(c, d, strided, fused ? 2 : mode, in, out, g, fused)));
-  } else {
-    BK_CHECK(c, !fused, "internal: fused transform on the general path");
-    BK_TRY(gen_launch(c, d, strided, pc.ttype[d] == 1 ? 2 : mode, in, out, g));
-  }
-  return BK_OK;
+  if (ln.fast && aligned) return fast_launch(c, ln, strided, fused ? 2 : mode, in, out, g, fused);
+  BK_CHECK(c, !fused, "internal: fused transform on the general path");
+  return gen_launch(c, ln, strided, ln.type == 1 ? 2 : mode, in, out, g);
 }
 
 static inline bool aligned16(const void* a, const void* b) { return ((((uintptr_t)a) | ((uintptr_t)b)) & 15) == 0; }
+
+// Border entries behind the N grid values of an n-vector ride along with a transform kernel that can carry them (up to 32, in
+// its symbol sy); returns whether they do.  Otherwise precond_apply_one copies them.
+static bool border_tail(bkf::Symbol& sy, const double* in, double* out, long long n, long long N) {
+  if (n <= N || n - N > 32) return false;
+  sy.tail_src = in + N;
+  sy.tail_dst = out + N;
+  sy.tail_n = (int)(n - N);
+  return true;
+}
+
+// A spectral solve along the first nd dimensions of fields of nx * ny * nz values, in to out: forward passes d = 0 .. nd-1, the
+// middle step in the transformed basis, inverse passes d = nd-1 .. 0, each pass from one work buffer to the other.  Only the
+// first and the last pass touch in / out, so only they take the caller's alignment al.  A middle step the fast kernels can fuse
+// comes as its symbol sy (SH_DCT): it is fused into the last forward pass when that pass is on the fast path and al holds, and
+// the border entries of the n-vector then ride along (sy->tail_n > 0).  Otherwise mid(buffer) applies it in place.
+template <class Mid>
+static int spectral_solve(bk_ctx* c, int nd, int nx, int ny, int nz, const double* in, double* out, long long n, bool al,
+                          bkf::Symbol* sy, Mid mid) {
+  const Line* ln = c->pc.line;
+  double* buf[2] = {c->pc.work, c->pc.work2};
+  const bool fuse = sy && ln[nd - 1].fast && al;
+  if (fuse) border_tail(*sy, in, out, n, c->N0);
+  const int npass = fuse ? 2 * nd - 1 : 2 * nd;
+  int p = 0;
+  auto pass = [&](int d, int mode, const bkf::Symbol* fused) {
+    const bool edge = p == 0 || p == npass - 1;
+    const double* src = p == 0 ? in : buf[(p - 1) & 1];
+    double* dst = p == npass - 1 ? out : buf[p & 1];
+    ++p;
+    return transform_pass(c, ln[d], d, mode, src, dst, nx, ny, nz, edge ? al : true, fused);
+  };
+  for (int d = 0; d < nd; ++d) BK_TRY(pass(d, 0, fuse && d == nd - 1 ? sy : nullptr));
+  if (!fuse) BK_TRY(mid(buf[(nd - 1) & 1]));
+  for (int d = fuse ? nd - 2 : nd - 1; d >= 0; --d) BK_TRY(pass(d, 1, nullptr));
+  return BK_OK;
+}
 
 static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long n);
 
@@ -518,6 +516,7 @@ int bk_precond_apply_dev(bk_ctx* c, const double* in, double* out, long long n) 
 
 static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long n) {
   Precond& pc = c->pc;
+  const Line* ln = pc.line;
   const long long N = c->N0;
   bool tail_done = false;
   const bool timed = c->timing_now;  // per-application device time for bench.py's breakdown
@@ -526,88 +525,37 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
   if (pc.kind == BK_PC_SH_DCT) {
     const int nd = bk_kind_traits(c->kind)->ndims;
     const int nx = (int)c->dims[0], ny = (int)c->dims[1], nz = nd == 3 ? (int)c->dims[2] : 1;
-    double* A = pc.work;
-    double* B = pc.work2;
-    const int last = nd - 1;
     double scale = 1.0;
     for (int d = 0; d < nd; ++d) scale /= 2.0 * (double)c->dims[d];
-    if (pc.fast[last] && al) {
-      // x fwd, [y fwd,] (last dim: fwd + symbol + inverse in one kernel), [y inv,] x inv
-      bkf::Symbol sy{pc.lam[0], nd == 3 ? pc.lam[1] : nullptr, pc.a0, scale, nullptr, nullptr, 0};
-      if (n > N && n - N <= 32) {  // border entries ride along with the fused kernel
-        sy.tail_src = in + N;
-        sy.tail_dst = out + N;
-        sy.tail_n = (int)(n - N);
-        tail_done = true;
-      }
-      BK_TRY(transform_pass(c, 0, 0, in, A, nx, ny, nz, al));
-      if (nd == 3) {
-        BK_TRY(transform_pass(c, 1, 0, A, B, nx, ny, nz, true));
-        BK_TRY(transform_pass(c, 2, 0, B, A, nx, ny, nz, true, &sy));
-        BK_TRY(transform_pass(c, 1, 1, A, B, nx, ny, nz, true));
-        BK_TRY(transform_pass(c, 0, 1, B, out, nx, ny, nz, al));
-      } else {
-        BK_TRY(transform_pass(c, 1, 0, A, B, nx, ny, nz, true, &sy));
-        BK_TRY(transform_pass(c, 0, 1, B, out, nx, ny, nz, al));
-      }
-    } else {
-      BK_TRY(transform_pass(c, 0, 0, in, A, nx, ny, nz, al));
-      BK_TRY(transform_pass(c, 1, 0, A, B, nx, ny, nz, true));
-      double* cur = B;
-      double* oth = A;
-      if (nd == 3) {
-        BK_TRY(transform_pass(c, 2, 0, B, A, nx, ny, nz, true));
-        cur = A;
-        oth = B;
-      }
-      BK_TRY(bk_launch_ordered(c, k_sh_symbol_div, bk_lin_grid(c, N), 256, 0, cur, nx, ny, nz, pc.lam[0], pc.lam[1],
-                               nd == 3 ? pc.lam[2] : nullptr, pc.a0, scale));
-      if (nd == 3) {
-        BK_TRY(transform_pass(c, 2, 1, cur, oth, nx, ny, nz, true));
-        std::swap(cur, oth);
-      }
-      BK_TRY(transform_pass(c, 1, 1, cur, oth, nx, ny, nz, true));
-      BK_TRY(transform_pass(c, 0, 1, oth, out, nx, ny, nz, al));
-    }
+    bkf::Symbol sy{ln[0].lam, nd == 3 ? ln[1].lam : nullptr, pc.a0, scale, nullptr, nullptr, 0};
+    BK_TRY(spectral_solve(c, nd, nx, ny, nz, in, out, n, al, &sy, [&](double* v) {
+      return bk_launch_ordered(c, k_sh_symbol_div, bk_lin_grid(c, N), 256, 0, v, nx, ny, nz, ln[0].lam, ln[1].lam,
+                               nd == 3 ? ln[2].lam : nullptr, pc.a0, scale);
+    }));
+    tail_done = sy.tail_n > 0;
   } else if (pc.kind == BK_PC_SH_FFT) {
-    const double* ts = nullptr;
-    double* td = nullptr;
-    int tn = 0;
-    if (n > N && n - N <= 32) {  // border entries ride along with the y pass
-      ts = in + N;
-      td = out + N;
-      tn = (int)(n - N);
-      tail_done = true;
-    }
+    bkf::Symbol tail{};
+    tail_done = border_tail(tail, in, out, n, N);
     const PerPw pw{0, PW_NONE, in, nullptr, nullptr, 0.0, 0.0, 0.0, 0.0, 0.0};
-    BK_TRY(periodic_pipeline(c, in, out, pw, false, 1.0, pc.a0, ts, td, tn));
+    BK_TRY(periodic_pipeline(c, in, out, pw, false, 1.0, pc.a0, tail));
   } else if (pc.kind == BK_PC_CGL_DST) {
     const int nx = (int)c->dims[0], ny = (int)c->dims[1];
     const long long nblk = (c->kind == BK_POTRAP_CGL2D) ? 2 * c->dims[2] : 2;  // components x slices
-    double* A = pc.work;
-    double* B = pc.work2;
-    BK_TRY(transform_pass(c, 0, 0, in, A, nx, ny, (int)nblk, al));
-    BK_TRY(transform_pass(c, 1, 0, A, B, nx, ny, (int)nblk, true));
-    BK_TRY(bk_launch_ordered(c, k_helmholtz_symbol_div, bk_lin_grid(c, (long long)nx * ny * nblk), 256, 0, B, nx, ny, nblk,
-                             pc.lam[0], pc.lam[1], pc.a0, pc.a1));
-    BK_TRY(transform_pass(c, 1, 1, B, A, nx, ny, (int)nblk, true));
-    BK_TRY(transform_pass(c, 0, 1, A, out, nx, ny, (int)nblk, al));
+    BK_TRY(spectral_solve(c, 2, nx, ny, (int)nblk, in, out, n, al, nullptr, [&](double* v) {
+      return bk_launch_ordered(c, k_helmholtz_symbol_div, bk_lin_grid(c, (long long)nx * ny * nblk), 256, 0, v, nx, ny, nblk,
+                               ln[0].lam, ln[1].lam, pc.a0, pc.a1);
+    }));
     if (c->kind == BK_POTRAP_CGL2D) BK_CUDA(c, cudaMemcpyAsync(out + N - 1, in + N - 1, 8, cudaMemcpyDeviceToDevice, c->stream));
   } else if (pc.kind == BK_PC_POTRAP_CIRC) {
     const int nx = (int)c->dims[0], ny = (int)c->dims[1], M = (int)c->dims[2];
     const long long nn = (long long)nx * ny, Ns = 2 * nn;
-    const int nf = 2 * M;
-    double* A = pc.work;
-    double* Bf = pc.work2;
     // DST-I in space over all 2M slice components (mixed-radix FFT of the odd extension, bk_fft_gen.cuh), the circulant
     // solve in time per spatial mode, DST-I back.  While J' is selected (bk_jac_set_transpose) this is P'^-1: the transposed
     // time solve, then x_M = r_M and the period entry pass through (one copy: they are the last Ns + 1 entries).
-    BK_TRY(transform_pass(c, 0, 0, in, A, nx, ny, nf, al));
-    BK_TRY(transform_pass(c, 1, 0, A, Bf, nx, ny, nf, true));
-    BK_TRY(bk_launch_ordered(c, c->transpose ? k_potrap_time_tr : k_potrap_time, (unsigned)((nn + 127) / 128), 128, 0, Bf, nn, nx,
-                             M - 1, pc.lam[0], pc.lam[1], pc.po_T / M, pc.po_r, pc.po_nu, pc.tdft));
-    BK_TRY(transform_pass(c, 1, 1, Bf, A, nx, ny, nf, true));
-    BK_TRY(transform_pass(c, 0, 1, A, out, nx, ny, nf, al));
+    BK_TRY(spectral_solve(c, 2, nx, ny, 2 * M, in, out, n, al, nullptr, [&](double* v) {
+      return bk_launch_ordered(c, c->transpose ? k_potrap_time<true> : k_potrap_time<false>, (unsigned)((nn + 127) / 128), 128, 0,
+                               v, nn, nx, M - 1, ln[0].lam, ln[1].lam, pc.po_T / M, pc.po_r, pc.po_nu, pc.tdft);
+    }));
     if (c->transpose)
       BK_CUDA(c, cudaMemcpyAsync(out + (M - 1) * Ns, in + (M - 1) * Ns, 8 * (size_t)(Ns + 1), cudaMemcpyDeviceToDevice, c->stream));
     else

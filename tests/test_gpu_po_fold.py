@@ -1,4 +1,4 @@
-"""GPU tests of J' of the Trapeze functional (k_potrap_apply_tr), the transposed circulant preconditioner (k_potrap_time_tr) and
+"""GPU tests of J' of the Trapeze functional (k_potrap_apply_tr), the transposed circulant preconditioner (k_potrap_time<true>) and
 the folds of periodic orbits built on them (periodic.newton_fold_po / continuation_fold_po), against the sparse Trapeze Jacobian
 of tests/potrap_sparse_oracle.py."""
 import numpy as np

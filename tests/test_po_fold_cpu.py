@@ -164,9 +164,9 @@ def test_continuation_fold_po_follows_the_closed_form_in_c5(sl_fold):
 
 # ------------------------------------------------------------------------------------------------ sm_90a code
 def test_adjoint_kernels_are_in_the_sm_90a_code():
-    """k_potrap_apply_tr uses no local memory.  k_potrap_time_tr, like k_potrap_time, keeps its four per-thread arrays of
-    BK_PO_KMAX double2 (the time DFT of one spatial mode) in local memory: it has exactly the forward kernel's stack frame,
-    4096 bytes, with no spills (ptxas reports LOCAL:0, i.e. no spill space) and the same register count"""
+    """k_potrap_apply_tr uses no local memory.  k_potrap_time<true> (the transposed solve), like k_potrap_time<false>, keeps its
+    four per-thread arrays of BK_PO_KMAX double2 (the time DFT of one spatial mode) in local memory: it has exactly the forward
+    kernel's stack frame, 4096 bytes, with no spills (ptxas reports LOCAL:0, i.e. no spill space) and the same register count"""
     if shutil.which("cuobjdump") is None:
         pytest.skip("cuobjdump not on PATH")
     bk = g.load_package()
@@ -184,8 +184,8 @@ def test_adjoint_kernels_are_in_the_sm_90a_code():
     tr = [c for k, c in cnt.items() if "k_potrap_apply_tr" in k]
     assert len(tr) == 1
     assert tr[0]["LDL"] == 0 and tr[0]["STL"] == 0 and tr[0]["DFMA"] + tr[0]["DMUL"] >= 20, dict(tr[0])
-    time_tr = [c for k, c in cnt.items() if "k_potrap_time_tr" in k]
-    time = [c for k, c in cnt.items() if "k_potrap_time" in k and "k_potrap_time_tr" not in k]
+    time_tr = [c for k, c in cnt.items() if "k_potrap_timeILb1E" in k]   # mangled k_potrap_time<true>
+    time = [c for k, c in cnt.items() if "k_potrap_timeILb0E" in k]
     assert len(time_tr) == 1 and len(time) == 1
     assert "arch = sm_90a" in out
     res = subprocess.run(["cuobjdump", "-res-usage", bk.lib.LIB_PATH], capture_output=True, text=True).stdout.splitlines()
@@ -194,8 +194,8 @@ def test_adjoint_kernels_are_in_the_sm_90a_code():
         m = re.search(r"Function (\S+):", a)
         if m and "k_potrap_" in m.group(1):
             usage[m.group(1)] = dict(re.findall(r"(REG|STACK|LOCAL):(\d+)", b))
-    fwd = next(v for k, v in usage.items() if "k_potrap_time" in k and "k_potrap_time_tr" not in k)
-    trn = next(v for k, v in usage.items() if "k_potrap_time_tr" in k)
+    fwd = next(v for k, v in usage.items() if "k_potrap_timeILb0E" in k)
+    trn = next(v for k, v in usage.items() if "k_potrap_timeILb1E" in k)
     app = next(v for k, v in usage.items() if "k_potrap_apply_tr" in k)
     assert trn == fwd and fwd["STACK"] == "4096" and fwd["LOCAL"] == "0", (trn, fwd)
     assert app["STACK"] == "0" and app["LOCAL"] == "0", app

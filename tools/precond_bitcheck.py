@@ -1,0 +1,158 @@
+"""Writes the result of every preconditioner path on seeded inputs as .npy files, so that two builds can be compared bit for bit:
+
+   python tools/precond_bitcheck.py --out DIR [--root TREE]
+   cmp DIR_A/x.npy DIR_B/x.npy   (for every file)
+
+TREE is the repository whose build is loaded (default: the one holding this script); the script uses the public API only, so it
+runs against any build of the library.  Cases: BK_PC_SH_DCT in 2-D and 3-D at power-of-two, mixed and odd sizes on aligned
+vectors and on vectors offset by one double; the border entries of right-preconditioned matrix-free bordered solves (one border
+and a block of two), which a plain application never has; BK_COMPLEX contexts; BK_PC_CGL_DST on cGL2d and Trapeze contexts;
+BK_PC_POTRAP_CIRC with J' off and on; BK_PC_CHAN_TRIDIAG; BK_PC_SH_FFT with a right-preconditioned periodic GMRES solve.  The
+BK_PC_SH_DCT cases run again in a child process under BK_FFT_NO_FAST=1 (general kernel everywhere; files nofast_*)."""
+import argparse
+import ctypes as C
+import importlib.util
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+SH_DCT_2D = [(1024, 1024), (151, 100), (62, 64), (64, 62), (256, 128)]
+SH_DCT_3D = [(64, 64, 64), (48, 32, 16)]
+SH_PAR = (-0.1, 1.3)
+CGL_PAR = (1.2, 0.1, 1.0, -1.0, 1.0)
+
+
+def load(root):
+    spec = importlib.util.spec_from_file_location("bitcheck_graft_entry", os.path.join(root, "__graft_entry__.py"))
+    ge = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(ge)
+    return ge.load_package()
+
+
+class Dump:
+    def __init__(self, out, prefix):
+        self.out, self.prefix = out, prefix
+        os.makedirs(out, exist_ok=True)
+
+    def __call__(self, name, a):
+        np.save(os.path.join(self.out, self.prefix + name + ".npy"), np.asarray(a, dtype=np.float64))
+
+
+def applications(bk, ctx, r, name, dump):
+    """host vectors (staged, aligned), device vectors, and device vectors offset by 8 bytes (in and out, then in only)"""
+    dump(name + "_host", ctx.precond_apply(r))
+    dump(name + "_dev", ctx.precond_apply(ctx.to_device(r)).numpy())
+    n = ctx.N
+    big_in, big_out = ctx.zeros(n + 2), ctx.zeros(n + 2)
+    host = np.concatenate([[0.0], r, [0.0]])
+    assert ctx.lib.bk_vec_upload(ctx.handle, big_in.dptr, host.ctypes.data, len(host)) == 0
+    for tag, shift_out in (("off8", 8), ("off8in", 0)):
+        big_out.zero_()
+        st = ctx.lib.bk_precond_apply(ctx.handle, C.c_void_p(big_in.dptr + 8), C.c_void_p(big_out.dptr + shift_out))
+        assert st == 0, ctx.lib.bk_last_error(ctx.handle)
+        dump(f"{name}_{tag}", big_out.numpy())
+
+
+def bordered(bk, ctx, u, rng, name, dump, restart=30):
+    """right-preconditioned matrix-free bordered solves at u: N + 1 (one border) and N + 2 (a block of two) unknowns"""
+    N = ctx.N
+    ls = bk.GMRESB200(reltol=1e-12, restart=restart, maxiter=restart, Pr=True)
+    J = ctx.jacobian(u)
+    dR, dzu, R = rng.standard_normal(N), rng.standard_normal(N), rng.standard_normal(N)
+    dX, dl, _, it = bk.MatrixFreeBLSB200(ls)(J, dR, dzu, 0.8, R, -0.4, shift=-0.5, dotscale=1.0 / N)
+    dump(name + "_bls1", np.concatenate([dX, [dl, it]]))
+    a = (rng.standard_normal(N), rng.standard_normal(N))
+    b = (rng.standard_normal(N), rng.standard_normal(N))
+    x, p, _, it = bk.MatrixFreeBLSB200(ls).solve_block(J, a, b, [[0.9, 0.1], [-0.2, 1.1]], R, [0.3, -0.7], shift=-0.5,
+                                                        dotscale=1.0 / N)
+    dump(name + "_bls2", np.concatenate([x, p, [it]]))
+
+
+def sh_dct(bk, dump):
+    for dims in SH_DCT_2D + SH_DCT_3D:
+        kind = bk.BK_SH2D if len(dims) == 2 else bk.BK_SH3D
+        L = (8 * np.pi, 4 * np.pi / np.sqrt(3)) if len(dims) == 2 else (np.pi, 1.3 * np.pi, 0.7 * np.pi)
+        ctx = bk.Context(kind, dims, L, krylov_m=30, params=SH_PAR)
+        rng = np.random.default_rng(sum(dims))
+        name = "sh_dct_" + "x".join(map(str, dims))
+        for shift in (1.0, 0.25):
+            ctx.precond_setup(bk.BK_PC_SH_DCT, shift)
+            applications(bk, ctx, rng.standard_normal(ctx.N), f"{name}_s{shift}", dump)
+        if dims in ((256, 128), (151, 100), (48, 32, 16)):
+            bordered(bk, ctx, 0.3 * rng.standard_normal(ctx.N), rng, name, dump)
+        ctx.close()
+    ctx = bk.Context(bk.BK_SH2D, (256, 128), (8 * np.pi, 4 * np.pi), krylov_m=2, params=SH_PAR, complex=True)
+    ctx.precond_setup(bk.BK_PC_SH_DCT, 1.0)
+    applications(bk, ctx, np.random.default_rng(1).standard_normal(ctx.N), "sh_dct_complex_256x128", dump)
+    ctx.close()
+
+
+def others(bk, dump):
+    rng = np.random.default_rng(7)
+    for dims in ((41, 21), (512, 512)):
+        ctx = bk.Context(bk.BK_CGL2D, dims, (0.5 * np.pi, np.pi), krylov_m=30, params=CGL_PAR)
+        ctx.precond_setup(bk.BK_PC_CGL_DST, 1.0, -0.05)
+        name = "cgl_dst_" + "x".join(map(str, dims))
+        applications(bk, ctx, rng.standard_normal(ctx.N), name, dump)
+        bordered(bk, ctx, 0.3 * rng.standard_normal(ctx.N), rng, name, dump)
+        ctx.close()
+    ctx = bk.Context(bk.BK_CGL2D, (24, 12), (np.pi, np.pi / 2), krylov_m=2, params=CGL_PAR, complex=True)
+    ctx.precond_setup(bk.BK_PC_CGL_DST, -1.0, 1.0)
+    applications(bk, ctx, rng.standard_normal(ctx.N), "cgl_dst_complex_24x12", dump)
+    ctx.close()
+    for dims, M in (((16, 12), 10), ((41, 21), 30)):
+        ctx = bk.Context(bk.BK_POTRAP_CGL2D, (*dims, M), (np.pi, np.pi / 2), krylov_m=30, params=(1.3,) + CGL_PAR[1:])
+        name = f"potrap_{dims[0]}x{dims[1]}x{M}"
+        r = rng.standard_normal(ctx.N)
+        ctx.precond_setup(bk.BK_PC_CGL_DST, 1.0, -0.05)
+        applications(bk, ctx, r, name + "_cgl_dst", dump)
+        ctx.precond_setup(bk.BK_PC_POTRAP_CIRC, 6.3)
+        applications(bk, ctx, r, name + "_circ", dump)
+        ctx.set_transpose(True)
+        applications(bk, ctx, r, name + "_circ_tr", dump)
+        ctx.set_transpose(False)
+        x = 0.1 * rng.standard_normal(ctx.N)
+        x[-1] = 6.3
+        ctx.potrap_set_section(rng.standard_normal(ctx.N - 1) / np.sqrt(ctx.N), x[:-1])
+        bordered(bk, ctx, x, rng, name + "_circ", dump)
+        ctx.close()
+    ctx = bk.Context(bk.BK_CHAN, (1000,), krylov_m=2, params=(3.3, 0.01))
+    ctx.precond_setup(bk.BK_PC_CHAN_TRIDIAG)
+    applications(bk, ctx, rng.standard_normal(ctx.N), "chan_tridiag_1000", dump)
+    ctx.close()
+    for dims in ((256, 128), (64, 2048)):
+        ctx = bk.Context(bk.BK_SH2D_PERIODIC, dims, (8 * np.pi, 4 * np.pi), krylov_m=40, params=(-0.15, 1.3))
+        name = "sh_fft_" + "x".join(map(str, dims))
+        for a0 in (1.0, 0.25):
+            ctx.precond_setup(bk.BK_PC_SH_FFT, a0)
+            applications(bk, ctx, rng.standard_normal(ctx.N), f"{name}_a{a0}", dump)
+        u = 0.3 * rng.standard_normal(ctx.N)
+        bordered(bk, ctx, u, rng, name, dump)
+        J, rhs = ctx.jacobian(u), rng.standard_normal(ctx.N)
+        for fused in (True, False):
+            x, _, it = bk.GMRESB200(reltol=1e-12, restart=40, maxiter=40, Pr=True, fused=fused)(J, rhs)
+            dump(f"{name}_gmres_fused{int(fused)}", np.concatenate([x, [it]]))
+        ctx.close()
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--out", required=True)
+    ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    ap.add_argument("--sh-dct-only", action="store_true", help=argparse.SUPPRESS)  # the BK_FFT_NO_FAST child
+    a = ap.parse_args()
+    bk = load(os.path.abspath(a.root))
+    if a.sh_dct_only:
+        sh_dct(bk, Dump(a.out, "nofast_"))
+        return
+    sh_dct(bk, Dump(a.out, ""))
+    others(bk, Dump(a.out, ""))
+    env = dict(os.environ, BK_FFT_NO_FAST="1")  # read once per process by the library
+    subprocess.run([sys.executable, os.path.abspath(__file__), "--out", a.out, "--root", a.root, "--sh-dct-only"], env=env, check=True)
+    print(f"{len(os.listdir(a.out))} files in {a.out}")
+
+
+if __name__ == "__main__":
+    main()
