@@ -7,9 +7,11 @@
 //   i.e. the same fused JVP+Arnoldi kernels as the corrector;
 //   eigenvalues theta of (J - sigma)^-1 of largest magnitude, lambda = sigma + 1/theta, sorted by
 //   decreasing real part (src/EigSolver.jl:16-19).
-// Outer iteration: explicitly restarted Arnoldi with two classical Gram-Schmidt passes (CGS2) on the
-// device (same k2_dots / k2_update kernels as GMRES); the small Hessenberg eigenproblem is solved
-// on the host (complex shifted QR + inverse iteration), like the Givens rotations of GMRES.
+// Outer iteration: Arnoldi with two classical Gram-Schmidt passes (CGS2) on the device (same k2_dots /
+// k2_update kernels as GMRES), restarted by thick_restart for kinds with a symmetric Jacobian (Jacobi on
+// the projected matrix) and by explicit_restart for the others (the small Hessenberg eigenproblem by
+// complex shifted QR + inverse iteration on the host, like the Givens rotations of GMRES).  Both fill one
+// Ritz result and share one convergence test; eig_work grows the workspace only after every argument check.
 #include <algorithm>
 #include <cmath>
 #include <complex>
@@ -239,8 +241,47 @@ struct EigWork {
   double* hB;    // second-pass corrections
   double* gco;   // dot-product coefficients handed from k2_dots to k2_update
   double* coef;  // 2 S: lincomb coefficients
-  double* hp;    // pinned host copy of hA | hB
+  double* hp;    // pinned host copy of hA | hB; also the staged coefficients of q_lincomb
 };
+
+// The workspace for Krylov dimension m: grows Q, eig_dev and eig_pinned together (and Q2 for the thick restart of sym kinds)
+static int eig_work(bk_ctx* c, int m, bool sym, EigWork* ws) {
+  if (c->qcap < m) {
+    BK_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (c->Q) cudaFree(c->Q);
+    if (c->eig_dev) cudaFree(c->eig_dev);
+    if (c->eig_pinned) cudaFreeHost(c->eig_pinned);
+    c->Q = c->eig_dev = c->eig_pinned = nullptr;
+    BK_CUDA(c, cudaMalloc(&c->Q, 8 * (size_t)c->ld * (m + 1)));
+    BK_CUDA(c, cudaMalloc(&c->eig_dev, 8 * (size_t)(m + 4) * 6));
+    BK_CUDA(c, cudaMallocHost(&c->eig_pinned, 8 * (size_t)(m + 4) * 6));
+    c->qcap = m;
+    BK_TRY(bk_launch_ordered(c, k_fill_ones, (m + 4 + 255) / 256, 256, 0, c->eig_dev, m + 4));
+  }
+  if (sym && (!c->Q2 || c->q2cap < m)) {
+    BK_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (c->Q2) cudaFree(c->Q2);
+    BK_CUDA(c, cudaMalloc(&c->Q2, 8 * (size_t)c->ld * (m + 1)));
+    c->q2cap = m;
+  }
+  const int S = m + 4;
+  *ws = EigWork{S, c->eig_dev, c->eig_dev + S, c->eig_dev + 2 * S, c->eig_dev + 3 * S, c->eig_dev + 4 * S, c->eig_pinned};
+  return BK_OK;
+}
+
+// dst = sum_i coef[i] Q_i over the first k columns (coef on the host), copied on to host memory `host` when given.  The
+// coefficients travel through the pinned ws.hp, so the call ends with a stream synchronise before ws.hp can be written again.
+static int q_lincomb(bk_ctx* c, const EigWork& ws, const double* coef, int k, long long n, double* dst, double* host = nullptr) {
+  std::copy(coef, coef + k, ws.hp);
+  BK_CUDA(c, cudaMemcpyAsync(ws.coef, ws.hp, 8 * (size_t)k, cudaMemcpyHostToDevice, c->stream));
+  BK_TRY(bk_launch_lincomb(c, c->Q, nullptr, dst, 0.0, n, k, ws.coef));
+  if (host) {
+    BK_CUDA(c, cudaMemcpyAsync(host, dst, 8 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+    c->stats.d2h_bytes += 8 * n;
+  }
+  BK_CUDA(c, cudaStreamSynchronize(c->stream));
+  return BK_OK;
+}
 
 // Q_0 = x / ||x||
 static int arnoldi_start(bk_ctx* c, const EigWork& ws, const double* x, long long n) {
@@ -289,118 +330,81 @@ static int arnoldi_expand(bk_ctx* c, const EigWork& ws, const OpDesc& op, const 
   return BK_OK;
 }
 
-extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, int32_t krylovdim, double tol,
-                                        int32_t maxrestart, const bk_gmres_opts* inner, const double* v0, double* vals_re,
-                                        double* vals_im, double* vecs, int32_t* nconv, int32_t* nops) {
-  BK_ENTER(c);
-  BkRange nvtx_range("bk_eigs_shift_invert");
-  // the operator of a complex context is the real-equivalent form of ((-sigma + i a0_imag) I + J): neither symmetric for the
-  // thick restart nor mapped back by lambda = sigma + 1/theta, and every eigenvalue of J would come out twice
-  BK_CHECK(c, !c->cplx, "bk_eigs_shift_invert: not available in a BK_COMPLEX context");
-  BK_CHECK(c, c->have_state, "bk_jac_set_state must be called first");
-  BK_CHECK(c, inner != nullptr && vals_re && vals_im, "null argument");
-  const long long n = c->N;
-  int m = krylovdim;
-  if ((long long)m > n) m = (int)n;
-  BK_CHECK(c, nev >= 1 && nev <= m, "need 1 <= nev <= krylovdim <= N");
-  if (maxrestart < 1) maxrestart = 1;
-  // workspace
-  if (c->qcap < m) {
-    BK_CUDA(c, cudaStreamSynchronize(c->stream));
-    if (c->Q) cudaFree(c->Q);
-    if (c->eig_dev) cudaFree(c->eig_dev);
-    if (c->eig_pinned) cudaFreeHost(c->eig_pinned);
-    c->Q = c->eig_dev = c->eig_pinned = nullptr;
-    BK_CUDA(c, cudaMalloc(&c->Q, 8 * (size_t)c->ld * (m + 1)));
-    BK_CUDA(c, cudaMalloc(&c->eig_dev, 8 * (size_t)(m + 4) * 6));
-    BK_CUDA(c, cudaMallocHost(&c->eig_pinned, 8 * (size_t)(m + 4) * 6));
-    c->qcap = m;
-    BK_TRY(bk_launch_ordered(c, k_fill_ones, (m + 4 + 255) / 256, 256, 0, c->eig_dev, m + 4));
-  }
-  // partial-sum buffer must hold m rows
-  BK_CHECK(c, m <= c->m, "krylovdim exceeds the context's krylov_m (partial-sum workspace)");
-  const int S = m + 4;
-  const EigWork ws{S, c->eig_dev, c->eig_dev + S, c->eig_dev + 2 * S, c->eig_dev + 3 * S, c->eig_dev + 4 * S, c->eig_pinned};
-  double* coef = ws.coef;
-  double* hp = ws.hp;
-  double* x;
-  BK_TRY(bk_tmp(c, 3, &x));
-  OpDesc op = bk_make_op(c, -sigma, 1.0);  // (a0 I + a1 J) with a0 = -sigma (src/EigSolver.jl:260)
-
-  // start vector
-  if (v0) {
-    cudaMemcpyKind kd = bk_is_device_ptr(v0) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    BK_CUDA(c, cudaMemcpyAsync(x, v0, 8 * (size_t)n, kd, c->stream));
-  } else {
-    BK_TRY(bk_launch_ordered(c, k_start_vector, c->nsm * 4, 256, 0, x, n));
-  }
-  int total_ops = 0;
-  std::vector<double> H((size_t)(m + 1) * m);
-  std::vector<cplx> ev, ritz(nev);
-  std::vector<std::vector<cplx>> Y(nev);
+namespace {
+// What a restart strategy hands back: the min(nev, keff) wanted Ritz values theta of (J - sigma)^-1, their vectors y in the
+// basis Q_0..Q_{keff-1}, whether they converged, and the inner solves spent
+struct Ritz {
+  std::vector<cplx> theta;
+  std::vector<std::vector<cplx>> Y;
+  int keff;
   bool converged = false;
-  int keff = m;
-  // ---------------- symmetric operators (Swift-Hohenberg): thick-restart (Krylov-Schur with Ritz vectors) ----------------
-  const bool sym = bk_kind_traits(c->kind)->jac_sym;
-  std::vector<double> Ssym, wsym;
+  int nops = 0;
+};
+}  // namespace
+
+// The Ritz test shared by both restarts on the pairs (theta_q, y_q), q < min(nev, keff), of one Arnoldi factorisation: the
+// residual |h_{m+1,m}| |y_q[keff-1]| of every pair is within tol |theta_q|, or the Krylov space is invariant (keff < m).  The
+// thick restart's pairs are real: std::abs(cplx(x, 0)) is hypot(x, 0) = |x| exactly.
+static void ritz_test(Ritz& r, int nev, int m, const std::vector<double>& H, double tol) {
+  const int nv = std::min(nev, r.keff);
+  const double hlast = (r.keff == m) ? H[m + (size_t)(m - 1) * (m + 1)] : 0.0;
+  bool all = true;
+  for (int q = 0; q < nv; ++q)
+    if (fabs(hlast) * std::abs(r.Y[q][r.keff - 1]) > tol * fmax(std::abs(r.theta[q]), 1e-300)) all = false;
+  r.converged = all || r.keff < m;
+}
+
+// Symmetric operators (Swift-Hohenberg): thick restart (Krylov-Schur with Ritz vectors).  Each restart keeps the pkeep
+// wanted Ritz vectors and the residual direction, and expands from there.
+static int thick_restart(bk_ctx* c, const EigWork& ws, const OpDesc& op, const bk_gmres_opts* inner, double* x, long long n,
+                         int m, int nev, double tol, int maxrestart, Ritz& r) {
+  std::vector<double> H((size_t)(m + 1) * m), S, w;
   std::vector<int> order;
-  if (sym) {
-    if (!c->Q2 || c->q2cap < m) {
-      BK_CUDA(c, cudaStreamSynchronize(c->stream));
-      if (c->Q2) cudaFree(c->Q2);
-      BK_CUDA(c, cudaMalloc(&c->Q2, 8 * (size_t)c->ld * (m + 1)));
-      c->q2cap = m;
+  BK_TRY(arnoldi_start(c, ws, x, n));
+  int kstart = 0;
+  for (int rs = 0; rs < maxrestart && !r.converged; ++rs) {
+    BK_TRY(arnoldi_expand(c, ws, op, inner, x, n, m, kstart, H, &r.keff, &r.nops));
+    const int keff = r.keff;
+    // symmetrised projected matrix (exactly symmetric in exact arithmetic), mirrored from the upper triangle of H.  After a
+    // restart the retained Ritz values sit on the diagonal of columns 0..kstart-1, and the arrow <Q_q, Op q_kstart> that couples
+    // them to the residual direction is column kstart's Gram-Schmidt coefficients, so the lower triangle is never needed.
+    std::vector<double> A((size_t)keff * keff);
+    for (int jj = 0; jj < keff; ++jj)
+      for (int i = 0; i < keff; ++i) A[i + (size_t)jj * keff] = H[std::min(i, jj) + (size_t)std::max(i, jj) * (m + 1)];
+    jacobi_eig(A, keff, w, S);
+    order.resize(keff);
+    for (int i = 0; i < keff; ++i) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](int a, int b) { return fabs(w[a]) > fabs(w[b]); });
+    for (int q = 0; q < std::min(nev, keff); ++q) {
+      r.theta[q] = cplx(w[order[q]], 0.0);
+      r.Y[q].assign(S.begin() + (size_t)order[q] * keff, S.begin() + (size_t)(order[q] + 1) * keff);  // column order[q] of S
     }
-    std::fill(H.begin(), H.end(), 0.0);
-    BK_TRY(arnoldi_start(c, ws, x, n));
-    int kstart = 0;
-    for (int rs = 0; rs < maxrestart && !converged; ++rs) {
-      BK_TRY(arnoldi_expand(c, ws, op, inner, x, n, m, kstart, H, &keff, &total_ops));
-      // symmetrised projected matrix (exactly symmetric in exact arithmetic), mirrored from the upper triangle of H.  After a
-      // restart the retained Ritz values sit on the diagonal of columns 0..kstart-1, and the arrow <Q_q, Op q_kstart> that couples
-      // them to the residual direction is column kstart's Gram-Schmidt coefficients, so the lower triangle is never needed.
-      std::vector<double> A((size_t)keff * keff);
-      for (int jj = 0; jj < keff; ++jj)
-        for (int i = 0; i < keff; ++i) A[i + (size_t)jj * keff] = H[std::min(i, jj) + (size_t)std::max(i, jj) * (m + 1)];
-      jacobi_eig(A, keff, wsym, Ssym);
-      order.resize(keff);
-      for (int i = 0; i < keff; ++i) order[i] = i;
-      std::sort(order.begin(), order.end(), [&](int a, int b) { return fabs(wsym[a]) > fabs(wsym[b]); });
-      const double hlast = (keff == m) ? H[m + (size_t)(m - 1) * (m + 1)] : 0.0;
-      int nv = std::min<int>(nev, keff);
-      bool all = true;
-      for (int q = 0; q < nv; ++q) {
-        const int iq = order[q];
-        ritz[q] = cplx(wsym[iq], 0.0);
-        Y[q].assign(keff, cplx(0, 0));
-        for (int i = 0; i < keff; ++i) Y[q][i] = cplx(Ssym[i + (size_t)iq * keff], 0.0);
-        double resid = fabs(hlast) * fabs(Ssym[(keff - 1) + (size_t)iq * keff]);
-        if (resid > tol * fmax(fabs(wsym[iq]), 1e-300)) all = false;
-      }
-      for (int q = nv; q < nev; ++q) ritz[q] = cplx(0, 0);
-      converged = all || keff < m;
-      if (!converged && rs + 1 < maxrestart) {
-        int pkeep = std::min(keff - 2, nev + std::max(8, (m - nev) / 3));
-        if (pkeep < 1) pkeep = 1;
-        for (int q = 0; q < pkeep; ++q) {  // Q2_q = Q S[:, order[q]]
-          for (int i = 0; i < keff; ++i) hp[i] = Ssym[i + (size_t)order[q] * keff];
-          BK_CUDA(c, cudaMemcpyAsync(coef, hp, 8 * (size_t)keff, cudaMemcpyHostToDevice, c->stream));
-          BK_TRY(bk_launch_lincomb(c, c->Q, nullptr, c->Q2 + (size_t)q * c->ld, 0.0, n, keff, coef));
-          BK_CUDA(c, cudaStreamSynchronize(c->stream));
-        }
-        BK_TRY(bk_dev_copy(c, c->Q2 + (size_t)pkeep * c->ld, c->Q + (size_t)keff * c->ld, n));  // residual direction q_{m+1}
-        BK_CUDA(c, cudaMemcpyAsync(c->Q, c->Q2, 8 * (size_t)c->ld * (pkeep + 1), cudaMemcpyDeviceToDevice, c->stream));
-        std::fill(H.begin(), H.end(), 0.0);
-        for (int q = 0; q < pkeep; ++q) H[q + (size_t)q * (m + 1)] = wsym[order[q]];
-        kstart = pkeep;
-      }
+    ritz_test(r, nev, m, H, tol);
+    if (!r.converged && rs + 1 < maxrestart) {
+      int pkeep = std::min(keff - 2, nev + std::max(8, (m - nev) / 3));
+      if (pkeep < 1) pkeep = 1;
+      for (int q = 0; q < pkeep; ++q)  // Q2_q = Q S[:, order[q]]
+        BK_TRY(q_lincomb(c, ws, S.data() + (size_t)order[q] * keff, keff, n, c->Q2 + (size_t)q * c->ld));
+      BK_TRY(bk_dev_copy(c, c->Q2 + (size_t)pkeep * c->ld, c->Q + (size_t)keff * c->ld, n));  // residual direction q_{m+1}
+      BK_CUDA(c, cudaMemcpyAsync(c->Q, c->Q2, 8 * (size_t)c->ld * (pkeep + 1), cudaMemcpyDeviceToDevice, c->stream));
+      std::fill(H.begin(), H.end(), 0.0);
+      for (int q = 0; q < pkeep; ++q) H[q + (size_t)q * (m + 1)] = w[order[q]];
+      kstart = pkeep;
     }
   }
-  for (int rs = 0; !sym && rs < maxrestart && !converged; ++rs) {
+  return BK_OK;
+}
+
+// The other operators: explicit restart from the sum of the real parts of the wanted Ritz vectors.
+static int explicit_restart(bk_ctx* c, const EigWork& ws, const OpDesc& op, const bk_gmres_opts* inner, double* x, long long n,
+                            int m, int nev, double tol, int maxrestart, Ritz& r) {
+  std::vector<double> H((size_t)(m + 1) * m);
+  std::vector<cplx> ev;
+  for (int rs = 0; rs < maxrestart && !r.converged; ++rs) {
     std::fill(H.begin(), H.end(), 0.0);
     BK_TRY(arnoldi_start(c, ws, x, n));
-    BK_TRY(arnoldi_expand(c, ws, op, inner, x, n, m, 0, H, &keff, &total_ops));
-    // Ritz values / vectors of H(keff x keff)
+    BK_TRY(arnoldi_expand(c, ws, op, inner, x, n, m, 0, H, &r.keff, &r.nops));
+    const int keff = r.keff;
     BK_CHECK(c, hess_eigvals(H, keff, m + 1, ev), "QR iteration on the Hessenberg matrix did not converge");
     // the complex QR returns the members of a conjugate pair with moduli that differ in the last bits: make them exact
     // conjugates, so that the tie rule below, and not rounding, decides which member an nev cutting the pair keeps
@@ -418,36 +422,60 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
       if (da != db) return da > db;
       return a.imag() > b.imag();
     });
-    int nv = std::min<int>(nev, keff);
-    double hlast = (keff == m) ? H[m + (size_t)(m - 1) * (m + 1)] : 0.0;
-    bool all = true;
+    const int nv = std::min(nev, keff);
     for (int q = 0; q < nv; ++q) {
-      ritz[q] = ev[q];
-      hess_eigvec(H, keff, m + 1, ev[q], Y[q]);
-      double resid = fabs(hlast) * std::abs(Y[q][keff - 1]);
-      if (resid > tol * fmax(std::abs(ev[q]), 1e-300)) all = false;
+      r.theta[q] = ev[q];
+      hess_eigvec(H, keff, m + 1, ev[q], r.Y[q]);
     }
-    for (int q = nv; q < nev; ++q) ritz[q] = cplx(0, 0);
-    converged = all || keff < m;
-    if (!converged && rs + 1 < maxrestart) {
-      // restart vector = sum of the real parts of the wanted Ritz vectors
-      for (int i = 0; i < keff; ++i) {
-        double s = 0;
-        for (int q = 0; q < nv; ++q) s += Y[q][i].real();
-        hp[i] = s;
-      }
-      BK_CUDA(c, cudaMemcpyAsync(coef, hp, 8 * (size_t)keff, cudaMemcpyHostToDevice, c->stream));
-      BK_TRY(bk_launch_lincomb(c, c->Q, nullptr, x, 0.0, n, keff, coef));
-      BK_CUDA(c, cudaStreamSynchronize(c->stream));
+    ritz_test(r, nev, m, H, tol);
+    if (!r.converged && rs + 1 < maxrestart) {
+      std::vector<double> v(keff, 0.0);  // restart vector = sum of the real parts of the wanted Ritz vectors
+      for (int q = 0; q < nv; ++q)
+        for (int i = 0; i < keff; ++i) v[i] += r.Y[q][i].real();
+      BK_TRY(q_lincomb(c, ws, v.data(), keff, n, x));
     }
   }
+  return BK_OK;
+}
+
+extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, int32_t krylovdim, double tol,
+                                        int32_t maxrestart, const bk_gmres_opts* inner, const double* v0, double* vals_re,
+                                        double* vals_im, double* vecs, int32_t* nconv, int32_t* nops) {
+  BK_ENTER(c);
+  BkRange nvtx_range("bk_eigs_shift_invert");
+  // the operator of a complex context is the real-equivalent form of ((-sigma + i a0_imag) I + J): neither symmetric for the
+  // thick restart nor mapped back by lambda = sigma + 1/theta, and every eigenvalue of J would come out twice
+  BK_CHECK(c, !c->cplx, "bk_eigs_shift_invert: not available in a BK_COMPLEX context");
+  BK_CHECK(c, c->have_state, "bk_jac_set_state must be called first");
+  BK_CHECK(c, inner != nullptr && vals_re && vals_im, "null argument");
+  const long long n = c->N;
+  int m = krylovdim;
+  if ((long long)m > n) m = (int)n;
+  BK_CHECK(c, nev >= 1 && nev <= m, "need 1 <= nev <= krylovdim <= N");
+  // partial-sum buffer must hold m rows
+  BK_CHECK(c, m <= c->m, "krylovdim exceeds the context's krylov_m (partial-sum workspace)");
+  if (maxrestart < 1) maxrestart = 1;
+  const bool sym = bk_kind_traits(c->kind)->jac_sym;
+  EigWork ws;
+  BK_TRY(eig_work(c, m, sym, &ws));
+  double* x;
+  BK_TRY(bk_tmp(c, 3, &x));
+  OpDesc op = bk_make_op(c, -sigma, 1.0);  // (a0 I + a1 J) with a0 = -sigma (src/EigSolver.jl:260)
+  if (v0) {
+    cudaMemcpyKind kd = bk_is_device_ptr(v0) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    BK_CUDA(c, cudaMemcpyAsync(x, v0, 8 * (size_t)n, kd, c->stream));
+  } else {
+    BK_TRY(bk_launch_ordered(c, k_start_vector, c->nsm * 4, 256, 0, x, n));
+  }
+  Ritz r{std::vector<cplx>(nev), std::vector<std::vector<cplx>>(nev), m};
+  BK_TRY((sym ? thick_restart : explicit_restart)(c, ws, op, inner, x, n, m, nev, tol, maxrestart, r));
   // map back, sort by decreasing real part (ties: decreasing imaginary part)
-  int nv = std::min<int>(nev, keff);
+  const int nv = std::min<int>(nev, r.keff);
   std::vector<int> idx(nv);
   std::vector<cplx> lam(nv);
   for (int q = 0; q < nv; ++q) {
     idx[q] = q;
-    lam[q] = sigma + 1.0 / ritz[q];
+    lam[q] = sigma + 1.0 / r.theta[q];
   }
   std::sort(idx.begin(), idx.end(), [&](int a, int b) {
     if (lam[a].real() != lam[b].real()) return lam[a].real() > lam[b].real();
@@ -462,22 +490,17 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
     double* tmpv;
     BK_TRY(bk_tmp(c, 4, &tmpv));
     const bool dev_out = bk_is_device_ptr(vecs);
+    std::vector<double> yq(r.keff);
     for (int q = 0; q < nv; ++q) {
-      const std::vector<cplx>& y = Y[idx[q]];
-      bool use_im = lam[idx[q]].imag() < 0;
-      for (int i = 0; i < keff; ++i) hp[i] = use_im ? y[i].imag() : y[i].real();
-      BK_CUDA(c, cudaMemcpyAsync(coef, hp, 8 * (size_t)keff, cudaMemcpyHostToDevice, c->stream));
-      double* dst = dev_out ? vecs + (size_t)q * n : tmpv;
-      BK_TRY(bk_launch_lincomb(c, c->Q, nullptr, dst, 0.0, n, keff, coef));
-      if (!dev_out) {
-        BK_CUDA(c, cudaMemcpyAsync(vecs + (size_t)q * n, tmpv, 8 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
-        c->stats.d2h_bytes += 8 * n;
-      }
-      BK_CUDA(c, cudaStreamSynchronize(c->stream));
+      const std::vector<cplx>& y = r.Y[idx[q]];
+      const bool use_im = lam[idx[q]].imag() < 0;
+      for (int i = 0; i < r.keff; ++i) yq[i] = use_im ? y[i].imag() : y[i].real();
+      double* col = vecs + (size_t)q * n;
+      BK_TRY(q_lincomb(c, ws, yq.data(), r.keff, n, dev_out ? col : tmpv, dev_out ? nullptr : col));
     }
   }
   BK_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (nconv) *nconv = converged ? nv : 0;
-  if (nops) *nops = total_ops;
-  return converged ? BK_OK : BK_NOT_CONVERGED;
+  if (nconv) *nconv = r.converged ? nv : 0;
+  if (nops) *nops = r.nops;
+  return r.converged ? BK_OK : BK_NOT_CONVERGED;
 }

@@ -11,19 +11,24 @@
 //                               and, in the same kernel, h_i = <v_i, w> for i <= j (per-CTA partials ->
 //                               deterministic last-block sum).  Algorithmic traffic 8N(j+2) bytes: read u,
 //                               V_1..V_j, write w.  Only real SH2d with an even nx, at most one border and no
-//                               left preconditioner (fuses_jvp); every other operator runs its stand-alone
+//                               left preconditioner (Solve::fuses_jvp); every other operator runs its stand-alone
 //                               apply and then
 //           k2_dots<E>        : h_i = <v_i, w> over w already in memory, 8N(j+1).
 //   pass 2  k2_update<E>      : v'_{j+1} = w - sum_i h_i v_i, ||v'_{j+1}||^2 reduced the same way.
 //                               Algorithmic traffic 8N(j+2): read w, V_1..V_j, write v'_{j+1}.
 //   k_lincomb                 : x = beta x + sum_i y_i s_i v'_i at restart and at the end.
 //
-// Periodic SH2d (BK_SH2D_PERIODIC) with BK_PC_SH_FFT on either side and fused set (fuses_pc): the preconditioned operator of a
-// step is ONE spectral pipeline (bk_periodic_fused: 3 transform kernels, 64N) in place of apply + preconditioner, then k2_dots.
+// Periodic SH2d (BK_SH2D_PERIODIC) with BK_PC_SH_FFT on either side and fused set (Solve::fuses_pc): the preconditioned operator
+// of a step is ONE spectral pipeline (bk_periodic_fused: 3 transform kernels, 64N) in place of apply + preconditioner, then
+// k2_dots.
 //
 // The basis is stored UN-normalised (v'_i) with the scalars s_i = 1/||v'_i|| kept on device, so
 // normalisation costs no memory pass ("deferred as a scalar") and the host never has to be in the
 // loop to launch the next step: Givens rotations run on the host one iteration behind the GPU.
+//
+// Host: plan_solve checks the arguments and makes every per-solve decision once (a Solve); bk_gmres_dev runs the restart
+// loop with the true-residual check; each restart runs one cycle (Arnoldi steps launched ahead, the Givens rotations one
+// column behind) and then update_solution (back substitution, then x += M V' y).
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -129,20 +134,19 @@ static size_t sh2_scratch_bytes(int E) { return sizeof(double) * (size_t)((BK2_R
     default: { constexpr int EE = 8; __VA_ARGS__; } break; \
   }
 
-// Whether the Arnoldi steps of a solve run k2_fused (JVP + dots in one kernel) or the stand-alone apply + k2_dots.  k2_fused
-// tiles one real SH2d grid in TMA rows of an even length and carries at most one border; the operator output must feed the
-// dots directly, so no left preconditioner.  3-D always runs unfused: a ring kernel would gain < 5 % (DESIGN.md §4.4).
-static bool fuses_jvp(const bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o) {
-  const bool left = o->pc_side == BK_SIDE_LEFT && c->pc.kind != BK_PC_NONE;
-  return o->fused && op.kind == BK_SH2D && op.nx % 2 == 0 && !op.cplx && op.bordered <= 1 && !left;
-}
-
-// Whether the Arnoldi steps of a solve apply the preconditioned operator of BK_SH2D_PERIODIC in ONE spectral pipeline
-// (bk_periodic_fused: P (a0 I + a1 J) = P d - a1 I, (a0 I + a1 J) P = d P - a1 I) instead of precond + apply or apply + precond.
-static bool fuses_pc(const bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o) {
-  const bool side = o->pc_side == BK_SIDE_LEFT || o->pc_side == BK_SIDE_RIGHT;
-  return o->fused && op.kind == BK_SH2D_PERIODIC && c->pc.kind == BK_PC_SH_FFT && side && op.bordered == 0 && !op.cplx;
-}
+namespace {
+// One GMRES solve: its operator and size, the restart length clamped to the workspace and to n, and the decisions that hold for
+// the whole solve.  orth is the only field that changes: a failed true-residual check switches a CGS solve to CGS2.
+struct Solve {
+  OpDesc op;
+  long long n;
+  int restart, maxiter;
+  bool left, right;     // a preconditioner is set up and applied on that side
+  bool fuses_jvp, fuses_pc;
+  int orth;
+  std::vector<double> H, g, cs, sn;  // Hessenberg columns after the Givens rotations, rotated rhs, rotations
+};
+}  // namespace
 
 static int launch_fused(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* w, int j, double* hcol) {
   const int tiles_x = (op.nx + BK2_ROW - 1) / BK2_ROW;
@@ -166,9 +170,6 @@ int bk_launch_dots(bk_ctx* c, const double* basis, const double* scales, const d
   BK2_DISPATCH(p.E, return bk_launch(c, k2_dots<EE>, dim3(p.grid), dim3(BK2_THREADS), p.smem, w, n, basis, c->ld, j, scales,
                                      c->partials, c->counters + 1, hcol, gcoef, p.keep, p.NS, p.sred_off));
 }
-static int launch_dots(bk_ctx* c, const double* w, long long n, int j, double* hcol) {
-  return bk_launch_dots(c, c->V, c->scales, w, n, j, hcol, c->gcoef);
-}
 
 int bk_launch_update(bk_ctx* c, const double* basis, const double* gcoef, const double* w, long long n, int j, double* vout,
                      double* h_out, double* scale_out) {
@@ -177,21 +178,43 @@ int bk_launch_update(bk_ctx* c, const double* basis, const double* gcoef, const 
   BK2_DISPATCH(p.E, return bk_launch(c, k2_update<EE>, dim3(p.grid), dim3(BK2_THREADS), p.smem, w, n, basis, c->ld, j, gcoef, vout,
                                      c->partials, c->counters + 2, h_out, scale_out, p.keep, p.NS));
 }
-static int launch_update(bk_ctx* c, const double* w, long long n, int j, double* vout, double* h_out, double* scale_out) {
-  return bk_launch_update(c, c->V, c->gcoef, w, n, j, vout, h_out, scale_out);
-}
 
 int bk_launch_lincomb(bk_ctx* c, const double* basis, const double* scales, double* x, double beta, long long n, int k,
                       const double* coef_dev) {
   return bk_launch_ordered(c, k_lincomb, chunk_grid(n), BK_THREADS, 0, x, beta, n, basis, c->ld, k, coef_dev, scales);
 }
-static int launch_lincomb(bk_ctx* c, double* x, double beta, long long n, int k, const double* coef_dev, bool use_scales) {
-  return bk_launch_lincomb(c, c->V, use_scales ? c->scales : nullptr, x, beta, n, k, coef_dev);
+
+static int plan_solve(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, Solve* s) {
+  s->op = op;
+  const long long n = s->n = op.N + op.bordered;
+  BK_CHECK(c, n <= c->ld, "system larger than the context");
+  // the TMA rows of k2_dots / k2_update are read in pairs: an odd length needs one zero pad element behind it
+  BK_CHECK(c, (n % 2 == 0) || n + 1 <= c->ld, "no pad element left for an odd-sized bordered system");
+  int& restart = s->restart = o->restart;
+  if (restart > c->m) restart = c->m;
+  if ((long long)restart > n) restart = (int)n;
+  BK_CHECK(c, restart >= 1, "restart must be >= 1");
+  BK_CHECK(c, o->pc_side == BK_SIDE_NONE || c->pc.kind != BK_PC_NONE, "pc_side set but no preconditioner was set up");
+  s->maxiter = o->maxiter;
+  s->left = o->pc_side == BK_SIDE_LEFT && c->pc.kind != BK_PC_NONE;
+  s->right = o->pc_side == BK_SIDE_RIGHT && c->pc.kind != BK_PC_NONE;
+  // Whether the Arnoldi steps run k2_fused (JVP + dots in one kernel) or the stand-alone apply + k2_dots.  k2_fused tiles one
+  // real SH2d grid in TMA rows of an even length and carries at most one border; the operator output must feed the dots
+  // directly, so no left preconditioner.  3-D always runs unfused: a ring kernel would gain < 5 % (DESIGN.md §4.4).
+  s->fuses_jvp = o->fused && op.kind == BK_SH2D && op.nx % 2 == 0 && !op.cplx && op.bordered <= 1 && !s->left;
+  // Whether the Arnoldi steps apply the preconditioned operator of BK_SH2D_PERIODIC in ONE spectral pipeline (bk_periodic_fused:
+  // P (a0 I + a1 J) = P d - a1 I, (a0 I + a1 J) P = d P - a1 I) instead of precond + apply or apply + precond.
+  s->fuses_pc = o->fused && op.kind == BK_SH2D_PERIODIC && c->pc.kind == BK_PC_SH_FFT && (s->left || s->right) &&
+                op.bordered == 0 && !op.cplx;
+  s->orth = o->orth;
+  s->H.resize((size_t)(restart + 1) * restart);
+  s->g.resize(restart + 1);
+  s->cs = s->sn = std::vector<double>(restart);
+  return BK_OK;
 }
 
 // One Arnoldi step k (0-based): basis v'_0..v'_k -> v'_{k+1}, H column k on device (+ async copy to pinned host).
-// fuse: fuses_jvp() of the solve; fuse_pc: fuses_pc() of the solve.
-static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, long long n, int k, bool fuse, bool fuse_pc) {
+static int arnoldi_step(bk_ctx* c, const Solve& s, int k) {
   const int j = k + 1;
   const int mh = c->m + 4;
   // The H column is written by the kernels' last CTA straight into pinned, device-mapped host memory (UVA): no
@@ -200,40 +223,39 @@ static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, lon
   double* hcol2 = c->h_pinned + (size_t)(c->m + 1) * mh + (size_t)k * mh;
   const double* in = c->V + (size_t)k * c->ld;
   const double* sp = c->scales + k;
-  const bool left = o->pc_side == BK_SIDE_LEFT && c->pc.kind != BK_PC_NONE;
-  const bool right = o->pc_side == BK_SIDE_RIGHT && c->pc.kind != BK_PC_NONE;
-  if (right && !fuse_pc) {
-    BK_TRY(bk_precond_apply_dev(c, in, c->z, n));
+  if (s.right && !s.fuses_pc) {
+    BK_TRY(bk_precond_apply_dev(c, in, c->z, s.n));
     in = c->z;
   }
   const bool timed = c->timing_now;
   const double* wfin = c->w;
-  if (fuse_pc) {
-    BK_TRY(bk_periodic_fused(c, op, in, sp, c->w, left));
-  } else if (!fuse) {
-    BK_TRY(bk_launch_apply(c, op, in, sp, c->w));
-    if (left) {
-      BK_TRY(bk_precond_apply_dev(c, c->w, c->r, n));
+  if (s.fuses_pc) {
+    BK_TRY(bk_periodic_fused(c, s.op, in, sp, c->w, s.left));
+  } else if (!s.fuses_jvp) {
+    BK_TRY(bk_launch_apply(c, s.op, in, sp, c->w));
+    if (s.left) {
+      BK_TRY(bk_precond_apply_dev(c, c->w, c->r, s.n));
       wfin = c->r;
     }
   }
   if (timed) c->fused_timer.begin(c->stream);
-  BK_TRY(fuse ? launch_fused(c, op, in, sp, c->w, j, hcol) : launch_dots(c, wfin, n, j, hcol));
+  BK_TRY(s.fuses_jvp ? launch_fused(c, s.op, in, sp, c->w, j, hcol)
+                     : bk_launch_dots(c, c->V, c->scales, wfin, s.n, j, hcol, c->gcoef));
   if (timed) c->fused_timer.end(c->stream);
   double* vnext = c->V + (size_t)(k + 1) * c->ld;
   if (timed) c->fused_timer.begin(c->stream);
-  BK_TRY(launch_update(c, wfin, n, j, vnext, hcol + j, c->scales + k + 1));
+  BK_TRY(bk_launch_update(c, c->V, c->gcoef, wfin, s.n, j, vnext, hcol + j, c->scales + k + 1));
   if (timed) c->fused_timer.end(c->stream);
-  if (o->orth == BK_ORTH_CGS2) {
-    BK_TRY(launch_dots(c, vnext, n, j, hcol2));
-    BK_TRY(launch_update(c, vnext, n, j, vnext, hcol + j, c->scales + k + 1));
+  if (s.orth == BK_ORTH_CGS2) {
+    BK_TRY(bk_launch_dots(c, c->V, c->scales, vnext, s.n, j, hcol2, c->gcoef));
+    BK_TRY(bk_launch_update(c, c->V, c->gcoef, vnext, s.n, j, vnext, hcol + j, c->scales + k + 1));
   }
   BK_CUDA(c, cudaEventRecord(c->events[k], c->stream));
   // algorithmic bytes of the step (SURVEY 8d): B(j) = 8N(2j+4); the bordered map reads a and b as well (+16N, "40N" K2')
-  const long long step_bytes = 8LL * n * (2LL * j + 4) + (op.bordered ? 16LL * n : 0LL);
+  const long long step_bytes = 8LL * s.n * (2LL * j + 4) + (s.op.bordered ? 16LL * s.n : 0LL);
   c->stats.last_fused_bytes += step_bytes;
   c->stats.last_fused_launches += 2;
-  if (fuse && (c->timing_now || !c->timing)) {  // with sampled timing the totals cover the timed solves only (bytes and ms must match)
+  if (s.fuses_jvp && (c->timing_now || !c->timing)) {  // with sampled timing the totals cover the timed solves only (bytes and ms must match)
     c->stats.total_fused_bytes += step_bytes;
     c->stats.total_fused_launches += 2;
   }
@@ -241,42 +263,92 @@ static int arnoldi_step(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, lon
 }
 
 // initial (preconditioned) residual -> v'_0, returns beta on the host
-static int init_residual(bk_ctx* c, const OpDesc& op, const bk_gmres_opts* o, long long n, const double* rhs, const double* x,
-                         bool x_zero, double* beta) {
-  const bool left = o->pc_side == BK_SIDE_LEFT && c->pc.kind != BK_PC_NONE;
+static int init_residual(bk_ctx* c, const Solve& s, const double* rhs, const double* x, bool x_zero, double* beta) {
   const double* r = rhs;
   if (!x_zero) {
-    BK_TRY(bk_launch_apply(c, op, x, nullptr, c->w));
-    BK_TRY(bk_dev_axpby(c, c->w, 1.0, rhs, -1.0, n));  // w = rhs - A x
+    BK_TRY(bk_launch_apply(c, s.op, x, nullptr, c->w));
+    BK_TRY(bk_dev_axpby(c, c->w, 1.0, rhs, -1.0, s.n));  // w = rhs - A x
     r = c->w;
   }
-  if (left) {
-    BK_TRY(bk_precond_apply_dev(c, r, c->r, n));
+  if (s.left) {
+    BK_TRY(bk_precond_apply_dev(c, r, c->r, s.n));
     r = c->r;
   }
-  BK_TRY(launch_update(c, r, n, 0, c->V, c->red_out, c->scales));
+  BK_TRY(bk_launch_update(c, c->V, c->gcoef, r, s.n, 0, c->V, c->red_out, c->scales));
   BK_CUDA(c, cudaMemcpyAsync(c->red_pinned, c->red_out, 8, cudaMemcpyDeviceToHost, c->stream));
   BK_CUDA(c, cudaStreamSynchronize(c->stream));
   *beta = c->red_pinned[0];
   return BK_OK;
 }
 
+// One restart cycle from v'_0 with norm beta: the device runs at most two Arnoldi steps ahead of the host, which applies the
+// Givens rotations of each column once its event has fired.  *k is the number of columns kept, *res the residual estimate after
+// the last of them (unchanged when k = 0); *total counts the columns of every cycle.  Speculative steps may still be in flight
+// on return: they only touch gcoef, not coef_pinned.
+static int cycle(bk_ctx* c, Solve& s, double beta, double tol, int* total, int* k, double* res) {
+  const int mh = c->m + 4;
+  std::fill(s.g.begin(), s.g.end(), 0.0);
+  s.g[0] = beta;
+  int kl = 0, kd = 0;
+  while (true) {
+    if (kl < s.restart && *total + (kl - kd) < s.maxiter && kl - kd < 2) {
+      BK_TRY(arnoldi_step(c, s, kl++));
+      continue;
+    }
+    if (kd == kl) break;
+    BK_CUDA(c, cudaEventSynchronize(c->events[kd]));
+    // ---- Givens update of column kd on the host (one step behind the device) ----
+    const double* hc = c->h_pinned + (size_t)kd * mh;
+    const double* hc2 = c->h_pinned + (size_t)(c->m + 1) * mh + (size_t)kd * mh;
+    double* Hk = s.H.data() + (size_t)kd * (s.restart + 1);
+    for (int i = 0; i <= kd; ++i) Hk[i] = hc[i] + (s.orth == BK_ORTH_CGS2 ? hc2[i] : 0.0);
+    const double hk1 = hc[kd + 1];
+    for (int i = 0; i < kd; ++i) {
+      double t = s.cs[i] * Hk[i] + s.sn[i] * Hk[i + 1];
+      Hk[i + 1] = -s.sn[i] * Hk[i] + s.cs[i] * Hk[i + 1];
+      Hk[i] = t;
+    }
+    double d = hypot(Hk[kd], hk1);
+    if (!(d > 0.0) || !std::isfinite(d)) break;  // unusable column (exact breakdown): stop with the columns gathered so far
+    s.cs[kd] = Hk[kd] / d;
+    s.sn[kd] = hk1 / d;
+    Hk[kd] = d;
+    s.g[kd + 1] = -s.sn[kd] * s.g[kd];
+    s.g[kd] = s.cs[kd] * s.g[kd];
+    *res = fabs(s.g[kd + 1]);
+    ++kd;
+    ++*total;
+    if (*res <= tol || *total >= s.maxiter || hk1 == 0.0) break;
+  }
+  *k = kd;
+  return BK_OK;
+}
+
+// x += M V' diag(s) y with R y = g over the first k columns, M the right preconditioner or I (x_zero: x is still all zeros)
+static int update_solution(bk_ctx* c, const Solve& s, int k, double* x, bool x_zero) {
+  double* y = c->coef_pinned;  // in-flight speculative steps only touch gcoef, never coef_pinned
+  for (int i = k - 1; i >= 0; --i) {  // back substitution R y = g
+    double t = s.g[i];
+    for (int q = i + 1; q < k; ++q) t -= s.H[(size_t)q * (s.restart + 1) + i] * y[q];
+    y[i] = t / s.H[(size_t)i * (s.restart + 1) + i];
+  }
+  double* coef_dev = c->hcols2 + (size_t)c->m * (c->m + 4);  // last row of hcols2 is free scratch
+  BK_CUDA(c, cudaMemcpyAsync(coef_dev, c->coef_pinned, 8 * (size_t)k, cudaMemcpyHostToDevice, c->stream));
+  if (s.right) {
+    BK_TRY(bk_launch_lincomb(c, c->V, c->scales, c->w, 0.0, s.n, k, coef_dev));
+    BK_TRY(bk_precond_apply_dev(c, c->w, c->z, s.n));
+    BK_TRY(bk_dev_axpby(c, x, 1.0, c->z, x_zero ? 0.0 : 1.0, s.n));
+  } else {
+    BK_TRY(bk_launch_lincomb(c, c->V, c->scales, x, x_zero ? 0.0 : 1.0, s.n, k, coef_dev));
+  }
+  BK_CUDA(c, cudaStreamSynchronize(c->stream));  // coef_pinned is reused by the next cycle
+  return BK_OK;
+}
+
 int bk_gmres_dev(bk_ctx* c, const OpDesc& op, const double* rhs, double* x, const bk_gmres_opts* o, int* converged,
                  int* iters, double* resnorm) {
-  const long long n = op.N + op.bordered;
-  BK_CHECK(c, n <= c->ld, "system larger than the context");
-  // the TMA rows of k2_dots / k2_update are read in pairs: an odd length needs one zero pad element behind it
-  BK_CHECK(c, (n % 2 == 0) || n + 1 <= c->ld, "no pad element left for an odd-sized bordered system");
-  int restart = o->restart;
-  if (restart > c->m) restart = c->m;
-  if ((long long)restart > n) restart = (int)n;
-  BK_CHECK(c, restart >= 1, "restart must be >= 1");
-  const int maxiter = o->maxiter;
-  const int mh = c->m + 4;
-  const bool right = o->pc_side == BK_SIDE_RIGHT && c->pc.kind != BK_PC_NONE;
-  BK_CHECK(c, o->pc_side == BK_SIDE_NONE || c->pc.kind != BK_PC_NONE, "pc_side set but no preconditioner was set up");
-  const bool fuse = fuses_jvp(c, op, o);
-  const bool fuse_pc = fuses_pc(c, op, o);
+  Solve s;
+  BK_TRY(plan_solve(c, op, o, &s));
   c->stats.last_fused_bytes = 0;
   c->stats.last_fused_launches = 0;
   c->stats.last_fused_ms = 0.0;
@@ -284,114 +356,40 @@ int bk_gmres_dev(bk_ctx* c, const OpDesc& op, const double* rhs, double* x, cons
   c->timing_now = c->timing && (c->solve_count % c->timing_every == 0);
   c->fused_timer.used = 0;  // drop what a failed solve left behind
 
-  BK_CUDA(c, cudaMemsetAsync(x, 0, 8 * (size_t)n, c->stream));  // initially_zero = true (src/LinearSolver.jl:171)
-  bool x_zero = true;
+  BK_CUDA(c, cudaMemsetAsync(x, 0, 8 * (size_t)s.n, c->stream));  // initially_zero = true (src/LinearSolver.jl:171)
+  bool x_zero = true, conv = false;
   int total = 0;
-  bool conv = false;
-  double tol = 0.0, res = 0.0;
-  std::vector<double> H((size_t)(restart + 1) * restart), g(restart + 1), cs(restart), sn(restart), y(restart);
-  bool first = true;
+  double beta = 0, res = 0.0;
+  BK_TRY(init_residual(c, s, rhs, x, x_zero, &beta));
+  const double tol = fmax(o->reltol * beta, o->abstol);
   // Single-pass classical Gram-Schmidt (north_star) can lose orthogonality on long cycles / tight tolerances, and the
   // Givens estimate |g[k+1]| then under-reports the residual (the reference's backend uses modified GS).  A cycle that ends
   // "converged" after >= 40 Krylov vectors or with reltol < 1e-9 is therefore verified against the TRUE residual
-  // (one extra operator application); on failure the solve continues with CGS2 cycles from the current iterate.
-  bk_gmres_opts oo = *o;
-  o = &oo;
-  bool verify_pending = false;
+  // (the next cycle's initial residual); on failure the solve continues with CGS2 cycles from the current iterate.
   while (true) {
-    double beta = 0;
-    BK_TRY(init_residual(c, op, o, n, rhs, x, x_zero, &beta));
-    if (first) {
-      tol = fmax(o->reltol * beta, o->abstol);
-      first = false;
-    }
-    if (verify_pending) {
-      verify_pending = false;
-      if (beta <= 4.0 * tol) {  // rounding slack between the Givens recurrence and the recomputed residual
-        res = beta;
-        conv = true;
-        break;
-      }
-      oo.orth = BK_ORTH_CGS2;
-      c->stats.cgs_fallbacks++;
-    }
     res = beta;
-    if (!(res > tol) || total >= maxiter || !(beta > 0.0)) {
+    if (!(res > tol) || total >= s.maxiter || !(beta > 0.0)) {
       conv = res <= tol;
       break;
     }
-    std::fill(g.begin(), g.end(), 0.0);
-    g[0] = beta;
-    int kl = 0, kd = 0;
-    bool stop = false;
-    while (true) {
-      bool can_launch = kl < restart && (total + (kl - kd)) < maxiter && !stop;
-      if (can_launch && (kl - kd) < 2) {
-        BK_TRY(arnoldi_step(c, op, o, n, kl, fuse, fuse_pc));
-        ++kl;
-        continue;
-      }
-      if (kd == kl) break;
-      BK_CUDA(c, cudaEventSynchronize(c->events[kd]));
-      // ---- Givens update of column kd on the host (one step behind the device) ----
-      const int k = kd;
-      const double* hc = c->h_pinned + (size_t)k * mh;
-      const double* hc2 = c->h_pinned + (size_t)(c->m + 1) * mh + (size_t)k * mh;
-      double* Hk = H.data() + (size_t)k * (restart + 1);
-      for (int i = 0; i <= k; ++i) Hk[i] = hc[i] + (o->orth == BK_ORTH_CGS2 ? hc2[i] : 0.0);
-      double hk1 = hc[k + 1];
-      for (int i = 0; i < k; ++i) {
-        double t = cs[i] * Hk[i] + sn[i] * Hk[i + 1];
-        Hk[i + 1] = -sn[i] * Hk[i] + cs[i] * Hk[i + 1];
-        Hk[i] = t;
-      }
-      double d = hypot(Hk[k], hk1);
-      if (!(d > 0.0) || !std::isfinite(d)) {
-        // unusable column (exact breakdown): stop with the columns gathered so far
-        stop = true;
-        break;
-      }
-      cs[k] = Hk[k] / d;
-      sn[k] = hk1 / d;
-      Hk[k] = d;
-      g[k + 1] = -sn[k] * g[k];
-      g[k] = cs[k] * g[k];
-      res = fabs(g[k + 1]);
-      ++kd;
-      ++total;
-      if (res <= tol || total >= maxiter || hk1 == 0.0) {
-        stop = true;
-        break;
-      }
-    }
-    const int k = kd;
+    int k = 0;
+    BK_TRY(cycle(c, s, beta, tol, &total, &k, &res));
     if (k > 0) {
-      // back substitution R y = g
-      for (int i = k - 1; i >= 0; --i) {
-        double t = g[i];
-        for (int q = i + 1; q < k; ++q) t -= H[(size_t)q * (restart + 1) + i] * y[q];
-        y[i] = t / H[(size_t)i * (restart + 1) + i];
-      }
-      // in-flight speculative steps must not still be reading coef/gcoef: they only touch gcoef, not coef_pinned
-      for (int i = 0; i < k; ++i) c->coef_pinned[i] = y[i];
-      double* coef_dev = c->hcols2 + (size_t)c->m * mh;  // last row of hcols2 is free scratch
-      BK_CUDA(c, cudaMemcpyAsync(coef_dev, c->coef_pinned, 8 * (size_t)k, cudaMemcpyHostToDevice, c->stream));
-      if (right) {
-        BK_TRY(launch_lincomb(c, c->w, 0.0, n, k, coef_dev, true));
-        BK_TRY(bk_precond_apply_dev(c, c->w, c->z, n));
-        BK_TRY(bk_dev_axpby(c, x, 1.0, c->z, x_zero ? 0.0 : 1.0, n));
-      } else {
-        BK_TRY(launch_lincomb(c, x, x_zero ? 0.0 : 1.0, n, k, coef_dev, true));
-      }
-      BK_CUDA(c, cudaStreamSynchronize(c->stream));  // coef_pinned is reused by the next cycle
+      BK_TRY(update_solution(c, s, k, x, x_zero));
       x_zero = false;
     }
     conv = res <= tol;
-    if (conv && oo.orth == BK_ORTH_CGS && (k >= 40 || oo.reltol < 1e-9) && total < maxiter) {
-      verify_pending = true;
-      continue;
+    const bool verify = conv && s.orth == BK_ORTH_CGS && (k >= 40 || o->reltol < 1e-9) && total < s.maxiter;
+    if (!verify && (conv || total >= s.maxiter || k == 0)) break;
+    BK_TRY(init_residual(c, s, rhs, x, x_zero, &beta));
+    if (verify) {
+      if (beta <= 4.0 * tol) {  // rounding slack between the Givens recurrence and the recomputed residual
+        res = beta;
+        break;
+      }
+      s.orth = BK_ORTH_CGS2;
+      c->stats.cgs_fallbacks++;
     }
-    if (conv || total >= maxiter || k == 0) break;
   }
   BK_CUDA(c, cudaStreamSynchronize(c->stream));
   c->stats.total_precond_applies += c->pc_timer.harvest(c->stats.total_precond_ms);
@@ -399,7 +397,7 @@ int bk_gmres_dev(bk_ctx* c, const OpDesc& op, const double* rhs, double* x, cons
     double ms = 0;
     c->fused_timer.harvest(ms);
     c->stats.last_fused_ms = ms;
-    if (fuse) c->stats.total_fused_ms += ms;
+    if (s.fuses_jvp) c->stats.total_fused_ms += ms;
   }
   if (converged) *converged = conv ? 1 : 0;
   if (iters) *iters = total;

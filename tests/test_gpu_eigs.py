@@ -509,12 +509,14 @@ def test_transposed_jacobian_cgl(bk):
 # ------------------------------------------------------------------------------------------------------------- 6. complex contexts
 def test_complex_context_is_refused_before_any_launch(bk):
     """A BK_COMPLEX context's operator is the real-equivalent form of ((-sigma + i a0_imag) I + J): not symmetric, not mapped
-    back by sigma + 1/theta, every eigenvalue twice.  bk_eigs_shift_invert refuses it with BK_ERR_ARG before launching anything."""
+    back by sigma + 1/theta, every eigenvalue twice.  bk_eigs_shift_invert refuses it with BK_ERR_ARG before launching anything.
+    So it does a krylovdim above the context's krylov_m in a real context: the workspace is only grown after every check."""
     dims, L = (8, 6), (8.3, 5.7)
-    ctx = bk.Context(bk.BK_SH2D, dims, L, krylov_m=8, params=(SH_L, SH_NU), complex=True)
-    J = ctx.cjacobian(np.full(ctx.N0, SH_C0))
-    ctx.sync()
-    before = ctx.stats()["kernel_launches"]
-    with pytest.raises(bk.BK200Error, match="BK_COMPLEX"):
-        bk.ShiftInvertB200(0.1, bk.GMRESB200(reltol=1e-10, restart=8, maxiter=80), krylovdim=8)(J, 2)
-    assert ctx.stats()["kernel_launches"] == before
+    for cplx, kd, refusal in ((True, 8, "BK_COMPLEX"), (False, 12, "krylov_m")):
+        ctx = bk.Context(bk.BK_SH2D, dims, L, krylov_m=8, params=(SH_L, SH_NU), complex=cplx)
+        J = ctx.cjacobian(np.full(ctx.N0, SH_C0)) if cplx else ctx.jacobian(np.full(ctx.N, SH_C0))
+        ctx.sync()
+        before = ctx.stats()["kernel_launches"]
+        with pytest.raises(bk.BK200Error, match=refusal):
+            bk.ShiftInvertB200(0.1, bk.GMRESB200(reltol=1e-10, restart=8, maxiter=80), krylovdim=kd)(J, 2)
+        assert ctx.stats()["kernel_launches"] == before, refusal

@@ -8,7 +8,14 @@ runs against any build of the library.  Cases: BK_PC_SH_DCT in 2-D and 3-D at po
 vectors and on vectors offset by one double; the border entries of right-preconditioned matrix-free bordered solves (one border
 and a block of two), which a plain application never has; BK_COMPLEX contexts; BK_PC_CGL_DST on cGL2d and Trapeze contexts;
 BK_PC_POTRAP_CIRC with J' off and on; BK_PC_CHAN_TRIDIAG; BK_PC_SH_FFT with a right-preconditioned periodic GMRES solve.  The
-BK_PC_SH_DCT cases run again in a child process under BK_FFT_NO_FAST=1 (general kernel everywhere; files nofast_*)."""
+BK_PC_SH_DCT cases run again in a child process under BK_FFT_NO_FAST=1 (general kernel everywhere; files nofast_*).
+
+The Krylov drivers (files krylov_*) write x, iters, resnorm and converged of each GMRES solve, the eigenvalues, eigenvectors,
+nconv and nops of each shift-invert solve, and the bk_get_stats counters after each call.  GMRES: SH2d with an even nx (k2_fused)
+and an odd nx (apply + k2_dots), CGS and CGS2, restart below the iteration count, Pl and Pr with BK_PC_SH_DCT, one border and a
+block of two, a solve whose CGS check falls back to CGS2, a BK_COMPLEX solve with an imaginary shift, and periodic SH2d with
+BK_PC_SH_FFT on each side, fused and not.  Eigensolver: SH2d thick restart and cGL2d explicit restart with restarts forced,
+eigenvectors to host and to device memory, and a given start vector."""
 import argparse
 import ctypes as C
 import importlib.util
@@ -17,6 +24,10 @@ import subprocess
 import sys
 
 import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from oracle import problems  # noqa: E402
 
 SH_DCT_2D = [(1024, 1024), (151, 100), (62, 64), (64, 62), (256, 128)]
 SH_DCT_3D = [(64, 64, 64), (48, 32, 16)]
@@ -137,10 +148,98 @@ def others(bk, dump):
         ctx.close()
 
 
+def counters(ctx, name, dump):
+    """the bk_get_stats counters (not the timers) after a call"""
+    dump(name + "_stats", [v for k, v in ctx.stats().items() if not k.endswith("_ms")])
+
+
+def gmres(bk, ctx, J, rhs, name, dump, a0=0.0, a1=1.0, **kw):
+    ls = bk.GMRESB200(**kw)
+    x, cv, it = ls(J, rhs, a0=a0, a1=a1)
+    dump(name, np.concatenate([x, [it, ls.last_resnorm, cv]]))
+    counters(ctx, name, dump)
+
+
+def eigs(bk, ctx, sigma, inner, nev, kd, maxrestart, name, dump, v0=None, device=False):
+    """bk_eigs_shift_invert with the eigenvectors written to host memory or to a device vector"""
+    re, im = np.zeros(nev), np.zeros(nev)
+    vecs = ctx.zeros(nev * ctx.N) if device else np.zeros(nev * ctx.N)
+    nconv, nops = C.c_int32(), C.c_int32()
+    dp = C.POINTER(C.c_double)
+    st = ctx.lib.bk_eigs_shift_invert(ctx.handle, sigma, nev, kd, 1e-8, maxrestart, C.byref(inner.opts()), C.c_void_p(
+        bk.lib.ptr(v0)), re.ctypes.data_as(dp), im.ctypes.data_as(dp), C.c_void_p(bk.lib.ptr(vecs)), C.byref(nconv), C.byref(nops))
+    assert st >= 0, ctx.lib.bk_last_error(ctx.handle)
+    dump(name, np.concatenate([re, im, vecs.numpy() if device else vecs, [st, nconv.value, nops.value]]))
+    counters(ctx, name, dump)
+
+
+def krylov(bk, dump):
+    L = (8 * np.pi, 4 * np.pi / np.sqrt(3))
+    rng = np.random.default_rng(11)
+    for dims in ((256, 128), (255, 96)):  # k2_fused; the stand-alone apply + k2_dots
+        ctx = bk.Context(bk.BK_SH2D, dims, L, krylov_m=60, params=SH_PAR)
+        u = problems.sh2d_sol0(*dims, *L) + 0.1 * rng.standard_normal(ctx.N)
+        J, rhs = ctx.jacobian(u), rng.standard_normal(ctx.N)
+        name = "krylov_sh2d_" + "x".join(map(str, dims))
+        a0 = 0.3 * (1 - 4 / (2 * L[0] / dims[0]) ** 2 - 4 / (2 * L[1] / dims[1]) ** 2) ** 2 + 3.0  # condition number ~5
+        for orth in ("cgs", "cgs2"):  # reltol < 1e-9: every converged CGS cycle is checked against the true residual
+            gmres(bk, ctx, J, rhs, f"{name}_{orth}", dump, a0, -1.0, reltol=1e-10, restart=60, maxiter=200, orth=orth)
+        gmres(bk, ctx, J, rhs, name + "_restart7", dump, a0, -1.0, reltol=1e-10, restart=7, maxiter=200)
+        ctx.precond_setup(bk.BK_PC_SH_DCT, 1.0)
+        for side in ("Pl", "Pr"):
+            gmres(bk, ctx, J, rhs, f"{name}_{side}", dump, 1.0, 1.0, reltol=1e-10, restart=60, maxiter=200, **{side: True})
+        bordered(bk, ctx, u, rng, name, dump)
+        counters(ctx, name + "_bls", dump)
+        ctx.close()
+    dims = (48, 32)  # reltol 1e-13 is below what single-pass CGS attains here: the CGS check fails once and CGS2 takes over
+    ctx = bk.Context(bk.BK_SH2D, dims, L, krylov_m=400, params=SH_PAR)
+    u = problems.sh2d_sol0(*dims, *L) + 0.1 * np.random.default_rng(1).standard_normal(ctx.N)
+    ctx.precond_setup(bk.BK_PC_SH_DCT, 1.0)
+    gmres(bk, ctx, ctx.jacobian(u), np.random.default_rng(7).standard_normal(ctx.N), "krylov_cgs_fallback", dump, 1.0, 1.0,
+          reltol=1e-13, restart=400, maxiter=400, Pr=True)
+    ctx.close()
+    ctx = bk.Context(bk.BK_SH2D, (64, 48), L, krylov_m=60, params=SH_PAR, complex=True)
+    J = ctx.cjacobian(0.3 * rng.standard_normal(ctx.N0))
+    rhs = rng.standard_normal(ctx.N0) + 1j * rng.standard_normal(ctx.N0)
+    ls = bk.ComplexGMRESB200(reltol=1e-10, restart=60, maxiter=300, orth="cgs2")
+    x, cv, it = ls(J, rhs, a0=complex(2.0, -0.7), a1=-1.0)
+    dump("krylov_complex", np.concatenate([x.real, x.imag, [it, ls.last_resnorm, cv]]))
+    counters(ctx, "krylov_complex", dump)
+    ctx.close()
+    ctx = bk.Context(bk.BK_SH2D_PERIODIC, (128, 128), (8 * np.pi, 8 * np.pi), krylov_m=40, params=(-0.15, 1.3))
+    J, rhs = ctx.jacobian(0.3 * rng.standard_normal(ctx.N)), rng.standard_normal(ctx.N)
+    ctx.precond_setup(bk.BK_PC_SH_FFT, 1.0)
+    for side in ("Pl", "Pr"):
+        for fused in (True, False):
+            gmres(bk, ctx, J, rhs, f"krylov_sh_fft_{side}_fused{int(fused)}", dump, reltol=1e-12, restart=40, maxiter=80,
+                  fused=fused, **{side: True})
+    ctx.close()
+
+    dims = (64, 48)
+    ctx = bk.Context(bk.BK_SH2D, dims, L, krylov_m=60, params=SH_PAR)
+    ctx.jacobian(problems.sh2d_sol0(*dims, *L))
+    ctx.precond_setup(bk.BK_PC_SH_DCT, 1.0)
+    inner = bk.GMRESB200(reltol=1e-10, restart=60, maxiter=600, Pr=True)
+    v0 = rng.standard_normal(ctx.N)
+    eigs(bk, ctx, 0.1, inner, 4, 10, 40, "krylov_eigs_thick", dump)  # krylovdim 10: restarted
+    eigs(bk, ctx, 0.1, inner, 4, 10, 40, "krylov_eigs_thick_dev", dump, device=True)
+    eigs(bk, ctx, 0.1, inner, 4, 10, 40, "krylov_eigs_thick_v0", dump, v0=v0)
+    eigs(bk, ctx, 0.1, inner, 4, 10, 40, "krylov_eigs_thick_v0dev", dump, v0=ctx.to_device(v0), device=True)
+    ctx.close()
+    ctx = bk.Context(bk.BK_CGL2D, (12, 8), (np.pi, np.pi / 2), krylov_m=60, params=(1.8, 0.1, 0.3, -1.0, 1.0))
+    ctx.jacobian(0.1 * np.random.default_rng(5).standard_normal(ctx.N))
+    inner = bk.GMRESB200(reltol=1e-12, restart=60, maxiter=2000, orth="cgs2")
+    v0 = rng.standard_normal(ctx.N)
+    eigs(bk, ctx, 0.5, inner, 4, 8, 200, "krylov_eigs_explicit", dump)  # krylovdim 8: restarted
+    eigs(bk, ctx, 0.5, inner, 4, 8, 200, "krylov_eigs_explicit_dev", dump, device=True)
+    eigs(bk, ctx, 0.5, inner, 4, 8, 200, "krylov_eigs_explicit_v0", dump, v0=v0)
+    ctx.close()
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--out", required=True)
-    ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    ap.add_argument("--root", default=ROOT)
     ap.add_argument("--sh-dct-only", action="store_true", help=argparse.SUPPRESS)  # the BK_FFT_NO_FAST child
     a = ap.parse_args()
     bk = load(os.path.abspath(a.root))
@@ -149,6 +248,7 @@ def main():
         return
     sh_dct(bk, Dump(a.out, ""))
     others(bk, Dump(a.out, ""))
+    krylov(bk, Dump(a.out, ""))
     env = dict(os.environ, BK_FFT_NO_FAST="1")  # read once per process by the library
     subprocess.run([sys.executable, os.path.abspath(__file__), "--out", a.out, "--root", a.root, "--sh-dct-only"], env=env, check=True)
     print(f"{len(os.listdir(a.out))} files in {a.out}")
