@@ -208,12 +208,13 @@ struct bk_ctx {
   double* host_pinned = nullptr; // pinned bounce buffer (ld doubles) for pageable host memory
   // generic temporaries for BLS/eigs
   std::vector<double*> tmp;
-  // bk_jet_moments, lazily allocated and grown: staged host vectors (N0 doubles each) and the tuples / results / partials
+  // bk_jet_moments and bk_deflation_moments, lazily allocated and grown: staged host vectors (one row each), the tuples /
+  // results / partials, and the pinned landing buffer of the results (BK_JET_MOMENTS_MAX_TUPLES doubles)
   double* mom_stage = nullptr;
   size_t mom_stage_cap = 0;  // bytes
   void* mom_work = nullptr;
   size_t mom_work_cap = 0;   // bytes
-  double* defl_pinned = nullptr;  // bk_deflation_moments: pinned landing buffer of the results (lazily allocated)
+  double* mom_pinned = nullptr;
   // bk_vec_alloc pool: live allocations (ptr -> padded length) and the recycled free list
   std::unordered_map<double*, size_t> vec_live;
   std::vector<std::pair<size_t, double*>> vec_pool;

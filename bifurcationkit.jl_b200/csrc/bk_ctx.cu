@@ -194,7 +194,7 @@ extern "C" int32_t bk_ctx_destroy(bk_ctx* c) {
     if (b) cudaFree(b);
   if (c->mom_stage) cudaFree(c->mom_stage);
   if (c->mom_work) cudaFree(c->mom_work);
-  if (c->defl_pinned) cudaFreeHost(c->defl_pinned);
+  if (c->mom_pinned) cudaFreeHost(c->mom_pinned);
   if (c->h_pinned) cudaFreeHost(c->h_pinned);
   if (c->red_pinned) cudaFreeHost(c->red_pinned);
   if (c->coef_pinned) cudaFreeHost(c->coef_pinned);

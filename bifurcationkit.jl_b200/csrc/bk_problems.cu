@@ -5,6 +5,12 @@
 //   P3 examples/SH3d.jl:16-53             P4 examples/cGL2d.jl:6-22,262-318
 //   P5 src/periodicorbit/PeriodicOrbitTrapeze.jl:209-330,362-386
 //   bordered map src/LinearBorderSolver.jl:299-335
+// Also the jets d2F / d3F (k_jet) and their contractions (k_jet_moments), which share one per-point form per kind (jet_form),
+// and the deflation moments.  Every cGL2d point, stand-alone or a Trapeze slice, is cgl_point on the one Dirichlet stencil
+// (lap_dirichlet); the Trapeze kernels split their flat index with trap_point, and k_potrap_section writes both the section
+// and the F-cache.  bk_jet_moments and bk_deflation_moments share their host plumbing: staging (stage_rows), the work buffer
+// (moment_work) and the read-back through a pinned buffer (moment_results).
+#include <algorithm>
 #include <cstring>
 
 #include "bk_common.cuh"
@@ -76,40 +82,35 @@ __device__ __forceinline__ void cgl_dnl(const CglPar& p, double u1, double u2, d
   f1 = a11 * d1 + (TR ? a21 : a12) * d2;  // TR: J' (the Laplacian is symmetric, only this 2 x 2 block changes)
   f2 = (TR ? a12 : a21) * d1 + a22 * d2;
 }
-// Dirichlet 5-point Laplacian (zero ghost cells; diagonal -2/h^2 everywhere, examples/cGL2d.jl:12-16)
-__device__ __forceinline__ double lap_dirichlet(const double* __restrict__ a, int i, int j, int nx, int ny, double cx,
-                                                double cy, double s) {
-  long long g = i + (long long)j * nx;
-  double c = a[g];
-  double xm = i > 0 ? a[g - 1] : 0.0, xp = i < nx - 1 ? a[g + 1] : 0.0;
-  double ym = j > 0 ? a[g - nx] : 0.0, yp = j < ny - 1 ? a[g + nx] : 0.0;
-  return s * (cx * (xm - 2.0 * c + xp) + cy * (ym - 2.0 * c + yp));
-}
-// the same stencil on the sum a + b of two fields (one stencil evaluation for the two slices of a J' row)
-__device__ __forceinline__ double lap_dirichlet_sum(const double* __restrict__ a, const double* __restrict__ b, int i, int j,
-                                                    int nx, int ny, double cx, double cy, double s) {
+// Dirichlet 5-point Laplacian (zero ghost cells; diagonal -2/h^2 everywhere, examples/cGL2d.jl:12-16) of the field whose value
+// at point g is at(g): one field, or the sum of two (one stencil evaluation for the two slices of a J' row)
+template <typename At>
+__device__ __forceinline__ double lap_dirichlet(At at, int i, int j, int nx, int ny, double cx, double cy, double s) {
   const long long g = i + (long long)j * nx;
-  const double c = a[g] + b[g];
-  const double xm = i > 0 ? a[g - 1] + b[g - 1] : 0.0, xp = i < nx - 1 ? a[g + 1] + b[g + 1] : 0.0;
-  const double ym = j > 0 ? a[g - nx] + b[g - nx] : 0.0, yp = j < ny - 1 ? a[g + nx] + b[g + nx] : 0.0;
+  const double c = at(g);
+  const double xm = i > 0 ? at(g - 1) : 0.0, xp = i < nx - 1 ? at(g + 1) : 0.0;
+  const double ym = j > 0 ? at(g - nx) : 0.0, yp = j < ny - 1 ? at(g + nx) : 0.0;
   return s * (cx * (xm - 2.0 * c + xp) + cy * (ym - 2.0 * c + yp));
 }
+struct Field {
+  const double* __restrict__ a;
+  __device__ __forceinline__ double operator()(long long g) const { return a[g]; }
+};
+struct FieldSum {
+  const double* __restrict__ a;
+  const double* __restrict__ b;
+  __device__ __forceinline__ double operator()(long long g) const { return a[g] + b[g]; }
+};
 // Vector field / JVP at one grid point of one slice: base pointers to the slice's [u1;u2].
 template <int MODE, bool TR = false>
 __device__ __forceinline__ void cgl_point(const CglPar& p, const double* __restrict__ u, const double* __restrict__ v,
                                           double s, int i, int j, int nx, int ny, double cx, double cy, double& o1,
                                           double& o2) {
-  long long n = (long long)nx * ny, g = i + (long long)j * nx;
-  if (MODE == 1) {
-    double u1 = s * v[g], u2 = s * v[g + n];
-    cgl_nl(p, u1, u2, o1, o2);
-    o1 += lap_dirichlet(v, i, j, nx, ny, cx, cy, s);
-    o2 += lap_dirichlet(v + n, i, j, nx, ny, cx, cy, s);
-  } else {
-    cgl_dnl<TR>(p, u[g], u[g + n], s * v[g], s * v[g + n], o1, o2);
-    o1 += lap_dirichlet(v, i, j, nx, ny, cx, cy, s);
-    o2 += lap_dirichlet(v + n, i, j, nx, ny, cx, cy, s);
-  }
+  const long long n = (long long)nx * ny, g = i + (long long)j * nx;
+  if (MODE == 1) cgl_nl(p, s * v[g], s * v[g + n], o1, o2);
+  else cgl_dnl<TR>(p, u[g], u[g + n], s * v[g], s * v[g + n], o1, o2);
+  o1 += lap_dirichlet(Field{v}, i, j, nx, ny, cx, cy, s);
+  o2 += lap_dirichlet(Field{v + n}, i, j, nx, ny, cx, cy, s);
 }
 __device__ __forceinline__ CglPar cgl_par(const OpDesc& op) {
   CglPar p;
@@ -119,6 +120,21 @@ __device__ __forceinline__ CglPar cgl_par(const OpDesc& op) {
   p.c3 = op.par[3];
   p.c5 = op.par[4];
   return p;
+}
+// Point q < n M of a Trapeze orbit (n = nx ny points, M slices of Ns = 2 n values): grid point g = i + j nx of slice sl, whose
+// first field is at o = sl Ns + g.  i and j are formed where they are used (k_potrap_apply_tr spills if they live longer).
+struct TrapPoint {
+  long long g, o;
+  int sl;
+  __device__ __forceinline__ int i(int nx) const { return (int)(g % nx); }
+  __device__ __forceinline__ int j(int nx) const { return (int)(g / nx); }
+};
+__device__ __forceinline__ TrapPoint trap_point(long long q, long long n) {
+  TrapPoint t;
+  t.g = q % n;
+  t.sl = (int)(q / n);
+  t.o = (long long)t.sl * (2 * n) + t.g;
+  return t;
 }
 
 template <int MODE>
@@ -162,10 +178,9 @@ static __global__ void __launch_bounds__(256) k_potrap_apply(OpDesc op, const do
   const double h2 = 0.5 * T / M, dh2 = 0.5 * dT / M;
   const long long total = n * M;
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
-    long long g = q % n;
-    int sl = (int)(q / n);
-    int i = (int)(g % nx), j = (int)(g / nx);
-    long long o = (long long)sl * Ns + g;
+    const TrapPoint t = trap_point(q, n);
+    const long long g = t.g, o = t.o;
+    const int sl = t.sl, i = t.i(nx), j = t.j(nx);
     if (sl == M - 1) {
       double c1 = s * (in[o] - in[g]), c2 = s * (in[o + n] - in[g + n]);
       out[o] = (MODE == 0) ? op.a0 * s * in[o] + op.a1 * c1 : c1;
@@ -195,36 +210,25 @@ static __global__ void __launch_bounds__(256) k_potrap_apply(OpDesc op, const do
     }
   }
 }
-// F(x_i) for every slice (the cache)
-static __global__ void __launch_bounds__(256) k_potrap_fcache(OpDesc op, const double* __restrict__ x, double* __restrict__ f) {
-  const int nx = op.nx, ny = op.ny, M = op.nz;
-  const long long n = (long long)nx * ny, Ns = 2 * n, total = n * M;
-  const CglPar p = cgl_par(op);
-  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
-    long long g = q % n;
-    int sl = (int)(q / n);
-    double a1, a2;
-    cgl_point<1>(p, nullptr, x + (long long)sl * Ns, 1.0, (int)(g % nx), (int)(g / nx), nx, ny, op.cx, op.cy, a1, a2);
-    f[(long long)sl * Ns + g] = a1;
-    f[(long long)sl * Ns + g + n] = a2;
-  }
-}
-// The section of the phase condition from an orbit x, in one pass over x: phi_i = scale F(x_i) for every slice, xpi = x
-// without the period (updatesection!, PeriodicOrbitTrapeze.jl:665-679: scale = 1/M; re_make :1077-1080: scale = 1)
+// phi_i = scale F(x_i) for every slice and, unless xpi is null, xpi = x without the period, in one pass over x: the section of
+// the phase condition from an orbit x (updatesection!, PeriodicOrbitTrapeze.jl:665-679: scale = 1/M; re_make :1077-1080:
+// scale = 1), or the F-cache at the Jacobian's state (scale = 1, no xpi)
 static __global__ void __launch_bounds__(256) k_potrap_section(OpDesc op, const double* __restrict__ x, double scale,
                                                                double* __restrict__ phi, double* __restrict__ xpi) {
   bk_pdl_sync();
   const int nx = op.nx, ny = op.ny, M = op.nz;
-  const long long n = (long long)nx * ny, Ns = 2 * n, total = n * M;
+  const long long n = (long long)nx * ny, total = n * M;
   const CglPar p = cgl_par(op);
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
-    const long long g = q % n, o = (q / n) * Ns + g;
+    const TrapPoint t = trap_point(q, n);
     double a1, a2;
-    cgl_point<1>(p, nullptr, x + (o - g), 1.0, (int)(g % nx), (int)(g / nx), nx, ny, op.cx, op.cy, a1, a2);
-    phi[o] = scale * a1;
-    phi[o + n] = scale * a2;
-    xpi[o] = x[o];
-    xpi[o + n] = x[o + n];
+    cgl_point<1>(p, nullptr, x + (t.o - t.g), 1.0, t.i(nx), t.j(nx), nx, ny, op.cx, op.cy, a1, a2);
+    phi[t.o] = scale * a1;
+    phi[t.o + n] = scale * a2;
+    if (xpi) {
+      xpi[t.o] = x[t.o];
+      xpi[t.o + n] = x[t.o + n];
+    }
   }
 }
 
@@ -241,18 +245,6 @@ __device__ __forceinline__ double chan_d2Nl(double x, double b) {
 __device__ __forceinline__ double chan_d3Nl(double x, double b) {
   const double h = 1.0 + b * x * x, x2 = x * x;
   return (-6.0 * b - 12.0 * b * x + 36.0 * b * b * x2 + 12.0 * b * b * x2 * x - 6.0 * b * b * b * x2 * x2) / (h * h * h * h);
-}
-// the per-point forms of the scalar kinds at point g, with ab = a[g] b[g] (c[g] is read for ORDER 3 only); chan: alpha = par[0],
-// beta = par[1]
-template <int ORDER>
-__device__ __forceinline__ double chan_jet(double alpha, double beta, double x, double ab, const double* c, long long g) {
-  if (ORDER == 2) return alpha * chan_d2Nl(x, beta) * ab;
-  return alpha * chan_d3Nl(x, beta) * ab * c[g];
-}
-// BK_SH2D, BK_SH3D, BK_SH2D_PERIODIC: F = -L1 u + l u + nu u^2 - u^3
-template <int ORDER>
-__device__ __forceinline__ double sh_jet(double nu, double u, double ab, const double* c, long long g) {
-  return ORDER == 2 ? (2.0 * nu - 6.0 * u) * ab : -6.0 * ab * c[g];
 }
 // cGL2d: NL(A) = (r + i nu) A - (c3 + i mu) |A|^2 A - c5 |A|^4 A (examples/cGL2d.jl:262-279).  With s = |A|^2 and
 // s_xy = 2 Re(x conj y), the forms are real-multilinear (s is not holomorphic):
@@ -286,29 +278,40 @@ __device__ __forceinline__ void cgl_jet(const CglPar& p, double2 A, double2 a, d
   o1 = -(p.c3 * t3.x - p.mu * t3.y) - p.c5 * t5.x;
   o2 = -(p.c3 * t3.y + p.mu * t3.x) - p.c5 * t5.y;
 }
+// The jet of kind KIND at grid point g of pts, from the values there of u, a, b and c (c is read for ORDER 3 only): d2F(u)[a, b]
+// (ORDER 2) or d3F(u)[a, b, c].  KIND is BK_CHAN, BK_CGL2D (double2 values: the pair (u1, u2)) or BK_SH2D for the three SH kinds.
+template <int KIND, int ORDER, typename V>
+__device__ __forceinline__ V jet_form(const OpDesc& op, V u, V a, V b, V c, long long g, long long pts) {
+  if constexpr (KIND == BK_CGL2D) {
+    V o;
+    cgl_jet<ORDER>(cgl_par(op), u, a, b, c, o.x, o.y);
+    return o;
+  } else if constexpr (KIND == BK_CHAN) {  // alpha = par[0], beta = par[1]; the boundary rows are linear
+    const double ab = a * b;
+    const double r = ORDER == 2 ? op.par[0] * chan_d2Nl(u, op.par[1]) * ab : op.par[0] * chan_d3Nl(u, op.par[1]) * ab * c;
+    return g > 0 && g < pts - 1 ? r : 0.0;
+  } else {  // F = -L1 u + l u + nu u^2 - u^3
+    const double ab = a * b;
+    return ORDER == 2 ? (2.0 * op.par[1] - 6.0 * u) * ab : -6.0 * ab * c;
+  }
+}
+// the pair (v[p], v[p + ld]) of a cGL2d point
+__device__ __forceinline__ double2 cgl_pair(const double* v, long long p, long long ld) { return make_double2(v[p], v[p + ld]); }
 template <int ORDER>
 static __global__ void __launch_bounds__(256) k_jet(OpDesc op, const double* u, const double* a, const double* b,
                                                     const double* c, double* out, long long n) {
   bk_pdl_sync();
   for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < n; g += (long long)gridDim.x * blockDim.x) {
     if (op.kind == BK_CGL2D) {
-      const CglPar p = cgl_par(op);
-      const double2 A = make_double2(u[g], u[g + n]);
-      const double2 da = make_double2(a[g], a[g + n]), db = make_double2(b[g], b[g + n]);
-      const double2 dc = ORDER == 3 ? make_double2(c[g], c[g + n]) : make_double2(0.0, 0.0);
-      double o1, o2;
-      cgl_jet<ORDER>(p, A, da, db, dc, o1, o2);
-      out[g] = o1;
-      out[g + n] = o2;
+      const double2 o = jet_form<BK_CGL2D, ORDER>(op, cgl_pair(u, g, n), cgl_pair(a, g, n), cgl_pair(b, g, n),
+                                                  ORDER == 3 ? cgl_pair(c, g, n) : make_double2(0.0, 0.0), g, n);
+      out[g] = o.x;
+      out[g + n] = o.y;
     } else if (op.kind == BK_CHAN) {
-      const double x = u[g];
-      const bool interior = g > 0 && g < n - 1;
-      const double ab = a[g] * b[g];
-      const double r = chan_jet<ORDER>(op.par[0], op.par[1], x, ab, c, g);
-      out[g] = interior ? r : 0.0;
-    } else {  // the SH kinds
-      const double ab = a[g] * b[g];
-      out[g] = sh_jet<ORDER>(op.par[1], u[g], ab, c, g);
+      out[g] = jet_form<BK_CHAN, ORDER>(op, u[g], a[g], b[g], ORDER == 3 ? c[g] : 0.0, g, n);
+    } else {
+      const double ag = a[g], bg = b[g];  // before u[g]: this load order keeps the loop's unrolling and registers
+      out[g] = jet_form<BK_SH2D, ORDER>(op, u[g], ag, bg, ORDER == 3 ? c[g] : 0.0, g, n);
     }
   }
 }
@@ -337,19 +340,13 @@ __device__ __forceinline__ double moment_tile(const OpDesc& op, const double* __
   const double* uu = s_v + urow * LD;
   double s = 0.0;
   for (int p = 0; p < np; ++p) {
-    if (KIND == BK_CGL2D) {
-      double o1, o2;
-      cgl_jet<ORDER>(cgl_par(op), make_double2(uu[p], uu[p + LD]), make_double2(va[p], va[p + LD]),
-                     make_double2(vb[p], vb[p + LD]), ORDER == 3 ? make_double2(vc[p], vc[p + LD]) : make_double2(0.0, 0.0),
-                     o1, o2);
-      s = fma(vi[p], o1, s);
-      s = fma(vi[p + LD], o2, s);
-    } else if (KIND == BK_CHAN) {
-      const long long g = base + p;
-      const double r = chan_jet<ORDER>(op.par[0], op.par[1], uu[p], va[p] * vb[p], vc, p);
-      s = fma(vi[p], g > 0 && g < pts - 1 ? r : 0.0, s);
+    if constexpr (KIND == BK_CGL2D) {
+      const double2 o = jet_form<KIND, ORDER>(op, cgl_pair(uu, p, LD), cgl_pair(va, p, LD), cgl_pair(vb, p, LD),
+                                              ORDER == 3 ? cgl_pair(vc, p, LD) : make_double2(0.0, 0.0), base + p, pts);
+      s = fma(vi[p], o.x, s);
+      s = fma(vi[p + LD], o.y, s);
     } else {
-      s = fma(vi[p], sh_jet<ORDER>(op.par[1], uu[p], va[p] * vb[p], vc, p), s);
+      s = fma(vi[p], jet_form<KIND, ORDER>(op, uu[p], va[p], vb[p], vc[p], base + p, pts), s);
     }
   }
   return s;
@@ -569,9 +566,9 @@ static __global__ void __launch_bounds__(256, 3) k_potrap_apply_tr(OpDesc op, co
   const double* wl = in + (long long)(M - 1) * Ns;
   double acc[1] = {0.0};
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
-    const long long g = q % n;
-    const int sl = (int)(q / n);
-    const long long o = (long long)sl * Ns + g;
+    const TrapPoint t = trap_point(q, n);
+    const long long g = t.g, o = t.o;
+    const int sl = t.sl;
     double r1 = op.phi[o] * wT, r2 = op.phi[o + n] * wT;
     if (sl == M - 1) {
       r1 += s * in[o];
@@ -582,12 +579,12 @@ static __global__ void __launch_bounds__(256, 3) k_potrap_apply_tr(OpDesc op, co
       const double* wn = in + (long long)nk * Ns;
       const double* uk = op.u + (long long)sl * Ns;
       const double* fk = op.fcache + (long long)sl * Ns;
-      const int i = (int)(g % nx), j = (int)(g / nx);
       const double d1 = wk[g] + wn[g], d2 = wk[g + n] + wn[g + n];
       double a1, a2;
       cgl_dnl<true>(p, uk[g], uk[g + n], s * d1, s * d2, a1, a2);
-      a1 += lap_dirichlet_sum(wk, wn, i, j, nx, ny, op.cx, op.cy, s);
-      a2 += lap_dirichlet_sum(wk + n, wn + n, i, j, nx, ny, op.cx, op.cy, s);
+      const int i = t.i(nx), j = t.j(nx);
+      a1 += lap_dirichlet(FieldSum{wk, wn}, i, j, nx, ny, op.cx, op.cy, s);
+      a2 += lap_dirichlet(FieldSum{wk + n, wn + n}, i, j, nx, ny, op.cx, op.cy, s);
       r1 += s * (wk[g] - wn[g]) - h2 * a1;
       r2 += s * (wk[g + n] - wn[g + n]) - h2 * a2;
       if (sl == 0) {
@@ -723,9 +720,9 @@ int bk_launch_apply(bk_ctx* c, const OpDesc& op, const double* in, const double*
 
 int bk_potrap_refresh_cache(bk_ctx* c) {
   if (c->kind != BK_POTRAP_CGL2D) return BK_OK;
-  OpDesc op = bk_make_op(c, 0, 1);
-  return bk_launch_ordered(c, k_potrap_fcache, bk_lin_grid(c, (long long)op.nx * op.ny * op.nz), 256, 0, op, c->u_state,
-                           c->fcache);
+  const OpDesc op = bk_make_op(c, 0, 1);
+  return bk_launch(c, k_potrap_section, bk_lin_grid(c, (long long)op.nx * op.ny * op.nz), 256, 0, op, c->u_state, 1.0, c->fcache,
+                   (double*)nullptr);
 }
 
 // ------------------------------------------------------------------------------------------ C ABI
@@ -777,10 +774,19 @@ extern "C" int32_t bk_jvp(bk_ctx* c, const double* v, double* out, double a0, do
   return bk_stage_out(c, out, c->N, dout);
 }
 
-// d2F (dx3 == nullptr) or d3F at the context's current params; every vector N0 doubles, host or device
-static int jet(bk_ctx* c, const double* u, const double* dx1, const double* dx2, const double* dx3, double* out) {
+// The checks bk_d2f, bk_d3f and bk_jet_moments share, then the jet form (jet_form) of the context's kind in *kind: BK_CHAN,
+// BK_CGL2D, or BK_SH2D for the three SH kinds
+static int jet_kind(bk_ctx* c, int* kind) {
   BK_CHECK(c, bk_kind_traits(c->kind)->has_jets, "d2F / d3F are not available for this problem kind");
   BK_CHECK(c, !c->cplx, "d2F / d3F act on real states: not available in a BK_COMPLEX context");
+  *kind = c->kind == BK_CHAN || c->kind == BK_CGL2D ? c->kind : BK_SH2D;
+  return BK_OK;
+}
+
+// d2F (dx3 == nullptr) or d3F at the context's current params; every vector N0 doubles, host or device
+static int jet(bk_ctx* c, const double* u, const double* dx1, const double* dx2, const double* dx3, double* out) {
+  int kind;
+  BK_TRY(jet_kind(c, &kind));
   const long long n = c->N0;
   double *du, *d1, *d2, *d3 = nullptr, *dout;
   BK_TRY(bk_stage_in(c, u, n, 0, true, &du));
@@ -788,7 +794,8 @@ static int jet(bk_ctx* c, const double* u, const double* dx1, const double* dx2,
   BK_TRY(bk_stage_in(c, dx2, n, 3, true, &d2));
   if (dx3) BK_TRY(bk_stage_in(c, dx3, n, 4, true, &d3));
   BK_TRY(bk_stage_in(c, out, n, 1, false, &dout));
-  const OpDesc op = bk_make_residual_op(c);
+  OpDesc op = bk_make_residual_op(c);
+  op.kind = kind;  // k_jet branches on the jet form
   const long long pts = n / bk_kind_traits(c->kind)->fields;
   if (dx3) BK_TRY(bk_launch(c, k_jet<3>, bk_lin_grid(c, pts), 256, 0, op, du, d1, d2, d3, dout, pts));
   else BK_TRY(bk_launch(c, k_jet<2>, bk_lin_grid(c, pts), 256, 0, op, du, d1, d2, d3, dout, pts));
@@ -822,13 +829,48 @@ static int grow(bk_ctx* c, void** buf, size_t* cap, size_t bytes) {
   return BK_OK;
 }
 
+// The device pointers of the k vectors v[0 .. k-1] of n doubles in d: a host vector is copied into row i of mom_stage (k rows),
+// a device pointer passes through
+static int stage_rows(bk_ctx* c, const double* const* v, int k, long long n, const double** d) {
+  for (int i = 0; i < k; ++i) {
+    d[i] = v[i];
+    if (bk_is_device_ptr(v[i])) continue;
+    BK_TRY(grow(c, (void**)&c->mom_stage, &c->mom_stage_cap, 8 * (size_t)n * k));
+    double* row = c->mom_stage + (size_t)n * i;
+    BK_CUDA(c, cudaMemcpyAsync(row, v[i], 8 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
+    c->stats.h2d_bytes += 8 * n;
+    d[i] = row;
+  }
+  return BK_OK;
+}
+
+// The work buffer of a moment pass, mom_work: `head` bytes from its start (the tuples), then the nres results at *res and the
+// G x nres partials at *part, each 256-byte aligned
+static int moment_work(bk_ctx* c, size_t head, int nres, int G, double** res, double** part) {
+  const size_t res_off = (head + 255) / 256 * 256, part_off = res_off + (8 * (size_t)nres + 255) / 256 * 256;
+  BK_TRY(grow(c, &c->mom_work, &c->mom_work_cap, part_off + 8 * (size_t)nres * G));
+  *res = (double*)((char*)c->mom_work + res_off);
+  *part = (double*)((char*)c->mom_work + part_off);
+  return BK_OK;
+}
+
+// The nres results of a moment pass to the host array out, through the pinned buffer mom_pinned
+static int moment_results(bk_ctx* c, const double* res, int nres, double* out) {
+  static_assert(BK_DEFLATION_MAX_ROOTS * 4 + 3 <= BK_JET_MOMENTS_MAX_TUPLES, "mom_pinned holds any result list");
+  if (!c->mom_pinned) BK_CUDA(c, cudaMallocHost((void**)&c->mom_pinned, 8 * (size_t)BK_JET_MOMENTS_MAX_TUPLES));
+  BK_CUDA(c, cudaMemcpyAsync(c->mom_pinned, res, 8 * (size_t)nres, cudaMemcpyDeviceToHost, c->stream));
+  BK_CUDA(c, cudaStreamSynchronize(c->stream));
+  memcpy(out, c->mom_pinned, 8 * (size_t)nres);
+  c->stats.d2h_bytes += 8 * nres;
+  return BK_OK;
+}
+
 extern "C" int32_t bk_jet_moments(bk_ctx* c, const double* u, int32_t nvec, const double* const* vecs, int32_t n2,
                                   const int32_t* idx2, int32_t n3, const int32_t* idx3, double* out) {
   BK_ENTER(c);
   BkRange nvtx_range("bk_jet_moments");
-  const BkKindTraits* kt = bk_kind_traits(c->kind);
-  BK_CHECK(c, kt->has_jets, "d2F / d3F are not available for this problem kind");
-  BK_CHECK(c, !c->cplx, "d2F / d3F act on real states: not available in a BK_COMPLEX context");
+  int kind;
+  BK_TRY(jet_kind(c, &kind));
   BK_CHECK(c, nvec >= 1 && nvec <= BK_JET_MOMENTS_MAX_VEC, "bk_jet_moments: nvec out of range");
   BK_CHECK(c, n2 >= 0 && n3 >= 0 && (long long)n2 + n3 <= BK_JET_MOMENTS_MAX_TUPLES, "bk_jet_moments: too many tuples");
   BK_CHECK(c, u && vecs && out && (n2 == 0 || idx2) && (n3 == 0 || idx3), "null argument");
@@ -842,46 +884,24 @@ extern "C" int32_t bk_jet_moments(bk_ctx* c, const double* u, int32_t nvec, cons
     tup[t] = make_int4(q[0], q[1], q[2], k == 4 ? q[3] : 0);
   }
   if (ntup == 0) return BK_OK;
-  // host vectors (and u) are staged once, each into its own N0 row of the per-context buffer
-  const long long n = c->N0, pts = n / kt->fields;
-  MomVecs vs;
-  for (int i = 0; i <= nvec; ++i) {
-    const double* p = i < nvec ? vecs[i] : u;
-    if (bk_is_device_ptr(p)) {
-      vs.v[i] = p;
-      continue;
-    }
-    BK_TRY(grow(c, (void**)&c->mom_stage, &c->mom_stage_cap, 8 * (size_t)n * (nvec + 1)));
-    double* row = c->mom_stage + (size_t)n * i;
-    BK_CUDA(c, cudaMemcpyAsync(row, p, 8 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
-    c->stats.h2d_bytes += 8 * n;
-    vs.v[i] = row;
-  }
-  for (int i = nvec + 1; i <= BK_JET_MOMENTS_MAX_VEC; ++i) vs.v[i] = nullptr;
-  // work buffer: tuples | results | partials (G x ntup)
+  const long long n = c->N0, fields = bk_kind_traits(c->kind)->fields, pts = n / fields;
+  MomVecs vs = {};  // the nvec vectors, then u
+  const double* src[BK_JET_MOMENTS_MAX_VEC + 1];
+  std::copy(vecs, vecs + nvec, src);
+  src[nvec] = u;
+  BK_TRY(stage_rows(c, src, nvec + 1, n, vs.v));
   const int G = bk_reduce_grid(c, pts);
-  const size_t tup_bytes = 16 * (size_t)ntup, res_off = (tup_bytes + 255) / 256 * 256;
-  const size_t part_off = res_off + (8 * (size_t)ntup + 255) / 256 * 256;
-  BK_TRY(grow(c, &c->mom_work, &c->mom_work_cap, part_off + 8 * (size_t)ntup * G));
-  char* work = (char*)c->mom_work;
-  BK_CUDA(c, cudaMemcpyAsync(work, tup.data(), tup_bytes, cudaMemcpyHostToDevice, c->stream));
+  const size_t tup_bytes = 16 * (size_t)ntup;
+  double *dres, *dpart;
+  BK_TRY(moment_work(c, tup_bytes, ntup, G, &dres, &dpart));
+  BK_CUDA(c, cudaMemcpyAsync(c->mom_work, tup.data(), tup_bytes, cudaMemcpyHostToDevice, c->stream));
   c->stats.h2d_bytes += tup_bytes;
-  const int4* dtup = (const int4*)work;
-  double* dres = (double*)(work + res_off);
-  double* dpart = (double*)(work + part_off);
   const OpDesc op = bk_make_residual_op(c);
-  const size_t smem = 8 * ((size_t)(nvec + 1) * kt->fields * (BK_MOM_TP + 1) + ntup);
-  if (c->kind == BK_CGL2D)
-    BK_TRY(bk_launch(c, k_jet_moments<BK_CGL2D>, G, 256, smem, op, vs, (int)nvec, dtup, ntup, (int)n2, pts, dpart));
-  else if (c->kind == BK_CHAN)
-    BK_TRY(bk_launch(c, k_jet_moments<BK_CHAN>, G, 256, smem, op, vs, (int)nvec, dtup, ntup, (int)n2, pts, dpart));
-  else
-    BK_TRY(bk_launch(c, k_jet_moments<BK_SH2D>, G, 256, smem, op, vs, (int)nvec, dtup, ntup, (int)n2, pts, dpart));
+  const size_t smem = 8 * ((size_t)(nvec + 1) * fields * (BK_MOM_TP + 1) + ntup);
+  const auto kern = kind == BK_CGL2D ? k_jet_moments<BK_CGL2D> : kind == BK_CHAN ? k_jet_moments<BK_CHAN> : k_jet_moments<BK_SH2D>;
+  BK_TRY(bk_launch(c, kern, G, 256, smem, op, vs, (int)nvec, (const int4*)c->mom_work, ntup, (int)n2, pts, dpart));
   BK_TRY(bk_launch_ordered(c, k_jet_moments_fold, (ntup + 255) / 256, 256, 0, (const double*)dpart, ntup, G, dres));
-  BK_CUDA(c, cudaMemcpyAsync(out, dres, 8 * (size_t)ntup, cudaMemcpyDeviceToHost, c->stream));
-  BK_CUDA(c, cudaStreamSynchronize(c->stream));
-  c->stats.d2h_bytes += 8 * ntup;
-  return BK_OK;
+  return moment_results(c, dres, ntup, out);
 }
 
 extern "C" int32_t bk_deflation_moments(bk_ctx* c, const double* u, int32_t nroots, const double* const* roots, int32_t ndir,
@@ -895,40 +915,25 @@ extern "C" int32_t bk_deflation_moments(bk_ctx* c, const double* u, int32_t nroo
   BK_CHECK(c, u && roots && out && (ndir == 0 || dirs), "null argument");
   for (int i = 0; i < nroots; ++i) BK_CHECK(c, roots[i] != nullptr, "null root");
   for (int a = 0; a < ndir; ++a) BK_CHECK(c, dirs[a] != nullptr, "null direction");
-  // host vectors are staged into rows of n doubles of the per-context buffer bk_jet_moments also uses
+  const double* src[BK_DEFLATION_MAX_ROOTS + 3];  // the roots, the directions, u
+  const double* dev[BK_DEFLATION_MAX_ROOTS + 3];
+  std::copy(roots, roots + nroots, src);
+  std::copy(dirs, dirs + ndir, src + nroots);
+  src[nroots + ndir] = u;
+  BK_TRY(stage_rows(c, src, nroots + ndir + 1, n, dev));
   DeflVecs vs = {};
-  const int nvec = nroots + ndir + 1;
-  for (int i = 0; i < nvec; ++i) {
-    const double* p = i < nroots ? roots[i] : (i < nroots + ndir ? dirs[i - nroots] : u);
-    if (!bk_is_device_ptr(p)) {
-      BK_TRY(grow(c, (void**)&c->mom_stage, &c->mom_stage_cap, 8 * (size_t)n * nvec));
-      double* row = c->mom_stage + (size_t)n * i;
-      BK_CUDA(c, cudaMemcpyAsync(row, p, 8 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
-      c->stats.h2d_bytes += 8 * n;
-      p = row;
-    }
-    if (i < nroots) vs.r[i] = p;
-    else if (i < nroots + ndir) vs.h[i - nroots] = p;
-    else vs.u = p;
-  }
+  std::copy(dev, dev + nroots, vs.r);
+  std::copy(dev + nroots, dev + nroots + ndir, vs.h);
+  vs.u = dev[nroots + ndir];
   const int W = 2 + ndir, ncol = nroots * W + ndir * (ndir + 1) / 2;
   const int G = bk_reduce_grid(c, (n + BK_DEFL_PPT - 1) / BK_DEFL_PPT);
-  const size_t part_off = (8 * (size_t)ncol + 255) / 256 * 256;
-  BK_TRY(grow(c, &c->mom_work, &c->mom_work_cap, part_off + 8 * (size_t)ncol * G));
-  double* dres = (double*)c->mom_work;
-  double* dpart = (double*)((char*)c->mom_work + part_off);
-  if (ndir == 0) BK_TRY(bk_launch(c, k_deflation_moments<0>, G, 256, 0, vs, (int)nroots, (long long)n, dpart));
-  else if (ndir == 1) BK_TRY(bk_launch(c, k_deflation_moments<1>, G, 256, 0, vs, (int)nroots, (long long)n, dpart));
-  else BK_TRY(bk_launch(c, k_deflation_moments<2>, G, 256, 0, vs, (int)nroots, (long long)n, dpart));
+  double *dres, *dpart;
+  BK_TRY(moment_work(c, 0, ncol, G, &dres, &dpart));
+  const auto kern = ndir == 0 ? k_deflation_moments<0> : ndir == 1 ? k_deflation_moments<1> : k_deflation_moments<2>;
+  BK_TRY(bk_launch(c, kern, G, 256, 0, vs, (int)nroots, (long long)n, dpart));
   BK_TRY(bk_launch_ordered(c, k_deflation_moments_fold, (32 * ncol + 255) / 256, 256, 0, (const double*)dpart, ncol, nroots * W, W,
                            G, dres));
-  if (!c->defl_pinned)
-    BK_CUDA(c, cudaMallocHost((void**)&c->defl_pinned, 8 * (size_t)(BK_DEFLATION_MAX_ROOTS * 4 + 3)));
-  BK_CUDA(c, cudaMemcpyAsync(c->defl_pinned, dres, 8 * (size_t)ncol, cudaMemcpyDeviceToHost, c->stream));
-  BK_CUDA(c, cudaStreamSynchronize(c->stream));
-  memcpy(out, c->defl_pinned, 8 * (size_t)ncol);
-  c->stats.d2h_bytes += 8 * ncol;
-  return BK_OK;
+  return moment_results(c, dres, ncol, out);
 }
 
 extern "C" int32_t bk_potrap_set_section(bk_ctx* c, const double* phi, const double* xpi) {

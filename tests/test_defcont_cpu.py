@@ -3,16 +3,14 @@ known answers of test/continuation/simple_continuation.jl:381-431 on host vector
 composed loop, with the moments restated on the host in long double; the closed-form autodiff derivative against a complex
 step; and the sm_90a code of the deflation-moment kernels (read with cuobjdump, no GPU needed)."""
 import collections
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 import __graft_entry__ as g
 from oracle import krylov
+from tests import sass_reader as SR
 from tests.test_normal_form_cpu import dense_eig
 
 
@@ -216,36 +214,11 @@ def test_newton_callback_stops_and_marks_unconverged():
 
 # ------------------------------------------------------------------------------------------------ the kernels in SASS
 def test_deflation_moment_kernels_are_in_the_sm_90a_code_without_local_memory():
-    if shutil.which("cuobjdump") is None:
-        pytest.skip("cuobjdump not on PATH")
-    bk = g.load_package()
-    if not os.path.exists(bk.lib.LIB_PATH):
-        bk.build()
-    out = subprocess.run(["cuobjdump", "-sass", bk.lib.LIB_PATH], capture_output=True, text=True).stdout
-    cnt, cur = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            cnt[cur] = collections.Counter()
-            continue
-        m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(@!?U?P\d+\s+)?([A-Z0-9_.]+)", line)
-        if m and cur:
-            cnt[cur][m.group(2).split(".")[0]] += 1
+    cnt = SR.mnemonics()
     mom = {k: c for k, c in cnt.items() if re.match(r"_Z19k_deflation_momentsILi(0|1|2)E", k)}
     assert len(mom) == 3, sorted(cnt)[:5]                     # 0, 1 and 2 directions
     for k, c in mom.items():
         assert c["LDL"] == 0 and c["STL"] == 0 and c["DFMA"] >= 4 and c["SHFL"] >= 5, (k, dict(c))
     assert any("k_deflation_moments_fold" in k for k in cnt)
-    res = subprocess.run(["cuobjdump", "--dump-resource-usage", bk.lib.LIB_PATH], capture_output=True, text=True).stdout
-    fn, seen = None, 0
-    for line in res.splitlines():
-        m = re.search(r"Function (\S+):", line)
-        if m:
-            fn = m.group(1)
-            continue
-        m = re.search(r"STACK:(\d+)", line)
-        if m and fn and "k_deflation_moments" in fn:
-            assert int(m.group(1)) == 0, (fn, line.strip())
-            seen += 1
-    assert seen == 4
+    usage = {k: u for k, u in SR.resources().items() if "k_deflation_moments" in k}
+    assert all(u.stack == 0 for u in usage.values()) and len(usage) == 4, usage

@@ -2,17 +2,12 @@
 periodic.py) on host arrays: the Stuart-Landau values of the reference's test/normal_forms/testNF.jl:369-450, the complex
 jets composed from real ones, the Trapeze orbits of Stuart-Landau against their closed form, the section hook, and the sm_90a
 code of the section kernel (read with cuobjdump, no GPU needed)."""
-import collections
-import re
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 
 import __graft_entry__ as g
 from oracle import krylov, bls as obls, potrap, problems
-from tests import jets_oracle as JO
+from tests import jets_oracle as JO, sass_reader as SR
 from tests.test_codim2_curves_cpu import NumpyProblem2
 from tests.test_host_logic_cpu import BlsAdapter, DenseComplexProblem, _dense_cls
 from tests.test_normal_form_cpu import dense_eig
@@ -248,22 +243,9 @@ def test_section_hook_after_accepted_steps():
 
 # ------------------------------------------------------------------------------------------------ sm_90a code
 def test_section_kernel_is_in_the_sm_90a_code_without_local_memory():
-    if shutil.which("cuobjdump") is None:
-        pytest.skip("cuobjdump not on PATH")
-    bk = g.load_package()
-    out = subprocess.run(["cuobjdump", "-sass", bk.lib.LIB_PATH], capture_output=True, text=True).stdout
-    cnt, cur = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            cnt[cur] = collections.Counter()
-            continue
-        m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(@!?U?P\d+\s+)?([A-Z0-9_.]+)", line)
-        if m and cur:
-            cnt[cur][m.group(2).split(".")[0]] += 1
+    cnt = SR.mnemonics()
     sec = {k: c for k, c in cnt.items() if "k_potrap_section" in k}
     assert len(sec) == 1
     c = next(iter(sec.values()))
     assert c["LDL"] == 0 and c["STL"] == 0 and c["DFMA"] + c["DMUL"] >= 10, dict(c)
-    assert "arch = sm_90a" in out
+    assert "arch = sm_90a" in SR.cuobjdump("-sass")

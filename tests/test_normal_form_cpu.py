@@ -1,19 +1,15 @@
 """CPU tests of the simple-branch-point normal form and branch switching (bifurcationkit.jl_b200/normalform.py) on host arrays,
 pinned to the reference's test/normal_forms/testNF.jl; the NumPy jets of tests/jets_oracle.py against finite differences of the
 oracle's dF; and the sm_90a code of the jet kernels (read with cuobjdump, no GPU needed)."""
-import collections
 import dataclasses
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 import __graft_entry__ as g
 from oracle import krylov, bls as obls, problems
-from tests import jets_oracle as JO
+from tests import jets_oracle as JO, sass_reader as SR
 from tests.sh_periodic_oracle import PeriodicSH
 from tests.test_codim2_curves_cpu import NumpyProblem2
 from tests.test_host_logic_cpu import BlsAdapter
@@ -228,22 +224,7 @@ def test_rejections_follow_the_reference():
 
 # ------------------------------------------------------------------------------------------------ 7. the jet kernels in SASS
 def test_jet_kernels_are_in_the_sm_90a_code_without_local_memory():
-    if shutil.which("cuobjdump") is None:
-        pytest.skip("cuobjdump not on PATH")
-    bk = g.load_package()
-    if not os.path.exists(bk.lib.LIB_PATH):
-        bk.build()
-    out = subprocess.run(["cuobjdump", "-sass", bk.lib.LIB_PATH], capture_output=True, text=True).stdout
-    cnt, cur = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            cnt[cur] = collections.Counter()
-            continue
-        m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(@!?U?P\d+\s+)?([A-Z0-9_.]+)", line)
-        if m and cur:
-            cnt[cur][m.group(2).split(".")[0]] += 1
+    cnt = SR.mnemonics()
     jets = {k: c for k, c in cnt.items() if re.match(r"_Z5k_jetILi[23]E", k)}
     assert len(jets) == 2, sorted(cnt)[:5]
     for k, c in jets.items():

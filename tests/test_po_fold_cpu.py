@@ -1,17 +1,12 @@
 """CPU tests of the folds of periodic orbits (periodic.continuation_po_events, newton_fold_po, continuation_fold_po) on a host twin
 of the Trapeze problem: the sparse Trapeze Jacobian of tests/potrap_sparse_oracle.py against the Trapeze JVP, the fold of cycles
 of Stuart-Landau against its closed form, and the sm_90a code of the J' kernels (read with cuobjdump, no GPU needed)."""
-import collections
-import re
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 
 import __graft_entry__ as g
 from oracle import krylov, bls as obls, potrap, problems
-from tests import potrap_sparse_oracle as PS
+from tests import potrap_sparse_oracle as PS, sass_reader as SR
 from tests.test_hopf_po_cpu import Fsl, JFsl, SLProblem
 from tests.test_host_logic_cpu import BlsAdapter, DenseComplexProblem, _dense_cls
 from tests.test_normal_form_cpu import dense_eig
@@ -167,35 +162,17 @@ def test_adjoint_kernels_are_in_the_sm_90a_code():
     """k_potrap_apply_tr uses no local memory.  k_potrap_time<true> (the transposed solve), like k_potrap_time<false>, keeps its
     four per-thread arrays of BK_PO_KMAX double2 (the time DFT of one spatial mode) in local memory: it has exactly the forward
     kernel's stack frame, 4096 bytes, with no spills (ptxas reports LOCAL:0, i.e. no spill space) and the same register count"""
-    if shutil.which("cuobjdump") is None:
-        pytest.skip("cuobjdump not on PATH")
-    bk = g.load_package()
-    out = subprocess.run(["cuobjdump", "-sass", bk.lib.LIB_PATH], capture_output=True, text=True).stdout
-    cnt, cur = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            cnt[cur] = collections.Counter()
-            continue
-        m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(@!?U?P\d+\s+)?([A-Z0-9_.]+)", line)
-        if m and cur:
-            cnt[cur][m.group(2).split(".")[0]] += 1
+    cnt = SR.mnemonics()
     tr = [c for k, c in cnt.items() if "k_potrap_apply_tr" in k]
     assert len(tr) == 1
     assert tr[0]["LDL"] == 0 and tr[0]["STL"] == 0 and tr[0]["DFMA"] + tr[0]["DMUL"] >= 20, dict(tr[0])
     time_tr = [c for k, c in cnt.items() if "k_potrap_timeILb1E" in k]   # mangled k_potrap_time<true>
     time = [c for k, c in cnt.items() if "k_potrap_timeILb0E" in k]
     assert len(time_tr) == 1 and len(time) == 1
-    assert "arch = sm_90a" in out
-    res = subprocess.run(["cuobjdump", "-res-usage", bk.lib.LIB_PATH], capture_output=True, text=True).stdout.splitlines()
-    usage = {}
-    for a, b in zip(res, res[1:]):
-        m = re.search(r"Function (\S+):", a)
-        if m and "k_potrap_" in m.group(1):
-            usage[m.group(1)] = dict(re.findall(r"(REG|STACK|LOCAL):(\d+)", b))
+    assert "arch = sm_90a" in SR.cuobjdump("-sass")
+    usage = SR.resources()
     fwd = next(v for k, v in usage.items() if "k_potrap_timeILb0E" in k)
     trn = next(v for k, v in usage.items() if "k_potrap_timeILb1E" in k)
     app = next(v for k, v in usage.items() if "k_potrap_apply_tr" in k)
-    assert trn == fwd and fwd["STACK"] == "4096" and fwd["LOCAL"] == "0", (trn, fwd)
-    assert app["STACK"] == "0" and app["LOCAL"] == "0", app
+    assert trn == fwd and fwd.stack == 4096 and fwd.local == 0, (trn, fwd)
+    assert app.stack == 0 and app.local == 0, app

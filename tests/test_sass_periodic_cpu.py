@@ -1,37 +1,16 @@
 """The periodic transform modes (bk_fft_fast.cuh: k_contig MODE 2 / 3, k_strided MODE 3) are in the sm_90a library, stage their
 tables with bulk copies completing on an mbarrier, and spill nothing to local memory in the instantiations the library launches
 (values per thread E = 4 below n = 1024, E = 8 from 1024 on; bk_precond.cu::fast_loge).  Read with cuobjdump, no GPU needed."""
-import collections
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
-import __graft_entry__ as g
+from tests import sass_reader as SR
 
 
 @pytest.fixture(scope="module")
 def sass():
-    if shutil.which("cuobjdump") is None:
-        pytest.skip("cuobjdump not on PATH")
-    bk = g.load_package()
-    if not os.path.exists(bk.lib.LIB_PATH):
-        bk.build()
-    elfs = subprocess.run(["cuobjdump", "--list-elf", bk.lib.LIB_PATH], capture_output=True, text=True).stdout
-    out = subprocess.run(["cuobjdump", "-sass", bk.lib.LIB_PATH], capture_output=True, text=True).stdout
-    cnt, cur = {}, None
-    for l in out.splitlines():
-        m = re.search(r"Function : (\S+)", l)
-        if m:
-            cur = m.group(1)
-            cnt[cur] = collections.Counter()
-            continue
-        m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(@!?U?P\d+\s+)?([A-Z0-9_.]+)", l)
-        if m and cur:
-            cnt[cur][m.group(2).split(".")[0]] += 1
-    return elfs, cnt
+    return SR.cuobjdump("--list-elf"), SR.mnemonics()
 
 
 def _periodic(cnt):

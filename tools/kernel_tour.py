@@ -29,7 +29,7 @@ c.precond_setup(bk.BK_PC_CGL_DST, 1.0, -0.05)
 for _ in range(2):
     c.residual(u, out); c.jacobian(u); c.jvp(v, out); c.precond_apply(v, out)
 c.sync(); del c
-# Trapeze 512^2 x 30: k_potrap_apply, k_potrap_fcache, k_potrap_phase
+# Trapeze 512^2 x 30: k_potrap_apply, k_potrap_section (the F-cache), k_potrap_phase
 M = 30
 c = bk.Context(bk.BK_POTRAP_CGL2D, (512, 512, M), (np.pi, np.pi / 2), krylov_m=4, params=(1.2, 0.1, 1.0, -1.0, 1.0))
 x = c.to_device(np.concatenate([rng.standard_normal(c.N - 1) * 0.1, [6.3]])); v = c.to_device(rng.standard_normal(c.N)); out = c.zeros()

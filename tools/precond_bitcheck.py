@@ -15,7 +15,14 @@ nconv and nops of each shift-invert solve, and the bk_get_stats counters after e
 and an odd nx (apply + k2_dots), CGS and CGS2, restart below the iteration count, Pl and Pr with BK_PC_SH_DCT, one border and a
 block of two, a solve whose CGS check falls back to CGS2, a BK_COMPLEX solve with an imaginary shift, and periodic SH2d with
 BK_PC_SH_FFT on each side, fused and not.  Eigensolver: SH2d thick restart and cGL2d explicit restart with restarts forced,
-eigenvectors to host and to device memory, and a given start vector."""
+eigenvectors to host and to device memory, and a given start vector.
+
+The problem kernels (files problems_*) write their outputs and the bk_get_stats counters after each call, on host and on device
+vectors: residual and JVP (a0 != 0, a1 != 1) of chan, SH2d (odd and even nx), SH3d, periodic SH2d, cGL2d (J and J'), BK_COMPLEX
+cGL2d with an imaginary shift (J and J'), and Trapeze (J and J' after a section is set, reading the F-cache that
+bk_jac_set_state fills); bls_map / bls_map_block on cGL2d and Trapeze contexts; d2F / d3F of every kind with jets; jet moments
+of chan, SH2d and cGL2d, with more than 64 vectors and more than 8192 tuples; deflation moments with 0, 1 and 2 directions,
+1, 5, 64 and 70 roots, and a prefix n < N0; and potrap_update_section at scale 1/M and 1, each followed by a residual."""
 import argparse
 import ctypes as C
 import importlib.util
@@ -236,6 +243,129 @@ def krylov(bk, dump):
     ctx.close()
 
 
+def problem_kernels(bk, dump):
+    rng = np.random.default_rng(13)
+
+    def both(ctx, name, f, v):
+        """f on a host vector and on a device vector, then the counters"""
+        dump(name + "_host", f(v))
+        dump(name + "_dev", f(ctx.to_device(v)).numpy())
+        counters(ctx, name, dump)
+
+    def res_jvp(ctx, name, u, n=None):
+        n = ctx.N if n is None else n
+        both(ctx, name + "_res", ctx.residual, u)
+        ctx.jacobian(u)
+        both(ctx, name + "_jvp", lambda v: ctx.jvp(v, a0=0.7, a1=-1.3), rng.standard_normal(n))
+
+    def jets(ctx, name):
+        u, a, b, c = (rng.standard_normal(ctx.N0) for _ in range(4))
+        dump(name + "_d2f_host", ctx.d2f(u, a, b))
+        dump(name + "_d3f_host", ctx.d3f(u, a, b, c))
+        du, da, db, dc = (ctx.to_device(x) for x in (u, a, b, c))
+        dump(name + "_d2f_dev", ctx.d2f(du, da, db).numpy())
+        dump(name + "_d3f_dev", ctx.d3f(du, da, db, dc).numpy())
+        counters(ctx, name + "_jets", dump)
+
+    def moments(ctx, name, nvec):
+        u = 0.5 * rng.standard_normal(ctx.N0)
+        vecs = [rng.standard_normal(ctx.N0) for _ in range(nvec)]
+        idx2, idx3 = rng.integers(0, nvec, (40, 3)), rng.integers(0, nvec, (30, 4))
+        dump(name + "_mom_host", ctx.jet_moments(u, vecs, idx2, idx3))
+        dump(name + "_mom_dev", ctx.jet_moments(ctx.to_device(u), [ctx.to_device(v) for v in vecs], idx2, idx3))
+        counters(ctx, name + "_mom", dump)
+
+    L2 = (8 * np.pi, 4 * np.pi / np.sqrt(3))
+    ctx = bk.Context(bk.BK_CHAN, (1000,), (1.0,), krylov_m=4, params=(3.3, 0.01))
+    res_jvp(ctx, "problems_chan", 0.3 * rng.standard_normal(ctx.N))
+    jets(ctx, "problems_chan")
+    moments(ctx, "problems_chan", 5)
+    ctx.close()
+    for dims in ((96, 64), (95, 64)):
+        ctx = bk.Context(bk.BK_SH2D, dims, L2, krylov_m=4, params=SH_PAR)
+        name = "problems_sh2d_" + "x".join(map(str, dims))
+        res_jvp(ctx, name, 0.3 * rng.standard_normal(ctx.N))
+        jets(ctx, name)
+        ctx.close()
+    ctx = bk.Context(bk.BK_SH2D, (64, 48), L2, krylov_m=4, params=SH_PAR)
+    moments(ctx, "problems_sh2d_64x48", 70)  # more than BK_JET_MOMENTS_MAX_VEC vectors: several calls
+    u, vecs = rng.standard_normal(ctx.N0), [rng.standard_normal(ctx.N0) for _ in range(8)]
+    dump("problems_sh2d_mom_tuples", ctx.jet_moments(u, vecs, rng.integers(0, 8, (6000, 3)), rng.integers(0, 8, (4000, 4))))
+    counters(ctx, "problems_sh2d_mom_tuples", dump)
+    ctx.close()
+    ctx = bk.Context(bk.BK_SH3D, (24, 20, 16), (np.pi, 1.3 * np.pi, 0.7 * np.pi), krylov_m=4, params=(0.1, 1.2))
+    res_jvp(ctx, "problems_sh3d", 0.3 * rng.standard_normal(ctx.N))
+    jets(ctx, "problems_sh3d")
+    ctx.close()
+    ctx = bk.Context(bk.BK_SH2D_PERIODIC, (128, 64), (8 * np.pi, 4 * np.pi), krylov_m=4, params=(-0.15, 1.3))
+    res_jvp(ctx, "problems_sh_periodic", 0.3 * rng.standard_normal(ctx.N))
+    jets(ctx, "problems_sh_periodic")
+    ctx.close()
+    ctx = bk.Context(bk.BK_CGL2D, (41, 21), (0.5 * np.pi, np.pi), krylov_m=4, params=CGL_PAR)
+    u = 0.3 * rng.standard_normal(ctx.N)
+    res_jvp(ctx, "problems_cgl", u)
+    ctx.set_transpose(True)
+    both(ctx, "problems_cgl_jvp_tr", lambda v: ctx.jvp(v, a0=0.7, a1=-1.3), rng.standard_normal(ctx.N))
+    ctx.set_transpose(False)
+    jets(ctx, "problems_cgl")
+    moments(ctx, "problems_cgl", 6)
+    J, N = ctx.jacobian(u), ctx.N
+    a, b = rng.standard_normal(N), rng.standard_normal(N)
+    dump("problems_cgl_bls1", bk.bls_map(J, a, b, 0.8, rng.standard_normal(N + 1), shift=-0.5, dotscale=1.0 / N))
+    ab = (rng.standard_normal(N), rng.standard_normal(N))
+    dump("problems_cgl_bls2", bk.bls_map_block(J, ab, (a, b), [[0.9, 0.1], [-0.2, 1.1]], rng.standard_normal(N + 2), shift=-0.5,
+                                                dotscale=1.0 / N))
+    counters(ctx, "problems_cgl_bls", dump)
+    ctx.close()
+    ctx = bk.Context(bk.BK_CGL2D, (24, 12), (np.pi, np.pi / 2), krylov_m=4, params=CGL_PAR, complex=True)
+    u = 0.3 * rng.standard_normal(ctx.N0)
+    both(ctx, "problems_cgl_complex_res", ctx.residual, u)
+    ctx.jacobian(u)
+    ctx.set_shift_imag(-0.6)
+    for tr in (False, True):
+        ctx.set_transpose(tr)
+        both(ctx, f"problems_cgl_complex_jvp_tr{int(tr)}", lambda v: ctx.jvp(v, a0=0.7, a1=-1.3), rng.standard_normal(ctx.N))
+    ctx.close()
+
+    M = 10
+    ctx = bk.Context(bk.BK_POTRAP_CGL2D, (16, 12, M), (np.pi, np.pi / 2), krylov_m=4, params=(1.3,) + CGL_PAR[1:])
+    n = ctx.N - 1
+    x = 0.1 * rng.standard_normal(ctx.N)
+    x[-1] = 6.3
+    ctx.potrap_set_section(rng.standard_normal(n) / np.sqrt(ctx.N), x[:-1])
+    res_jvp(ctx, "problems_potrap", x)  # the JVP reads the F-cache filled by bk_jac_set_state
+    ctx.set_transpose(True)
+    both(ctx, "problems_potrap_jvp_tr", lambda v: ctx.jvp(v, a0=0.7, a1=-1.3), rng.standard_normal(ctx.N))
+    ctx.set_transpose(False)
+    J = ctx.jacobian(x)
+    a, b = rng.standard_normal(ctx.N), rng.standard_normal(ctx.N)
+    dump("problems_potrap_bls1", bk.bls_map(J, a, b, 0.8, rng.standard_normal(ctx.N + 1), shift=-0.5, dotscale=1.0 / ctx.N))
+    ab = (rng.standard_normal(ctx.N), rng.standard_normal(ctx.N))
+    dump("problems_potrap_bls2", bk.bls_map_block(J, ab, (a, b), [[0.9, 0.1], [-0.2, 1.1]], rng.standard_normal(ctx.N + 2),
+                                                  shift=-0.5, dotscale=1.0 / ctx.N))
+    counters(ctx, "problems_potrap_bls", dump)
+    for scale in (1.0 / M, 1.0):
+        for tag, xs in (("host", x), ("dev", ctx.to_device(x))):
+            ctx.potrap_update_section(xs, scale)
+            dump(f"problems_potrap_section_{scale:.2f}_{tag}", ctx.residual(x))
+            counters(ctx, f"problems_potrap_section_{scale:.2f}_{tag}", dump)
+    ctx.close()
+
+    ctx = bk.Context(bk.BK_CHAN, (5000,), (1.0,), krylov_m=4, params=(3.3, 0.01))
+    u = rng.standard_normal(ctx.N0)
+    for nroots in (1, 5, 64, 70):
+        roots = [u + 0.1 * rng.standard_normal(ctx.N0) for _ in range(nroots)]
+        for ndir in (0, 1, 2):
+            dirs = [rng.standard_normal(ctx.N0) for _ in range(ndir)]
+            for n in (ctx.N0, 3001):
+                name = f"problems_defl_r{nroots}_d{ndir}_n{n}"
+                dump(name + "_host", np.concatenate([np.ravel(a) for a in ctx.deflation_moments(u, roots, dirs, n)]))
+                dev = ctx.deflation_moments(ctx.to_device(u), [ctx.to_device(r) for r in roots], [ctx.to_device(h) for h in dirs], n)
+                dump(name + "_dev", np.concatenate([np.ravel(a) for a in dev]))
+                counters(ctx, name, dump)
+    ctx.close()
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--out", required=True)
@@ -249,6 +379,7 @@ def main():
     sh_dct(bk, Dump(a.out, ""))
     others(bk, Dump(a.out, ""))
     krylov(bk, Dump(a.out, ""))
+    problem_kernels(bk, Dump(a.out, ""))
     env = dict(os.environ, BK_FFT_NO_FAST="1")  # read once per process by the library
     subprocess.run([sys.executable, os.path.abspath(__file__), "--out", a.out, "--root", a.root, "--sh-dct-only"], env=env, check=True)
     print(f"{len(os.listdir(a.out))} files in {a.out}")

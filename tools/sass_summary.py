@@ -3,24 +3,15 @@ paths (UBLKCP = cp.async.bulk / TMA bulk copy, SYNCS = mbarrier, FENCE.VIEW.ASYN
 LDS/STS = shared memory, LDG/STG = global, ACQBULK / griddepcontrol = PDL).   python tools/sass_summary.py   (prints the table)"""
 import collections, os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-so = os.path.join(ROOT, "bifurcationkit.jl_b200", "libbk200.so")
-out = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
+sys.path.insert(0, ROOT)
+from tests import sass_reader  # noqa: E402
+so = sass_reader.library()
 dem = lambda s: subprocess.run(["c++filt", s], capture_output=True, text=True).stdout.strip()
-cur, cnt = None, collections.OrderedDict()
-for l in out.splitlines():
-    m = re.search(r"Function : (\S+)", l)
-    if m:
-        cur = m.group(1)
-        cnt[cur] = collections.Counter()
-        continue
-    m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(@!?U?P\d+\s+)?([A-Z0-9_.]+)", l)
-    if m and cur:
-        op = m.group(2)
-        cnt[cur][op.split(".")[0]] += 1
-        if op.startswith("FENCE.VIEW.ASYNC"):
-            cnt[cur]["FENCE.VIEW.ASYNC"] += 1
-        if "ACQBULK" in op or "PREEXIT" in op or op.startswith("ACQ"):
-            cnt[cur]["PDL"] += 1
+cnt = collections.OrderedDict()
+for k, ops in sass_reader.opcodes(sass_reader.cuobjdump("-sass")).items():
+    c = cnt[k] = collections.Counter(op.split(".")[0] for op in ops)
+    c["FENCE.VIEW.ASYNC"] = sum(op.startswith("FENCE.VIEW.ASYNC") for op in ops)
+    c["PDL"] = sum("ACQBULK" in op or "PREEXIT" in op or op.startswith("ACQ") for op in ops)
 KEYS = ["UBLKCP", "UBLKPF", "SYNCS", "FENCE.VIEW.ASYNC", "DFMA", "DADD", "DMUL", "MUFU", "LDS", "STS", "LDG", "STG", "BAR", "LDL", "STL"]
 print(f"# {os.path.relpath(so, ROOT)}: SASS mnemonic counts per kernel (sm_90a), from `cuobjdump -sass`")
 print(f"{'instr':>7} " + " ".join(f"{k[:9]:>9}" for k in KEYS) + "  kernel")
