@@ -10,9 +10,10 @@ branches with the Trapeze functional and branch switching to them from a Hopf po
 diagrams, sibling branches continued concurrently).
 """
 from . import lib
-from .lib import (BK200Error, BK_CHAN, BK_SH2D, BK_SH3D, BK_CGL2D, BK_POTRAP_CGL2D, BK_SH2D_PERIODIC, BK_COMPLEX, BK_PC_NONE,
-                  BK_PC_SH_DCT, BK_PC_CHAN_TRIDIAG, BK_PC_CGL_DST, BK_PC_POTRAP_CIRC, BK_PC_SH_FFT, build)
-from .core import (Context, DeviceVec, Jacobian, TransposedJacobian, ComplexJacobian, GMRESB200, ComplexGMRESB200, BorderingBLSB200, MatrixFreeBLSB200, ShiftInvertB200,
+from .lib import (BK200Error, BK_CHAN, BK_SH2D, BK_SH3D, BK_CGL2D, BK_POTRAP_CGL2D, BK_SH2D_PERIODIC, BK_RD, BK_COMPLEX, BK_PC_NONE,
+                  BK_PC_SH_DCT, BK_PC_CHAN_TRIDIAG, BK_PC_CGL_DST, BK_PC_POTRAP_CIRC, BK_PC_SH_FFT, BK_PC_RD, BK_BC_NEUMANN,
+                  BK_BC_DIRICHLET, build)
+from .core import (Context, ReactionDiffusion, DeviceVec, Jacobian, TransposedJacobian, ComplexJacobian, GMRESB200, ComplexGMRESB200, BorderingBLSB200, MatrixFreeBLSB200, ShiftInvertB200,
                    bls_map, bls_map_block, make_opts, hessenberg_eig)
 from . import palc
 from . import segments

@@ -36,24 +36,80 @@ def _chk(ctx, status):
     return status
 
 
+class ReactionDiffusion:
+    """A reaction-diffusion model for a BK_RD context (bk_rd_model, include/bk200.h): F_i(u) = D_i Lap u_i + R_i(u) for the
+    fields i < `fields`, state [u_1; ..; u_F].
+
+    * bc: "neumann" (the clamp closure of examples/pd-1d.jl) or "dirichlet" (zero ghost cells, examples/cGL2d.jl), or the
+      BK_BC_* value; ndims: 1 or 2.
+    * diffusion: one entry per field, a number D or a pair (scale, pexp) for D = scale * prod_k p_k^pexp[k].
+    * terms: (eq, scale, pexp, fexp) tuples: scale * prod_k p_k^pexp[k] * prod_j u_j^fexp[j] is added to R_eq.  pexp and fexp
+      may be shorter than nparams / fields (missing exponents are 0), or a dict {index: exponent}.
+    * nparams: the length of the parameter tuple.
+    The library checks the model (counts, exponent ranges, indices) when the context is created."""
+
+    def __init__(self, fields, bc, diffusion, terms, nparams, ndims=1):
+        self.fields, self.ndims, self.nparams = int(fields), int(ndims), int(nparams)
+        bcs = {"neumann": _l.BK_BC_NEUMANN, "dirichlet": _l.BK_BC_DIRICHLET}
+        if isinstance(bc, str) and bc not in bcs:
+            raise _l.BK200Error(f"BK_RD: bc must be 'neumann' or 'dirichlet', not {bc!r}")
+        self.bc = bcs[bc] if isinstance(bc, str) else int(bc)
+        self.diffusion = [(float(d), ()) if np.isscalar(d) else (float(d[0]), d[1]) for d in diffusion]
+        self.terms = [(int(eq), float(sc), pe, fe) for eq, sc, pe, fe in terms]
+
+    @staticmethod
+    def _exps(e, n):
+        out = [0] * n
+        for k, v in (e.items() if isinstance(e, dict) else enumerate(e)):
+            if not 0 <= int(k) < n:
+                raise _l.BK200Error(f"BK_RD: exponent index {k} outside [0, {n})")
+            out[int(k)] = int(v)
+        return out
+
+    def c_model(self, complex=False):
+        """the bk_rd_model and its term array (keep both alive for the call)"""
+        if len(self.diffusion) != self.fields:
+            raise _l.BK200Error(f"BK_RD: {len(self.diffusion)} diffusion coefficients for {self.fields} fields")
+        arr = (_l.RdTerm * max(len(self.terms), 1))()
+        for t, (eq, sc, pe, fe) in zip(arr, self.terms):
+            t.eq, t.scale = eq, sc
+            t.pexp[:] = self._exps(pe, _l.BK_RD_MAX_PAR)
+            t.fexp[:] = self._exps(fe, _l.BK_RD_MAX_FIELDS)
+        m = _l.RdModel(fields=self.fields, ndims=self.ndims, bc=self.bc, nparams=self.nparams,
+                       flags=_l.BK_COMPLEX if complex else 0, nterms=len(self.terms))
+        for i, (sc, pe) in enumerate(self.diffusion[:_l.BK_RD_MAX_FIELDS]):
+            m.diff_scale[i] = sc
+            m.diff_pexp[i][:] = self._exps(pe, _l.BK_RD_MAX_PAR)
+        m.terms = arr
+        return m, arr
+
+
 class Context:
     """One per stream: owns the CUDA stream, Krylov workspace and the problem description.  Several contexts may share a
-    device, each used by one host thread at a time (bifdiagram.py runs sibling branches so, each on a `replicate`)."""
+    device, each used by one host thread at a time (bifdiagram.py runs sibling branches so, each on a `replicate`).
+    A BK_RD context takes its `model` (ReactionDiffusion)."""
 
-    def __init__(self, kind, dims, lengths=(1.0, 1.0, 1.0), krylov_m=100, device=0, params=None, complex=False):
+    def __init__(self, kind, dims, lengths=(1.0, 1.0, 1.0), krylov_m=100, device=0, params=None, complex=False, model=None):
         self.lib = _l.load()
         # the vector pool, for a DeviceVec collected on another thread.  Reentrant: a cyclic collection may run, on the thread
         # that holds the lock, between the Python steps around an allocation and finalise a DeviceVec of this context (the
         # library call itself has returned by then, so the pool is never entered twice at once)
         self._vec_lock = threading.RLock()
-        self._args = dict(kind=kind, dims=tuple(dims), lengths=tuple(lengths), krylov_m=krylov_m, device=device, complex=complex)
+        self._args = dict(kind=kind, dims=tuple(dims), lengths=tuple(lengths), krylov_m=krylov_m, device=device, complex=complex,
+                          model=model)
+        self.model = model
         self.precond_calls = []             # the last precond_setup of each kind, (kind, a0, a1, params), in call order
-        if complex:
-            kind |= _l.BK_COMPLEX  # vectors [re; im] of length 2 N0, shifts a0 + i a0_imag (include/bk200.h)
         d = (C.c_int64 * 3)(*(list(dims) + [1, 1, 1])[:3])
         L = (C.c_double * 3)(*(list(lengths) + [1.0, 1.0, 1.0])[:3])
         h = C.c_void_p()
-        st = self.lib.bk_ctx_create(device, kind, d, L, krylov_m, C.byref(h))
+        if kind == _l.BK_RD and model is not None:
+            m, _terms = model.c_model(complex)
+            st = self.lib.bk_rd_ctx_create(device, C.byref(m), d, L, krylov_m, C.byref(h))
+            kind |= _l.BK_COMPLEX if complex else 0
+        else:
+            if complex:
+                kind |= _l.BK_COMPLEX  # vectors [re; im] of length 2 N0, shifts a0 + i a0_imag (include/bk200.h)
+            st = self.lib.bk_ctx_create(device, kind, d, L, krylov_m, C.byref(h))
         self.handle = h
         if st < 0:
             msg = self.lib.bk_last_error(h) if h else b"context allocation failed"
@@ -613,6 +669,14 @@ class ShiftInvertB200:
                                                _l.ptr(vecs) if want_vectors else None, C.byref(nconv), C.byref(nops)))
         vals = re + 1j * im
         return vals, (vecs.T if want_vectors else None), nconv.value >= nev, nops.value
+
+
+def eigsolve(eigsolver, J, nev, vectors):
+    """eigsolver(J, nev) -> (vals, vecs, ...); with `vectors`, a ShiftInvertB200 is asked for its eigenvectors, which it computes
+    only on request (vecs is None otherwise)"""
+    if vectors and isinstance(eigsolver, ShiftInvertB200):
+        return eigsolver(J, nev, want_vectors=True)
+    return eigsolver(J, nev)
 
 
 def hessenberg_eig(H, vectors=True):

@@ -108,6 +108,8 @@ struct Precond {
   // potrap circulant preconditioner
   double2* tdft = nullptr;   // exp(-2 pi i j / (M-1))
   double po_r = 0, po_nu = 0, po_T = 0;
+  // BK_PC_RD: the diffusion coefficients at the params of the set-up
+  double rd_diff[BK_RD_MAX_FIELDS] = {};
 };
 
 // What the host code needs to know about a problem kind.  N0 = fields * dims[0] * ... * dims[ndims - 1] + extra.
@@ -121,7 +123,19 @@ struct BkKindTraits {
   bool pow2_grid;   // Nx and Ny must be powers of two from 64 to 2048
   bool has_jets;    // d2F / d3F available (bk_d2f, bk_d3f)
 };
-const BkKindTraits* bk_kind_traits(int kind);  // nullptr for an unknown kind
+const BkKindTraits* bk_kind_traits(int kind);  // nullptr for an unknown kind and for BK_RD, whose traits depend on its model
+
+// BK_RD: the model's terms with their parameter monomials evaluated at one parameter tuple (bk_set_params), passed by value to
+// the RD kernels (bk_problems.cu).  alpha packs the field exponents of a term, 3 bits per field.
+struct RdTable {
+  int nterms;
+  int bc;  // BK_BC_*
+  double diff[BK_RD_MAX_FIELDS];
+  double coef[BK_RD_MAX_TERMS];
+  int eq[BK_RD_MAX_TERMS];
+  int alpha[BK_RD_MAX_TERMS];
+};
+static_assert(BK_RD_MAX_PAR == BK_MAX_PAR, "an RD model reads the context's parameter tuple");
 
 // CUDA event pairs bracketing intervals on a stream, created on first use and reused from one harvest to the next.
 struct BkEventTimer {
@@ -167,9 +181,10 @@ struct bk_ctx {
   long long l2_bytes = 0;     // L2 cache size of the device (plan2: how many basis vectors a ring pass keeps in L2)
   cudaStream_t stream = nullptr;
   int kind = 0;
+  BkKindTraits kt = {};   // the kind's traits (bk_traits); BK_RD: from its model
   long long dims[3] = {1, 1, 1};
   double lengths[3] = {1, 1, 1};
-  double par[BK_MAX_PAR] = {0};
+  double par[BK_MAX_PAR] = {0};  // written only by bk_store_params
   long long N = 0;        // unknowns (BK_COMPLEX: 2 N0)
   long long N0 = 0;       // size of the real problem: length of the state u and of F(u)
   bool cplx = false;      // BK_COMPLEX context
@@ -181,6 +196,10 @@ struct bk_ctx {
   double* u_state = nullptr;
   double jpar[BK_MAX_PAR] = {0};
   bool have_state = false;
+  // BK_RD: the model (its terms copied) and its table at par (residual, jets) and at jpar (the Jacobian)
+  bk_rd_model rd_model = {};
+  std::vector<bk_rd_term> rd_terms;
+  RdTable rd_par = {}, rd_jpar = {};
   // potrap
   double* phi = nullptr;
   double* xpi = nullptr;
@@ -264,6 +283,9 @@ int bk_fail(bk_ctx* c, int code, const char* what, const char* file, int line);
   } while (0)
 
 // ---- host-side internal API (cross-TU) ----------------------------------------------------------
+static inline const BkKindTraits* bk_traits(const bk_ctx* c) { return &c->kt; }
+// the one writer of c->par: sets its first n entries and what is derived from them (the BK_RD table rd_par)
+void bk_store_params(bk_ctx* c, const double* p, int n);
 // Grid of the 256-thread grid-stride kernels: one CTA per 256 values, at most 8 per SM.
 static inline int bk_lin_grid(const bk_ctx* c, long long n) {
   long long g = (n + 255) / 256;

@@ -1,6 +1,7 @@
 // bk_ctx.cu -- context life cycle, host<->device staging and the S11 vector algebra kernels
 // (BorderedArray / VectorInterface methods of src/BorderedArrays.jl:30-35,53-70,79-217 for a
 // device-resident state vector).
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <map>
@@ -85,8 +86,73 @@ const BkKindTraits* bk_kind_traits(int kind) {
   return &table[kind];
 }
 
-extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dims[3], const double lengths[3],
-                                 int32_t krylov_m, bk_ctx** out) {
+// The checks of an RD model (bk200.h), all before any device work
+static int rd_validate(bk_ctx* c, const bk_rd_model* m) {
+  BK_CHECK(c, m != nullptr, "bk_rd_ctx_create: null model");
+  BK_CHECK(c, m->fields >= 1 && m->fields <= BK_RD_MAX_FIELDS, "BK_RD: fields must be 1 .. 4");
+  BK_CHECK(c, m->ndims == 1 || m->ndims == 2, "BK_RD: ndims must be 1 or 2");
+  BK_CHECK(c, m->bc == BK_BC_NEUMANN || m->bc == BK_BC_DIRICHLET, "BK_RD: bc must be BK_BC_NEUMANN or BK_BC_DIRICHLET");
+  BK_CHECK(c, m->nparams >= 0 && m->nparams <= BK_RD_MAX_PAR, "BK_RD: nparams must be 0 .. 8");
+  BK_CHECK(c, m->flags == 0 || m->flags == BK_COMPLEX, "BK_RD: flags must be 0 or BK_COMPLEX");
+  BK_CHECK(c, m->nterms >= 0 && m->nterms <= BK_RD_MAX_TERMS, "BK_RD: nterms must be 0 .. 64");
+  BK_CHECK(c, m->nterms == 0 || m->terms != nullptr, "BK_RD: null term list");
+  auto pexp_ok = [&](const int32_t* e) {
+    for (int k = 0; k < BK_RD_MAX_PAR; ++k) {
+      if (e[k] < -BK_RD_MAX_PEXP || e[k] > BK_RD_MAX_PEXP) return 1;
+      if (k >= m->nparams && e[k] != 0) return 2;
+    }
+    return 0;
+  };
+  for (int i = 0; i < m->fields; ++i) {
+    const int e = pexp_ok(m->diff_pexp[i]);
+    BK_CHECK(c, e != 1, "BK_RD: a diffusion parameter exponent is outside [-4, 4]");
+    BK_CHECK(c, e != 2, "BK_RD: a diffusion coefficient reads a parameter index >= nparams");
+    BK_CHECK(c, std::isfinite(m->diff_scale[i]), "BK_RD: a diffusion scale is not finite");
+  }
+  for (int t = 0; t < m->nterms; ++t) {
+    const bk_rd_term& tm = m->terms[t];
+    BK_CHECK(c, tm.eq >= 0 && tm.eq < m->fields, "BK_RD: a term's equation index is outside [0, fields)");
+    BK_CHECK(c, std::isfinite(tm.scale), "BK_RD: a term's scale is not finite");
+    const int e = pexp_ok(tm.pexp);
+    BK_CHECK(c, e != 1, "BK_RD: a term's parameter exponent is outside [-4, 4]");
+    BK_CHECK(c, e != 2, "BK_RD: a term reads a parameter index >= nparams");
+    int deg = 0;
+    for (int j = 0; j < BK_RD_MAX_FIELDS; ++j) {
+      BK_CHECK(c, tm.fexp[j] >= 0 && tm.fexp[j] <= BK_RD_MAX_DEGREE, "BK_RD: a term's field exponent is outside [0, 5]");
+      BK_CHECK(c, j < m->fields || tm.fexp[j] == 0, "BK_RD: a term has an exponent on a field index >= fields");
+      deg += tm.fexp[j];
+    }
+    BK_CHECK(c, deg <= BK_RD_MAX_DEGREE, "BK_RD: a term's degree |alpha| is above 5");
+  }
+  return BK_OK;
+}
+
+// The RD table at the parameter tuple p: every parameter monomial evaluated, the field exponents packed 3 bits per field
+static void rd_eval(const bk_ctx* c, const double* p, RdTable* t) {
+  const bk_rd_model& m = c->rd_model;
+  auto mono = [&](double s, const int32_t* e) {
+    for (int k = 0; k < m.nparams; ++k) {
+      for (int r = 0; r < e[k]; ++r) s *= p[k];
+      for (int r = 0; r < -e[k]; ++r) s /= p[k];
+    }
+    return s;
+  };
+  *t = RdTable{};
+  t->nterms = m.nterms;
+  t->bc = m.bc;
+  for (int i = 0; i < m.fields; ++i) t->diff[i] = mono(m.diff_scale[i], m.diff_pexp[i]);
+  for (int k = 0; k < m.nterms; ++k) {
+    const bk_rd_term& tm = c->rd_terms[k];
+    t->coef[k] = mono(tm.scale, tm.pexp);
+    t->eq[k] = tm.eq;
+    int a = 0;
+    for (int j = 0; j < m.fields; ++j) a |= tm.fexp[j] << (3 * j);
+    t->alpha[k] = a;
+  }
+}
+
+static int ctx_create(int32_t device, int32_t kind, const bk_rd_model* model, const int64_t dims[3], const double lengths[3],
+                      int32_t krylov_m, bk_ctx** out) {
   if (!out) return BK_ERR_ARG;
   *out = nullptr;
   bk_ctx* c = new (std::nothrow) bk_ctx();
@@ -100,8 +166,24 @@ extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dim
     c->dims[i] = dims ? (dims[i] > 0 ? dims[i] : 1) : 1;
     c->lengths[i] = lengths ? lengths[i] : 1.0;
   }
-  const BkKindTraits* kt = bk_kind_traits(kind);
-  if (!kt) return bk_fail(c, BK_ERR_ARG, "unknown problem kind", __FILE__, __LINE__);
+  if (kind == BK_RD) {
+    BK_CHECK(c, model != nullptr, "BK_RD contexts are created by bk_rd_ctx_create (the model describes the problem)");
+    BK_TRY(rd_validate(c, model));
+    c->rd_model = *model;
+    c->rd_terms.assign(model->terms, model->terms + model->nterms);
+    c->rd_model.terms = c->rd_terms.data();
+    for (int d = model->ndims; d < 3; ++d)
+      BK_CHECK(c, c->dims[d] == 1, "BK_RD: dims has more grid dimensions than the model's ndims");
+    //          ndims          fields         extra jac_sym              has_jt complex_ok pow2_grid has_jets
+    c->kt = {model->ndims, model->fields, 0, model->fields == 1, true, true, false, true};
+    rd_eval(c, c->par, &c->rd_par);
+    c->rd_jpar = c->rd_par;
+  } else {
+    const BkKindTraits* kt = bk_kind_traits(kind);
+    if (!kt) return bk_fail(c, BK_ERR_ARG, "unknown problem kind", __FILE__, __LINE__);
+    c->kt = *kt;
+  }
+  const BkKindTraits* kt = &c->kt;
   if (kt->pow2_grid)
     for (int d = 0; d < 2; ++d) {
       const long long v = c->dims[d];
@@ -176,6 +258,16 @@ extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dim
   return BK_OK;
 }
 
+extern "C" int32_t bk_ctx_create(int32_t device, int32_t kind, const int64_t dims[3], const double lengths[3],
+                                 int32_t krylov_m, bk_ctx** out) {
+  return ctx_create(device, kind, nullptr, dims, lengths, krylov_m, out);
+}
+
+extern "C" int32_t bk_rd_ctx_create(int32_t device, const bk_rd_model* model, const int64_t dims[3], const double lengths[3],
+                                    int32_t krylov_m, bk_ctx** out) {
+  return ctx_create(device, BK_RD | (model ? model->flags : 0), model, dims, lengths, krylov_m, out);
+}
+
 extern "C" int32_t bk_ctx_destroy(bk_ctx* c) {
   if (!c) return BK_OK;
   cudaSetDevice(c->device);
@@ -212,10 +304,15 @@ extern "C" int32_t bk_ctx_destroy(bk_ctx* c) {
 extern "C" const char* bk_last_error(bk_ctx* c) { return c ? c->err.c_str() : "null context"; }
 extern "C" int64_t bk_problem_size(bk_ctx* c) { return c ? c->N : 0; }
 extern "C" int64_t bk_state_size(bk_ctx* c) { return c ? c->N0 : 0; }
+void bk_store_params(bk_ctx* c, const double* p, int n) {
+  for (int i = 0; i < n; ++i) c->par[i] = p[i];
+  if (c->kind == BK_RD) rd_eval(c, c->par, &c->rd_par);
+}
 extern "C" int32_t bk_set_params(bk_ctx* c, const double* p, int32_t n) {
   BK_ENTER(c);
   BK_CHECK(c, p && n >= 0 && n <= BK_MAX_PAR, "bad params");
-  for (int i = 0; i < n; ++i) c->par[i] = p[i];
+  BK_CHECK(c, c->kind != BK_RD || n >= c->rd_model.nparams, "BK_RD: bk_set_params needs the model's nparams values");
+  bk_store_params(c, p, n);
   return BK_OK;
 }
 extern "C" int32_t bk_get_stats(bk_ctx* c, bk_stats* out) {

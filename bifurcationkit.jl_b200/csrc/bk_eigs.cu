@@ -455,7 +455,7 @@ extern "C" int32_t bk_eigs_shift_invert(bk_ctx* c, double sigma, int32_t nev, in
   // partial-sum buffer must hold m rows
   BK_CHECK(c, m <= c->m, "krylovdim exceeds the context's krylov_m (partial-sum workspace)");
   if (maxrestart < 1) maxrestart = 1;
-  const bool sym = bk_kind_traits(c->kind)->jac_sym;
+  const bool sym = bk_traits(c)->jac_sym;
   EigWork ws;
   BK_TRY(eig_work(c, m, sym, &ws));
   double* x;

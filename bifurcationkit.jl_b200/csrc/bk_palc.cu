@@ -149,7 +149,7 @@ extern "C" int32_t bk_palc_run(bk_ctx* c, const bk_palc_opts* po, const bk_gmres
   } catch (const std::exception& f) {
     status = bk_fail(c, BK_ERR_STATE, f.what(), __FILE__, __LINE__);
   }
-  memcpy(c->par, saved_par, sizeof saved_par);  // the caller's parameter tuple is left as it was
+  bk_store_params(c, saved_par, BK_MAX_PAR);  // the caller's parameter tuple (and what derives from it) is left as it was
   if (status == BK_OK && u_final && df != u_final) status = bk_vec_download(c, u_final, df, N);
   if (d0 != u0) bk_vec_free(c, d0);
   if (d1 && d1 != u1) bk_vec_free(c, d1);

@@ -47,6 +47,21 @@ static __global__ void __launch_bounds__(256) k_helmholtz_symbol_div(double* __r
     a[q] = a[q] / (a0 + a1 * (lx[i] + ly[j]));
   }
 }
+// BK_PC_RD: field f of the transformed blocks divided by a0 + a1 D_f (lx + ly) (times scale: 1 / prod 2 n_d for the DCT-II)
+struct RdDiff {
+  double d[BK_RD_MAX_FIELDS];
+};
+static __global__ void __launch_bounds__(256) k_rd_symbol_div(double* __restrict__ a, int nx, int ny, int fields,
+                                                              const double* __restrict__ lx, const double* __restrict__ ly,
+                                                              double a0, double a1, RdDiff D, double scale) {
+  const long long n = (long long)nx * ny, total = n * fields;
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
+    const long long g = q % n;
+    const int f = (int)(q / n), i = (int)(g % nx), j = (int)(g / nx);
+    const double df = f == 0 ? D.d[0] : f == 1 ? D.d[1] : f == 2 ? D.d[2] : D.d[3];
+    a[q] = a[q] * scale / (a0 + a1 * df * (lx[i] + (ly ? ly[j] : 0.0)));
+  }
+}
 
 // ---- potrap circulant preconditioner: time direction -------------------------------------------------------------------
 // B holds the DST-I coefficients of all 2M slice components (field f = 2*slice + comp, n values each).  One thread per
@@ -308,8 +323,8 @@ void line_free(Line& ln) {
     if (t) cudaFree(t);
 }
 
-// dimension d of a grid Laplacian. type 0: DCT-II (Neumann), 1: DST-I (Dirichlet)
-static int setup_dim(bk_ctx* c, int d, int type) {
+// the eigenvalues of dimension d of a grid Laplacian. type 0: DCT-II (Neumann), 1: DST-I (Dirichlet)
+static std::vector<double> dim_eigenvalues(const bk_ctx* c, int d, int type) {
   const long long n = c->dims[d];
   const double inv_h2 = bk_inv_h2(c, d);
   std::vector<double> lam(n);
@@ -317,8 +332,10 @@ static int setup_dim(bk_ctx* c, int d, int type) {
   for (long long k = 0; k < n; ++k)
     lam[k] = (type == 0) ? (double)((2.0L * cosl(PI * k / n) - 2.0L)) * inv_h2
                          : (double)(-(2.0L - 2.0L * cosl(PI * (k + 1) / (n + 1)))) * inv_h2;
-  return line_setup(c, c->pc.line[d], type, lam, true);
+  return lam;
 }
+// the transform of dimension d of a grid Laplacian
+static int setup_dim(bk_ctx* c, int d, int type) { return line_setup(c, c->pc.line[d], type, dim_eigenvalues(c, d, type), true); }
 
 // ---- BK_SH2D_PERIODIC: real 2-D FFT pipeline -------------------------------------------------------------------------------
 // Tables for both dimensions are built once at bk_ctx_create: every operator application (residual, JVP, preconditioner, the
@@ -382,7 +399,7 @@ extern "C" int32_t bk_precond_setup(bk_ctx* c, int32_t kind, double a0, double a
   if (!pc.work2) BK_CUDA(c, cudaMalloc(&pc.work2, 8 * (size_t)c->ld));
   if (kind == BK_PC_SH_DCT) {
     BK_CHECK(c, c->kind == BK_SH2D || c->kind == BK_SH3D, "BK_PC_SH_DCT needs a Swift-Hohenberg context");
-    for (int d = 0; d < bk_kind_traits(c->kind)->ndims; ++d) BK_TRY(setup_dim(c, d, 0));
+    for (int d = 0; d < bk_traits(c)->ndims; ++d) BK_TRY(setup_dim(c, d, 0));
   } else if (kind == BK_PC_SH_FFT) {
     BK_CHECK(c, c->kind == BK_SH2D_PERIODIC, "BK_PC_SH_FFT needs a BK_SH2D_PERIODIC context");
     BK_CHECK(c, a0 > 0, "BK_PC_SH_FFT: a0 must be > 0 (the symbol of L1 vanishes at |k| = 1)");
@@ -403,6 +420,23 @@ extern "C" int32_t bk_precond_setup(bk_ctx* c, int32_t kind, double a0, double a
     pc.po_T = a0;
     pc.po_r = c->par[0];   // (r, mu, nu, c3, c5)
     pc.po_nu = c->par[2];
+  } else if (kind == BK_PC_RD) {
+    BK_CHECK(c, c->kind == BK_RD, "BK_PC_RD needs a BK_RD context");
+    const int nd = bk_traits(c)->ndims, type = c->rd_model.bc == BK_BC_DIRICHLET ? 1 : 0;
+    std::vector<double> lam[2] = {dim_eigenvalues(c, 0, type), nd == 2 ? dim_eigenvalues(c, 1, type) : std::vector<double>(1, 0.0)};
+    // a vanishing symbol a0 + a1 D_f lambda has no inverse; one that cancels to rounding level is treated as vanishing.  Every
+    // field is checked before anything of the context's preconditioner changes, so a refused set-up leaves the previous one intact
+    for (int f = 0; f < bk_traits(c)->fields; ++f) {
+      const double df = c->rd_par.diff[f];
+      for (double ly : lam[1])
+        for (double lx : lam[0]) {
+          const double t = a1 * df * (lx + ly);
+          BK_CHECK(c, std::isfinite(a0 + t) && fabs(a0 + t) > 1e-13 * (fabs(a0) + fabs(t)),
+                   "BK_PC_RD: the symbol a0 + a1 D_i lambda vanishes for a mode of the grid (no inverse)");
+        }
+    }
+    for (int d = 0; d < nd; ++d) BK_TRY(setup_dim(c, d, type));
+    for (int f = 0; f < bk_traits(c)->fields; ++f) pc.rd_diff[f] = c->rd_par.diff[f];
   } else if (kind == BK_PC_CHAN_TRIDIAG) {
     BK_CHECK(c, c->kind == BK_CHAN, "BK_PC_CHAN_TRIDIAG needs a chan context");
     long long n = c->N0;
@@ -523,7 +557,7 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
   if (timed) c->pc_timer.begin(c->stream);
   const bool al = aligned16(in, out);
   if (pc.kind == BK_PC_SH_DCT) {
-    const int nd = bk_kind_traits(c->kind)->ndims;
+    const int nd = bk_traits(c)->ndims;
     const int nx = (int)c->dims[0], ny = (int)c->dims[1], nz = nd == 3 ? (int)c->dims[2] : 1;
     double scale = 1.0;
     for (int d = 0; d < nd; ++d) scale /= 2.0 * (double)c->dims[d];
@@ -560,6 +594,17 @@ static int precond_apply_one(bk_ctx* c, const double* in, double* out, long long
       BK_CUDA(c, cudaMemcpyAsync(out + (M - 1) * Ns, in + (M - 1) * Ns, 8 * (size_t)(Ns + 1), cudaMemcpyDeviceToDevice, c->stream));
     else
       BK_TRY(bk_launch_ordered(c, k_potrap_close, (unsigned)((Ns + 255) / 256), 256, 0, in, out, Ns, M));
+  } else if (pc.kind == BK_PC_RD) {
+    const int nd = bk_traits(c)->ndims, nx = (int)c->dims[0], ny = (int)c->dims[1], F = bk_traits(c)->fields;
+    double scale = 1.0;
+    if (c->rd_model.bc == BK_BC_NEUMANN)
+      for (int d = 0; d < nd; ++d) scale /= 2.0 * (double)c->dims[d];
+    RdDiff D;
+    for (int f = 0; f < BK_RD_MAX_FIELDS; ++f) D.d[f] = pc.rd_diff[f];
+    BK_TRY(spectral_solve(c, nd, nx, ny, F, in, out, n, al, nullptr, [&](double* v) {
+      return bk_launch_ordered(c, k_rd_symbol_div, bk_lin_grid(c, N), 256, 0, v, nx, ny, F, ln[0].lam, nd == 2 ? ln[1].lam : nullptr,
+                               pc.a0, pc.a1, D, scale);
+    }));
   } else if (pc.kind == BK_PC_CHAN_TRIDIAG) {
     BK_TRY(bk_launch_ordered(c, k_thomas, 1, 32, 0, pc.tri, in, out, (int)N));
   }

@@ -351,11 +351,12 @@ __device__ __forceinline__ double moment_tile(const OpDesc& op, const double* __
   }
   return s;
 }
-template <int KIND>
-static __global__ void __launch_bounds__(256) k_jet_moments(OpDesc op, MomVecs vs, int nvec, const int4* __restrict__ tup,
-                                                            int ntup, int n2, long long pts, double* __restrict__ partials) {
-  bk_pdl_sync();
-  constexpr int F = KIND == BK_CGL2D ? 2 : 1, LD = BK_MOM_TP + 1;
+// The pass of a moment kernel over the tiles, for F fields per point: tile2 / tile3 (s_v, q, urow, np, base) return the sum of an
+// order-2 / order-3 tuple q over the np points of the tile that starts at point base
+template <int F, class Tile2, class Tile3>
+__device__ __forceinline__ void jet_moments_pass(const MomVecs& vs, int nvec, const int4* __restrict__ tup, int ntup, int n2,
+                                                 long long pts, double* __restrict__ partials, Tile2 tile2, Tile3 tile3) {
+  constexpr int LD = BK_MOM_TP + 1;
   extern __shared__ double smem[];
   const int rows = (nvec + 1) * F;
   double* s_v = smem;                // rows x LD: row (vector, field), u last
@@ -373,11 +374,20 @@ static __global__ void __launch_bounds__(256) k_jet_moments(OpDesc op, MomVecs v
     __syncthreads();
     for (int t = threadIdx.x; t < ntup; t += blockDim.x) {
       const int4 q = tup[t];
-      s_acc[t] += t < n2 ? moment_tile<KIND, 2>(op, s_v, q, nvec * F, np, base, pts)
-                         : moment_tile<KIND, 3>(op, s_v, q, nvec * F, np, base, pts);
+      s_acc[t] += t < n2 ? tile2(s_v, q, nvec * F, np, base) : tile3(s_v, q, nvec * F, np, base);
     }
   }
   for (int t = threadIdx.x; t < ntup; t += blockDim.x) partials[(size_t)blockIdx.x * ntup + t] = s_acc[t];
+}
+template <int KIND>
+static __global__ void __launch_bounds__(256) k_jet_moments(OpDesc op, MomVecs vs, int nvec, const int4* __restrict__ tup,
+                                                            int ntup, int n2, long long pts, double* __restrict__ partials) {
+  bk_pdl_sync();
+  constexpr int F = KIND == BK_CGL2D ? 2 : 1;
+  jet_moments_pass<F>(
+      vs, nvec, tup, ntup, n2, pts, partials,
+      [&](const double* s_v, int4 q, int urow, int np, long long base) { return moment_tile<KIND, 2>(op, s_v, q, urow, np, base, pts); },
+      [&](const double* s_v, int4 q, int urow, int np, long long base) { return moment_tile<KIND, 3>(op, s_v, q, urow, np, base, pts); });
 }
 // out[t] = the sum of the G partials of tuple t, in CTA order
 static __global__ void __launch_bounds__(256) k_jet_moments_fold(const double* __restrict__ partials, int ntup, int G,
@@ -387,6 +397,210 @@ static __global__ void __launch_bounds__(256) k_jet_moments_fold(const double* _
     for (int b = 0; b < G; ++b) s += partials[(size_t)b * ntup + t];
     out[t] = s;
   }
+}
+
+// ------------------------------------------------------------------------------------------ reaction-diffusion (BK_RD)
+// F_i(u) = D_i Lap u_i + R_i(u), R_i = sum of the terms c_t prod_j u_j^a_tj with eq_t = i (bk200.h), over the table of effective
+// coefficients of bk_set_params (RdTable, by value: each context launches with its own).  One thread per grid point evaluates
+// every field there: the 2 ND stencil neighbours per field, then the terms in table order.  Exponents are run-time values, so
+// powers are bounded unrolled multiplications and a term reaches its equation by a select over the F fields: nothing indexes a
+// per-thread array at run time, and the values of a point stay in registers.
+__device__ __forceinline__ int rd_exp(int alpha, int j) { return (alpha >> (3 * j)) & 7; }
+// x^e for a run-time e <= BK_RD_MAX_DEGREE; 1 for e <= 0
+__device__ __forceinline__ double rd_pow(double x, int e) {
+  double r = 1.0;
+#pragma unroll
+  for (int k = 0; k < BK_RD_MAX_DEGREE; ++k) r = k < e ? r * x : r;
+  return r;
+}
+// acc[e] += x for the run-time field index e < F
+template <int F>
+__device__ __forceinline__ void rd_add(double (&acc)[F], int e, double x) {
+#pragma unroll
+  for (int f = 0; f < F; ++f)
+    if (e == f) acc[f] += x;
+}
+// the gradient of the monomial alpha at u: g_k = a_k u_k^(a_k - 1) prod_{j != k} u_j^a_j
+template <int F>
+__device__ __forceinline__ void rd_grad(int alpha, const double (&u)[F], double (&g)[F]) {
+  double pw[F], pd[F];
+#pragma unroll
+  for (int j = 0; j < F; ++j) {
+    const int a = rd_exp(alpha, j);
+    const double p = rd_pow(u[j], a - 1);
+    pd[j] = a * p;
+    pw[j] = a > 0 ? p * u[j] : 1.0;
+  }
+#pragma unroll
+  for (int k = 0; k < F; ++k) {
+    double t = pd[k];
+#pragma unroll
+    for (int j = 0; j < F; ++j)
+      if (j != k) t *= pw[j];
+    g[k] = t;
+  }
+}
+// The Laplacian of the field at v (unscaled) at point g = i + j nx: Neumann = clamp-to-edge ghost cells, Dirichlet = zero ghosts
+template <int ND>
+__device__ __forceinline__ double rd_lap(const double* __restrict__ v, long long g, int i, int j, int nx, int ny, double cx,
+                                         double cy, bool dirichlet) {
+  const double c = v[g], ghost = dirichlet ? 0.0 : c;
+  const double xm = i > 0 ? v[g - 1] : ghost, xp = i < nx - 1 ? v[g + 1] : ghost;
+  if constexpr (ND == 2) {
+    const double ym = j > 0 ? v[g - nx] : ghost, yp = j < ny - 1 ? v[g + nx] : ghost;
+    return cx * (xm - 2.0 * c + xp) + cy * (ym - 2.0 * c + yp);
+  }
+  return cx * (xm - 2.0 * c + xp);
+}
+// MODE 1: out = F(s v).  MODE 0: out = a0 s v + a1 J s v.  MODE 2: out = a0 s v + a1 J' s v (J' = the symmetric Laplacian plus
+// the transposed F x F reaction block).  s = *sp (1 when sp is NULL).
+template <int F, int ND, int MODE>
+static __global__ void __launch_bounds__(256) k_rd_apply(OpDesc op, const __grid_constant__ RdTable tb, const double* __restrict__ in,
+                                                         const double* __restrict__ sp, double* __restrict__ out) {
+  const int nx = op.nx, ny = ND == 2 ? op.ny : 1;
+  const long long n = (long long)nx * ny;
+  const double s = sp ? __ldg(sp) : 1.0;
+  const bool dir = tb.bc == BK_BC_DIRICHLET;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < n; g += (long long)gridDim.x * blockDim.x) {
+    const int i = ND == 2 ? (int)(g % nx) : (int)g, j = ND == 2 ? (int)(g / nx) : 0;
+    double v[F], u[F], r[F];
+#pragma unroll
+    for (int f = 0; f < F; ++f) {
+      v[f] = s * in[g + f * n];
+      r[f] = tb.diff[f] * (s * rd_lap<ND>(in + f * n, g, i, j, nx, ny, op.cx, op.cy, dir));
+      if (MODE != 1) u[f] = op.u[g + f * n];
+    }
+    for (int t = 0; t < tb.nterms; ++t) {
+      const int alpha = tb.alpha[t], e = tb.eq[t];
+      const double c = tb.coef[t];
+      if constexpr (MODE == 1) {
+        double m = c;
+#pragma unroll
+        for (int k = 0; k < F; ++k) m *= rd_pow(v[k], rd_exp(alpha, k));
+        rd_add(r, e, m);
+      } else {
+        double gr[F];
+        rd_grad(alpha, u, gr);
+        if constexpr (MODE == 0) {
+          double d = 0.0;
+#pragma unroll
+          for (int k = 0; k < F; ++k) d = fma(gr[k], v[k], d);
+          rd_add(r, e, c * d);
+        } else {
+          double we = 0.0;
+#pragma unroll
+          for (int f = 0; f < F; ++f) we = e == f ? v[f] : we;
+#pragma unroll
+          for (int k = 0; k < F; ++k) r[k] += c * gr[k] * we;
+        }
+      }
+    }
+#pragma unroll
+    for (int f = 0; f < F; ++f) out[g + f * n] = MODE == 1 ? r[f] : op.a0 * v[f] + op.a1 * r[f];
+  }
+}
+// The RD point form of the jets: o = d2F(u)[a, b] (ORDER 2) or d3F(u)[a, b, c] (ORDER 3) at one point; the Laplacian drops out.
+// Each monomial is expanded as a product of its factors (u_j + s a_j + t b_j + r c_j)^a_j, truncated to the multilinear terms in
+// the ORDER directions: component S (a subset of the directions, as a bit mask) of a factor is a_j^(|S|) u_j^(a_j - |S|) times
+// the product of the directions in S (x^(k) the falling factorial), and the full component of the product is the jet.
+template <int F, int ORDER>
+__device__ __forceinline__ void rd_jet(const RdTable& tb, const double (&u)[F], const double (&a)[F], const double (&b)[F],
+                                       const double (&c)[F], double (&o)[F]) {
+  constexpr int NS = 1 << ORDER;
+#pragma unroll
+  for (int f = 0; f < F; ++f) o[f] = 0.0;
+  for (int t = 0; t < tb.nterms; ++t) {
+    const int alpha = tb.alpha[t];
+    double m[NS];
+#pragma unroll
+    for (int S = 0; S < NS; ++S) m[S] = S == 0 ? 1.0 : 0.0;
+#pragma unroll
+    for (int j = 0; j < F; ++j) {
+      const int ae = rd_exp(alpha, j);
+      double pk[ORDER + 1];  // a^(k) u^(a - k)
+#pragma unroll
+      for (int k = 0; k <= ORDER; ++k) {
+        double ff = 1.0;
+#pragma unroll
+        for (int q = 0; q < k; ++q) ff *= (double)(ae - q);
+        pk[k] = ff * rd_pow(u[j], ae - k);
+      }
+      double fac[NS];
+#pragma unroll
+      for (int S = 0; S < NS; ++S) {
+        double x = pk[__builtin_popcount(S)];
+        if (S & 1) x *= a[j];
+        if (S & 2) x *= b[j];
+        if (S & 4) x *= c[j];
+        fac[S] = x;
+      }
+      double p[NS];
+#pragma unroll
+      for (int S = 0; S < NS; ++S) {
+        double acc = 0.0;
+#pragma unroll
+        for (int T = 0; T < NS; ++T)
+          if ((T & S) == T) acc = fma(m[T], fac[S & ~T], acc);
+        p[S] = acc;
+      }
+#pragma unroll
+      for (int S = 0; S < NS; ++S) m[S] = p[S];
+    }
+    rd_add(o, tb.eq[t], tb.coef[t] * m[NS - 1]);
+  }
+}
+template <int F, int ORDER>
+static __global__ void __launch_bounds__(256) k_rd_jet(const __grid_constant__ RdTable tb, const double* u, const double* a,
+                                                       const double* b, const double* c, double* out, long long n) {
+  bk_pdl_sync();
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < n; g += (long long)gridDim.x * blockDim.x) {
+    double uu[F], aa[F], bb[F], cc[F], o[F];
+#pragma unroll
+    for (int f = 0; f < F; ++f) {
+      uu[f] = u[g + f * n];
+      aa[f] = a[g + f * n];
+      bb[f] = b[g + f * n];
+      cc[f] = ORDER == 3 ? c[g + f * n] : 0.0;
+    }
+    rd_jet<F, ORDER>(tb, uu, aa, bb, cc, o);
+#pragma unroll
+    for (int f = 0; f < F; ++f) out[g + f * n] = o[f];
+  }
+}
+// k_jet_moments for BK_RD: the same pass and fold, with rd_jet as the point form
+template <int F, int ORDER>
+__device__ __forceinline__ double rd_moment_tile(const RdTable& tb, const double* __restrict__ s_v, int4 q, int urow, int np) {
+  constexpr int LD = BK_MOM_TP + 1;
+  const double* vi = s_v + q.x * F * LD;
+  const double* va = s_v + q.y * F * LD;
+  const double* vb = s_v + q.z * F * LD;
+  const double* vc = s_v + (ORDER == 3 ? q.w : q.z) * F * LD;
+  const double* uu = s_v + urow * LD;
+  double s = 0.0;
+  for (int p = 0; p < np; ++p) {
+    double u[F], a[F], b[F], c[F], o[F];
+#pragma unroll
+    for (int f = 0; f < F; ++f) {
+      u[f] = uu[p + f * LD];
+      a[f] = va[p + f * LD];
+      b[f] = vb[p + f * LD];
+      c[f] = vc[p + f * LD];
+    }
+    rd_jet<F, ORDER>(tb, u, a, b, c, o);
+#pragma unroll
+    for (int f = 0; f < F; ++f) s = fma(vi[p + f * LD], o[f], s);
+  }
+  return s;
+}
+template <int F>
+static __global__ void __launch_bounds__(256) k_rd_jet_moments(const __grid_constant__ RdTable tb, MomVecs vs, int nvec,
+                                                               const int4* __restrict__ tup, int ntup, int n2, long long pts,
+                                                               double* __restrict__ partials) {
+  bk_pdl_sync();
+  jet_moments_pass<F>(
+      vs, nvec, tup, ntup, n2, pts, partials,
+      [&](const double* s_v, int4 q, int urow, int np, long long) { return rd_moment_tile<F, 2>(tb, s_v, q, urow, np); },
+      [&](const double* s_v, int4 q, int urow, int np, long long) { return rd_moment_tile<F, 3>(tb, s_v, q, urow, np); });
 }
 
 // ------------------------------------------------------------------------------------------ deflation moments
@@ -656,9 +870,24 @@ static int launch_k2_apply(bk_ctx* c, const OpDesc& op, const double* in, const 
   return bk_launch_ordered(c, k2_apply<E, MODE>, grid, BK2_THREADS, Sh2Scratch<E>::BYTES, op, in, sp, out);
 }
 
+// The RD kernel of the context's fields and dimensions, as a function pointer out of a table
+#define BK_RD_BY_FIELDS(K, ...) {K<1, __VA_ARGS__>, K<2, __VA_ARGS__>, K<3, __VA_ARGS__>, K<4, __VA_ARGS__>}
+template <int MODE>
+static int launch_rd(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* out) {
+  // residual at the context's params, JVP / J' at the Jacobian's (bk_jac_set_state)
+  const int mode = MODE == 1 ? 1 : op.transpose ? 2 : 0;
+  static decltype(&k_rd_apply<1, 1, 0>) const kern[2][3][4] = {
+      {BK_RD_BY_FIELDS(k_rd_apply, 1, 0), BK_RD_BY_FIELDS(k_rd_apply, 1, 1), BK_RD_BY_FIELDS(k_rd_apply, 1, 2)},
+      {BK_RD_BY_FIELDS(k_rd_apply, 2, 0), BK_RD_BY_FIELDS(k_rd_apply, 2, 1), BK_RD_BY_FIELDS(k_rd_apply, 2, 2)}};
+  const BkKindTraits* kt = bk_traits(c);
+  return bk_launch_ordered(c, kern[kt->ndims - 1][mode][kt->fields - 1], bk_lin_grid(c, (long long)op.nx * op.ny), 256, 0, op,
+                           MODE == 1 ? c->rd_par : c->rd_jpar, in, sp, out);
+}
+
 template <int MODE>
 static int launch_kind(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* out) {
   switch (op.kind) {
+    case BK_RD: return launch_rd<MODE>(c, op, in, sp, out);
     case BK_SH2D:
       if ((op.nx % 2 == 0) && ((((uintptr_t)in) & 15) == 0)) return launch_k2_apply<BK2_EMAX, MODE>(c, op, in, sp, out);
       return bk_launch_ordered(c, k_sh_apply<2, MODE>, sh_num_tiles<2>(op.nx, op.ny, 1), BK_THREADS, ShSmem<2>::BYTES, op, in,
@@ -700,7 +929,7 @@ static __global__ void __launch_bounds__(256) k_cshift(double* __restrict__ out,
 }
 
 int bk_launch_apply(bk_ctx* c, const OpDesc& op, const double* in, const double* sp, double* out) {
-  if (op.transpose) BK_CHECK(c, bk_kind_traits(op.kind)->has_jt, "J' is not available for this problem kind");
+  if (op.transpose) BK_CHECK(c, bk_traits(c)->has_jt, "J' is not available for this problem kind");
   if (op.cplx) {
     // ((a0 + i a0i) I + a1 J)(x + i y): the real operator on both halves, then the cross terms of the imaginary shift
     OpDesc half = op;
@@ -743,6 +972,7 @@ extern "C" int32_t bk_jac_set_state(bk_ctx* c, const double* u) {
   BK_CUDA(c, cudaMemcpyAsync(c->u_state, u, 8 * (size_t)c->N0, kind, c->stream));
   if (kind == cudaMemcpyHostToDevice) c->stats.h2d_bytes += 8 * c->N0;
   for (int i = 0; i < BK_MAX_PAR; ++i) c->jpar[i] = c->par[i];
+  c->rd_jpar = c->rd_par;
   c->have_state = true;
   return bk_potrap_refresh_cache(c);
 }
@@ -756,7 +986,7 @@ extern "C" int32_t bk_jac_set_shift_imag(bk_ctx* c, double a0_imag) {
 
 extern "C" int32_t bk_jac_set_transpose(bk_ctx* c, int32_t on) {
   BK_ENTER(c);
-  BK_CHECK(c, !on || bk_kind_traits(c->kind)->has_jt, "J' is not available for this problem kind");
+  BK_CHECK(c, !on || bk_traits(c)->has_jt, "J' is not available for this problem kind");
   c->transpose = on != 0;
   return BK_OK;
 }
@@ -775,11 +1005,11 @@ extern "C" int32_t bk_jvp(bk_ctx* c, const double* v, double* out, double a0, do
 }
 
 // The checks bk_d2f, bk_d3f and bk_jet_moments share, then the jet form (jet_form) of the context's kind in *kind: BK_CHAN,
-// BK_CGL2D, or BK_SH2D for the three SH kinds
+// BK_CGL2D, BK_SH2D for the three SH kinds, or BK_RD (rd_jet)
 static int jet_kind(bk_ctx* c, int* kind) {
-  BK_CHECK(c, bk_kind_traits(c->kind)->has_jets, "d2F / d3F are not available for this problem kind");
+  BK_CHECK(c, bk_traits(c)->has_jets, "d2F / d3F are not available for this problem kind");
   BK_CHECK(c, !c->cplx, "d2F / d3F act on real states: not available in a BK_COMPLEX context");
-  *kind = c->kind == BK_CHAN || c->kind == BK_CGL2D ? c->kind : BK_SH2D;
+  *kind = c->kind == BK_CHAN || c->kind == BK_CGL2D || c->kind == BK_RD ? c->kind : BK_SH2D;
   return BK_OK;
 }
 
@@ -796,7 +1026,13 @@ static int jet(bk_ctx* c, const double* u, const double* dx1, const double* dx2,
   BK_TRY(bk_stage_in(c, out, n, 1, false, &dout));
   OpDesc op = bk_make_residual_op(c);
   op.kind = kind;  // k_jet branches on the jet form
-  const long long pts = n / bk_kind_traits(c->kind)->fields;
+  const int fields = bk_traits(c)->fields;
+  const long long pts = n / fields;
+  if (kind == BK_RD) {
+    static decltype(&k_rd_jet<1, 2>) const kern[2][4] = {BK_RD_BY_FIELDS(k_rd_jet, 2), BK_RD_BY_FIELDS(k_rd_jet, 3)};
+    BK_TRY(bk_launch(c, kern[dx3 ? 1 : 0][fields - 1], bk_lin_grid(c, pts), 256, 0, c->rd_par, du, d1, d2, d3, dout, pts));
+    return bk_stage_out(c, out, n, dout);
+  }
   if (dx3) BK_TRY(bk_launch(c, k_jet<3>, bk_lin_grid(c, pts), 256, 0, op, du, d1, d2, d3, dout, pts));
   else BK_TRY(bk_launch(c, k_jet<2>, bk_lin_grid(c, pts), 256, 0, op, du, d1, d2, d3, dout, pts));
   return bk_stage_out(c, out, n, dout);
@@ -884,7 +1120,7 @@ extern "C" int32_t bk_jet_moments(bk_ctx* c, const double* u, int32_t nvec, cons
     tup[t] = make_int4(q[0], q[1], q[2], k == 4 ? q[3] : 0);
   }
   if (ntup == 0) return BK_OK;
-  const long long n = c->N0, fields = bk_kind_traits(c->kind)->fields, pts = n / fields;
+  const long long n = c->N0, fields = bk_traits(c)->fields, pts = n / fields;
   MomVecs vs = {};  // the nvec vectors, then u
   const double* src[BK_JET_MOMENTS_MAX_VEC + 1];
   std::copy(vecs, vecs + nvec, src);
@@ -898,8 +1134,15 @@ extern "C" int32_t bk_jet_moments(bk_ctx* c, const double* u, int32_t nvec, cons
   c->stats.h2d_bytes += tup_bytes;
   const OpDesc op = bk_make_residual_op(c);
   const size_t smem = 8 * ((size_t)(nvec + 1) * fields * (BK_MOM_TP + 1) + ntup);
-  const auto kern = kind == BK_CGL2D ? k_jet_moments<BK_CGL2D> : kind == BK_CHAN ? k_jet_moments<BK_CHAN> : k_jet_moments<BK_SH2D>;
-  BK_TRY(bk_launch(c, kern, G, 256, smem, op, vs, (int)nvec, (const int4*)c->mom_work, ntup, (int)n2, pts, dpart));
+  if (kind == BK_RD) {
+    static decltype(&k_rd_jet_moments<1>) const kern[4] = {k_rd_jet_moments<1>, k_rd_jet_moments<2>, k_rd_jet_moments<3>,
+                                                               k_rd_jet_moments<4>};
+    BK_TRY(bk_launch(c, kern[fields - 1], G, 256, smem, c->rd_par, vs, (int)nvec, (const int4*)c->mom_work, ntup, (int)n2, pts,
+                     dpart));
+  } else {
+    const auto kern = kind == BK_CGL2D ? k_jet_moments<BK_CGL2D> : kind == BK_CHAN ? k_jet_moments<BK_CHAN> : k_jet_moments<BK_SH2D>;
+    BK_TRY(bk_launch(c, kern, G, 256, smem, op, vs, (int)nvec, (const int4*)c->mom_work, ntup, (int)n2, pts, dpart));
+  }
   BK_TRY(bk_launch_ordered(c, k_jet_moments_fold, (ntup + 255) / 256, 256, 0, (const double*)dpart, ntup, G, dres));
   return moment_results(c, dres, ntup, out);
 }

@@ -12,16 +12,18 @@ LIB_PATH = os.path.join(_HERE, "libbk200.so")
 CSRC = os.path.join(_HERE, "csrc")
 
 BK_OK, BK_NOT_CONVERGED = 0, 1
-BK_CHAN, BK_SH2D, BK_SH3D, BK_CGL2D, BK_POTRAP_CGL2D, BK_SH2D_PERIODIC = 1, 2, 3, 4, 5, 6
+BK_CHAN, BK_SH2D, BK_SH3D, BK_CGL2D, BK_POTRAP_CGL2D, BK_SH2D_PERIODIC, BK_RD = 1, 2, 3, 4, 5, 6, 7
 BK_COMPLEX = 0x100  # OR-ed into the kind: complexified context, vectors [re; im]
-BK_PC_NONE, BK_PC_SH_DCT, BK_PC_CHAN_TRIDIAG, BK_PC_CGL_DST, BK_PC_POTRAP_CIRC, BK_PC_SH_FFT = 0, 1, 2, 3, 4, 5
+BK_PC_NONE, BK_PC_SH_DCT, BK_PC_CHAN_TRIDIAG, BK_PC_CGL_DST, BK_PC_POTRAP_CIRC, BK_PC_SH_FFT, BK_PC_RD = 0, 1, 2, 3, 4, 5, 6
 BK_SIDE_NONE, BK_SIDE_LEFT, BK_SIDE_RIGHT = 0, 1, 2
 BK_ORTH_CGS, BK_ORTH_CGS2 = 0, 1
 BK_JET_MOMENTS_MAX_VEC, BK_JET_MOMENTS_MAX_TUPLES = 64, 8192   # the caps of bk_jet_moments (include/bk200.h)
 BK_DEFLATION_MAX_ROOTS = 64   # the cap of bk_deflation_moments
+BK_RD_MAX_FIELDS, BK_RD_MAX_PAR, BK_RD_MAX_TERMS = 4, 8, 64   # the bounds of a bk_rd_model
+BK_BC_NEUMANN, BK_BC_DIRICHLET = 0, 1
 
 SYMBOLS = [
-    "bk_ctx_create", "bk_ctx_destroy", "bk_last_error", "bk_problem_size", "bk_state_size", "bk_set_params", "bk_get_stats",
+    "bk_ctx_create", "bk_rd_ctx_create", "bk_ctx_destroy", "bk_last_error", "bk_problem_size", "bk_state_size", "bk_set_params", "bk_get_stats",
     "bk_set_timing", "bk_sync", "bk_stream",
     "bk_vec_alloc", "bk_vec_free", "bk_host_alloc", "bk_host_free", "bk_vec_upload", "bk_vec_download", "bk_vec_copy", "bk_vec_zero", "bk_vec_scale",
     "bk_vec_axpby", "bk_vec_dot", "bk_vec_norm2", "bk_vec_norminf", "bk_vec_diffdot",
@@ -35,6 +37,18 @@ SYMBOLS = [
 class GmresOpts(C.Structure):
     _fields_ = [("reltol", C.c_double), ("abstol", C.c_double), ("restart", C.c_int32), ("maxiter", C.c_int32),
                 ("pc_side", C.c_int32), ("orth", C.c_int32), ("fused", C.c_int32), ("reserved", C.c_int32)]
+
+
+class RdTerm(C.Structure):
+    """bk_rd_term (include/bk200.h)"""
+    _fields_ = [("scale", C.c_double), ("eq", C.c_int32), ("pexp", C.c_int32 * BK_RD_MAX_PAR), ("fexp", C.c_int32 * BK_RD_MAX_FIELDS)]
+
+
+class RdModel(C.Structure):
+    """bk_rd_model"""
+    _fields_ = [(k, C.c_int32) for k in ("fields", "ndims", "bc", "nparams", "flags", "nterms")] + \
+               [("diff_scale", C.c_double * BK_RD_MAX_FIELDS), ("diff_pexp", (C.c_int32 * BK_RD_MAX_PAR) * BK_RD_MAX_FIELDS),
+                ("terms", C.POINTER(RdTerm))]
 
 
 class Stats(C.Structure):
@@ -91,6 +105,7 @@ def load():
     i32, i64, dbl = C.c_int32, C.c_int64, C.c_double
     sig = {
         "bk_ctx_create": [i32, i32, C.POINTER(i64), dp, i32, C.POINTER(C.c_void_p)],
+        "bk_rd_ctx_create": [i32, C.POINTER(RdModel), C.POINTER(i64), dp, i32, C.POINTER(C.c_void_p)],
         "bk_ctx_destroy": [C.c_void_p],
         "bk_problem_size": [C.c_void_p],
         "bk_state_size": [C.c_void_p],

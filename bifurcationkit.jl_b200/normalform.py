@@ -39,7 +39,7 @@ import numpy as np
 import scipy.linalg as sla
 
 from .codim2 import _apply, ComplexProblemB200
-from .core import Context, DeviceVec, ComplexGMRESB200, ShiftInvertB200, MatrixFreeBLSB200
+from .core import Context, DeviceVec, ComplexGMRESB200, MatrixFreeBLSB200, eigsolve
 from .deflation import DeflationOperator, newton_deflated_or_fail
 from .palc import V, ContIterable, NewtonPar, re_make
 from . import events
@@ -75,7 +75,7 @@ def _given(x, z):
 
 def _eig(eigsolver, J, nev):
     """eigsolver(J, nev) with eigenvectors: (vals, vecs as columns)"""
-    out = eigsolver(J, nev, want_vectors=True) if isinstance(eigsolver, ShiftInvertB200) else eigsolver(J, nev)
+    out = eigsolve(eigsolver, J, nev, True)
     return np.asarray(out[0]), out[1]
 
 
@@ -310,7 +310,7 @@ def d3Fc(prob, x0, p, a, b, c):
 def _complex_twin(prob):
     """ComplexProblemB200 and ComplexGMRESB200 on a BK_COMPLEX context of the device problem's grid (codim2.py)"""
     ctx = prob.ctx
-    cctx = Context(ctx.kind, ctx.dims, ctx.lengths, krylov_m=ctx.krylov_m, params=ctx.params, complex=True)
+    cctx = Context(**{**ctx._args, "complex": True}, params=ctx.params)
     return ComplexProblemB200(cctx, prob.params, prob.lens)
 
 

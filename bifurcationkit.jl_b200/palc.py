@@ -18,7 +18,7 @@ import numpy as np
 
 from scipy.linalg import blas as _blas
 
-from .core import DeviceVec
+from .core import DeviceVec, eigsolve
 
 SQRT_EPS = math.sqrt(np.finfo(np.float64).eps)  # src/Problems.jl:69
 
@@ -221,9 +221,10 @@ class BifurcationProblemB200:
 
     @property
     def symmetric(self):
-        """is_symmetric(prob) (src/Problems.jl:126): J' = J for the Swift-Hohenberg kinds"""
+        """is_symmetric(prob) (src/Problems.jl:126): J' = J for the Swift-Hohenberg kinds and one-field reaction-diffusion models"""
         from . import lib as _l
-        return (self.ctx.kind & ~_l.BK_COMPLEX) in (_l.BK_SH2D, _l.BK_SH3D, _l.BK_SH2D_PERIODIC)
+        kind = self.ctx.kind & ~_l.BK_COMPLEX
+        return kind in (_l.BK_SH2D, _l.BK_SH3D, _l.BK_SH2D_PERIODIC) or (kind == _l.BK_RD and self.ctx.model.fields == 1)
 
 
 def re_make(prob, u0, p):
@@ -456,7 +457,7 @@ class ContIterable:
         eig = cp.newton_options.eigsolver
         if cp.detect_bifurcation <= 0 or eig is None:
             return
-        out = eig(self.prob.J(st.z_u, st.z_p), max(st.n_unstable[1] + 5, cp.nev))  # src/Utils.jl:78-79
+        out = eigsolve(eig, self.prob.J(st.z_u, st.z_p), max(st.n_unstable[1] + 5, cp.nev), cp.save_eigenvectors)  # src/Utils.jl:78-79
         vals = np.asarray(out[0])
         _, nu, ni = is_stable(cp, vals)
         st.n_unstable = (nu, st.n_unstable[0])

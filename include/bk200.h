@@ -47,6 +47,9 @@ enum {
    * the example's L is L1 + I).  Same layout and lengths as BK_SH2D: domain [-lx, lx), h = 2 lx / Nx.  Nx and Ny must be powers
    * of two from 64 to 2048 (BK_ERR_ARG otherwise).  Every operator application is three transform kernels (bk_fft_fast.cuh). */
   BK_SH2D_PERIODIC = 6,
+  /* reaction-diffusion system F_i(u) = D_i Lap u_i + R_i(u) with a polynomial R, described by a bk_rd_model: created only by
+   * bk_rd_ctx_create (bk_ctx_create refuses it).  dims (Nx) or (Nx, Ny), N = fields Nx Ny, field-major [u_1; ..; u_F] */
+  BK_RD = 7,
   /* OR-ed into one of the kinds above (not BK_POTRAP_CGL2D): a COMPLEXIFIED context for the complex shifts of the Hopf
    * minimally augmented system (src/codim2/MinAugHopf.jl:19-40, shift = Complex(0, -omega)) and complex eigenvector work.
    * Unknowns are z = x + i y stored split, [x; y]: bk_problem_size = 2 N0, with N0 = bk_state_size the size of the real
@@ -67,8 +70,10 @@ enum {
   BK_PC_POTRAP_CIRC = 4,/* Trapeze PO Jacobian of cGL linearised at the trivial state: DST-I in space (mixed-radix FFT of the odd extension, bk_fft_gen.cuh),
                            u1 +- i u2, DFT over the M-1 cyclic slices, scalar symbol; a0 = period T.  Stand-in for the ILU
                            of the assembled PO Jacobian (examples/cGL2d.jl:209-213) */
-  BK_PC_SH_FFT = 5      /* BK_SH2D_PERIODIC only: (L1 + a0 I)^-1 by real 2-D FFT, a0 > 0 (the symbol of L1 vanishes at |k| = 1); the
+  BK_PC_SH_FFT = 5,     /* BK_SH2D_PERIODIC only: (L1 + a0 I)^-1 by real 2-D FFT, a0 > 0 (the symbol of L1 vanishes at |k| = 1); the
                            example's L^-1 is a0 = 1 (examples/SH2d-fronts-cuda.jl:64,77-90) */
+  BK_PC_RD = 6          /* BK_RD only: per field (a0 I + a1 D_i Lap)^-1 by DCT-II (Neumann) or DST-I (Dirichlet) lines; refused when
+                           a symbol a0 + a1 D_i lambda vanishes (D_i at the params of the set-up) */
 };
 enum { BK_SIDE_NONE = 0, BK_SIDE_LEFT = 1, BK_SIDE_RIGHT = 2 };
 enum { BK_ORTH_CGS = 0, BK_ORTH_CGS2 = 1 };
@@ -111,6 +116,40 @@ typedef struct bk_stats {
 /* ---- context --------------------------------------------------------------------------- */
 int32_t bk_ctx_create(int32_t device, int32_t problem_kind, const int64_t dims[3], const double lengths[3],
                       int32_t krylov_m, bk_ctx** out);
+/* ---- BK_RD: reaction-diffusion models (examples/pd-1d.jl, examples/cGL2d.jl:6-22 and the Gray-Scott / Schnakenberg /
+ * Brusselator kinetics): F_i(u) = D_i Lap u_i + R_i(u), i < fields, with
+ *   D_i = diff_scale[i] prod_k p_k^diff_pexp[i][k],
+ *   R_i = sum over the terms t with eq = i of  scale_t prod_k p_k^pexp_t[k] prod_j u_j^fexp_t[j].
+ * Lap is the second-difference Laplacian with h = 2 l / N per dimension: Neumann = the clamp closure (diagonal -1/h^2 at the
+ * ends, examples/SH2d-fronts.jl:13-29, examples/pd-1d.jl), Dirichlet = zero ghost cells (diagonal -2/h^2, examples/cGL2d.jl:6-22).
+ * The parameter monomials are evaluated by bk_set_params; J, J' (the symmetric Laplacian and the transposed reaction block),
+ * d2F, d3F and bk_jet_moments are exact.  J is symmetric (the eigensolver's symmetric branch) when fields == 1.
+ * bk_rd_ctx_create refuses, with BK_ERR_ARG and a message before any device work, a model outside these ranges. */
+#define BK_RD_MAX_FIELDS 4
+#define BK_RD_MAX_PAR 8      /* the length of the parameter tuple of any context */
+#define BK_RD_MAX_TERMS 64
+#define BK_RD_MAX_PEXP 4     /* |parameter exponent| */
+#define BK_RD_MAX_DEGREE 5   /* field exponents are >= 0 and sum to at most this, per term */
+enum { BK_BC_NEUMANN = 0, BK_BC_DIRICHLET = 1 };
+typedef struct bk_rd_term {
+  double scale;
+  int32_t eq;                       /* the equation i < fields the term adds to */
+  int32_t pexp[BK_RD_MAX_PAR];      /* parameter exponents; 0 beyond nparams */
+  int32_t fexp[BK_RD_MAX_FIELDS];   /* field exponents; 0 beyond fields */
+} bk_rd_term;
+typedef struct bk_rd_model {
+  int32_t fields;   /* 1 .. BK_RD_MAX_FIELDS */
+  int32_t ndims;    /* 1 or 2 */
+  int32_t bc;       /* BK_BC_NEUMANN or BK_BC_DIRICHLET */
+  int32_t nparams;  /* 0 .. BK_RD_MAX_PAR: bk_set_params takes this many */
+  int32_t flags;    /* 0, or BK_COMPLEX for the complexified context of the model */
+  int32_t nterms;   /* 0 .. BK_RD_MAX_TERMS */
+  double diff_scale[BK_RD_MAX_FIELDS];
+  int32_t diff_pexp[BK_RD_MAX_FIELDS][BK_RD_MAX_PAR];
+  const bk_rd_term* terms;  /* nterms terms, copied at creation */
+} bk_rd_model;
+int32_t bk_rd_ctx_create(int32_t device, const bk_rd_model* model, const int64_t dims[3], const double lengths[3],
+                         int32_t krylov_m, bk_ctx** out);
 int32_t bk_ctx_destroy(bk_ctx* ctx);
 const char* bk_last_error(bk_ctx* ctx);
 int64_t bk_problem_size(bk_ctx* ctx);                       /* N = number of unknowns of F */
